@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """bench.py -- C-ViViT encode frames/s (headline, BASELINE.json configs[1]) + MaskGIT sample tokens/s.
 
-    python bench.py --gpus N --steps K --warmup W            # this framework (libphk.so, sm_100a)
+    python bench.py --gpus N --steps K --warmup W            # this framework (libphk.so, sm_90a)
+    python bench.py ... --dump-outputs DIR                   # + the last timed step's token ids as DIR/<name>.npy
     python bench.py --impl reference --gpus N ...            # the reference's CPU path (oracle port), rank 0
 
 A "step" is one pass of the hot path over one batch of synthetic input: one
@@ -45,7 +46,8 @@ def peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tf_burst=d["bf16_tflops"], tf_sustained=d["bf16_tflops_sustained"],
                     src="MEASURED_PEAKS.json")
-    return dict(hbm=6650.0, tf_burst=1590.0, tf_sustained=1400.0, src="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W): HBM3 3.35 TB/s, dense bf16 989 TFLOP/s -- not measured figures
+    return dict(hbm=3350.0, tf_burst=989.0, tf_sustained=989.0, src="fallback (H100 SXM data sheet)")
 
 
 class ClockSampler:
@@ -296,7 +298,7 @@ def run_reference(args, rank, world):
         "config": {"workload": "BASELINE.json configs[1]: CViViT(dim=512,image=256,patch=32,pt=2,depth=4+4,heads=8,"
                                "codebook=65536) encode+LFQ ids of (8,3,17,256,256) fp32 per GPU, random-init weights",
                    "batch_per_gpu": per_step, "frames": VIDEO[2],
-                   "note": "host CPU, oracle port of the reference modules (kind: port -- /root/reference is not on the "
+                   "note": "host CPU, oracle port of the reference modules (kind: port -- the reference package is not on the "
                            "GPU box), thread count auto-tuned"},
         "cpu_baseline": dict(value=fps, unit="frames/s", cores=cores, kind="port", sample=sample),
         "e2e": {"value": fps, "unit": "frames/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
@@ -502,7 +504,7 @@ def bench_make_video(dev, prec, world, barrier, sampler, chains_timed=3, b=2):
 
 
 def reference_gpu_leg(dev, maskgit=True):
-    """SURVEY 2a / 8d: the reference's own PyTorch path on this B200 (oracle port on CUDA, eager fp32 and autocast
+    """SURVEY 2a / 8d: the reference's own PyTorch path on this GPU (oracle port on CUDA, eager fp32 and autocast
     bf16) -- the same-box bar the build must beat."""
     sys.path.insert(0, os.path.join(ROOT, "tools"))
     import ref_gpu_bench as R
@@ -510,6 +512,15 @@ def reference_gpu_leg(dev, maskgit=True):
     if maskgit:
         out["maskgit"] = R.maskgit_leg(dev, iters=1)
     return out
+
+
+def dump_outputs(directory, **arrays):
+    """What the timed path returned in its last step, as float64 .npy files (token ids are exact in float64)."""
+    import numpy as np
+    import torch
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(directory, name + ".npy"), t.detach().cpu().to(torch.float64).numpy())
 
 
 def main():
@@ -524,6 +535,8 @@ def main():
     ap.add_argument("--no-refgpu", action="store_true")
     ap.add_argument("--no-train", action="store_true", help="skip the configs[3] training-step block")
     ap.add_argument("--no-makevideo", action="store_true", help="skip the configs[4] make_video block")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the token ids of the last timed step as DIR/<name>.npy (float64)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", 0))
     local = int(os.environ.get("LOCAL_RANK", 0))
@@ -554,7 +567,7 @@ def main():
     model = P.CViViT(**CFG2).to(dev).eval()
     model.precision = prec
     B, Cc, F, H, Wd = VIDEO
-    # three distinct input buffers (3 x 107 MB > 126 MB L2) so no timed step finds its video in L2
+    # three distinct input buffers (3 x 107 MB > 50 MB L2) so no timed step finds its video in L2
     host = [torch.randn(VIDEO, generator=torch.Generator().manual_seed(100 + rank * 10 + i)).pin_memory()
             for i in range(3)]
     vids = [h.to(dev, non_blocking=True) for h in host]
@@ -595,8 +608,10 @@ def main():
     ms_step = ms_total / K
     value = world * B * F * K / (ms_total / 1e3)
 
-    # the K-step window is tens of milliseconds (power and clocks have not settled): also a long run of the same loop
-    KS = 1500
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, cvivit_ids=ids)
+    # the K-step window is short (power and clocks have not settled): also a run of 20 times as many steps
+    KS = 20 * K
     e0.record()
     t_sus = time.perf_counter()
     for i in range(KS):
@@ -700,10 +715,10 @@ def main():
                                "codebook=65536) encode+LFQ ids of (8,3,17,256,256) fp32 per GPU, random-init weights",
                    "batch_per_gpu": B, "global_batch": B * world, "frames": F,
                    "parallelism": f"dp{world}: batch-sharded, one process per GPU, no data-path collective",
-                   "l2": "inputs rotate over 3 device buffers (3 x 107 MB > 126 MB L2)",
+                   "l2": "inputs rotate over 3 device buffers (3 x 107 MB > 50 MB L2)",
                    "precision_mode": {"f32": "PHK_PREC_F32 (fp32 FFMA GEMMs, parity mode)",
-                                      "bf16": "PHK_PREC_BF16 (tcgen05 bf16 GEMMs, fp32 accumulate/residual/LN/softmax)",
-                                      "bf16x3": "PHK_PREC_BF16X3 (tcgen05, split-bf16 operands: fp32-grade products)"}[args.prec]},
+                                      "bf16": "PHK_PREC_BF16 (wgmma bf16 GEMMs, fp32 accumulate/residual/LN/softmax)",
+                                      "bf16x3": "PHK_PREC_BF16X3 (wgmma, split-bf16 operands: fp32-grade products)"}[args.prec]},
         "e2e": {"value": e2e_value, "unit": "frames/s", "h2d_bytes_per_step": B * Cc * F * H * Wd * 4,
                 "d2h_bytes_per_step": B * tp * hh * ww * 8, "steps": KE,
                 "api": "CViViT.encode_host_iter -> phk_encode_pipe_submit/wait (C ABI; pinned host video -> host int64 "

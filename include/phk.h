@@ -1,5 +1,5 @@
 /*
- * phk.h -- C ABI of the B200-native phenaki hot path (libphk.so).
+ * phk.h -- C ABI of the H100-native phenaki hot path (libphk.so).
  *
  * The reference (lucidrains/phenaki-pytorch @ 9415d4e) has no FFI: the path sits behind
  * torch.nn.Module classes (phenaki_pytorch/__init__.py:1-4).  This header is the boundary a
@@ -16,11 +16,11 @@
  *     except the *_host entry points which copy from/to host memory and synchronise.
  *   - residual stream / LayerNorm / softmax are fp32.  `prec` selects the contraction type:
  *     PHK_PREC_F32  fp32 FFMA GEMMs (parity mode, token ids identical to the fp32 reference);
- *     PHK_PREC_BF16 bf16 operands on tcgen05 tensor cores with fp32 TMEM accumulation (the
+ *     PHK_PREC_BF16 bf16 operands on wgmma tensor cores with fp32 accumulation (the
  *                   dtype flow of the reference under torch.autocast(bfloat16), SURVEY H2).
  *     PHK_PREC_BF16X3 fp32-grade products ON the tensor cores: every nn.Linear operand is split into two bf16 terms
- *                   (x = hi + lo, |x - hi - lo| <= 2^-17 |x|) and C = A_hi W_hi + A_hi W_lo + A_lo W_hi is ONE tcgen05
- *                   GEMM over the concatenated K' = 3K ([hi | hi | lo] x [hi | lo | hi], fp32 TMEM accumulation);
+ *                   (x = hi + lo, |x - hi - lo| <= 2^-17 |x|) and C = A_hi W_hi + A_hi W_lo + A_lo W_hi is ONE wgmma
+ *                   GEMM over the concatenated K' = 3K ([hi | hi | lo] x [hi | lo | hi], fp32 accumulation);
  *                   everything else (LayerNorm, attention core, GEGLU, PEG, fp32 activations) is the parity mode's.
  *                   Token ids equal the fp32 reference's at the bars of tests/test_gpu_parity_at_size.py without
  *                   the FFMA GEMMs' cost.  Inference only (the training step treats it as PHK_PREC_F32).
@@ -179,7 +179,7 @@ int phk_gemm_f32(const float* A, int64_t lda, const float* W, int64_t ldw, float
                  int64_t M, int32_t N, int32_t K, const float* bias, const float* residual,
                  int64_t seg_len, int64_t seg_stride, int64_t seg_off, phk_stream_t s);
 
-/* Same contract on tcgen05 tensor cores: A,W bf16 (K-major, lda/ldw multiples of 8), fp32 TMEM
+/* Same contract on wgmma tensor cores: A,W bf16 (K-major, lda/ldw multiples of 8), fp32
  * accumulators, TMA-fed, warp-specialised.  epilogue: 0 store fp32 (+bias,+residual),
  * 1 store bf16 (+bias), 2 GEGLU on val/gate-interleaved W rows -> bf16 [M, N/2]. */
 int phk_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc,
@@ -218,7 +218,7 @@ int phk_gemm_bf16_ln(const void* A, int64_t lda, const void* W, int64_t ldw, flo
  *   stat_ws : PHK_LN_STAT_BYTES bytes of device scratch, 16-byte aligned, any content;
  *   counters: PHK_LN_COUNTERS zero-initialised 32-bit device words, consumed by the call (left non-zero) -- give every
  *             call of a stream-ordered sequence its own words and clear them together once per sequence. */
-#define PHK_LN_STAT_BYTES (2 * 148 * 128 * 8)
+#define PHK_LN_STAT_BYTES (2 * 132 * 128 * 8)
 #define PHK_LN_COUNTERS 160
 int phk_gemm_bf16_ln_ws(const void* A, int64_t lda, const void* W, int64_t ldw, float* C, int64_t ldc, int64_t M,
                         int32_t N, int32_t K, const float* bias, const float* ln_g, const float* ln_b, float ln_eps,
@@ -232,16 +232,15 @@ int phk_split3(const float* x, int64_t ld, void* out, int64_t rows, int32_t K, i
 
 /* debug aid: per-CTA clock64 phase stamps of phk_gemm_bf16 (16 x int64 per CTA); NULL disables */
 int phk_debug_gemm_trace(long long* device_buffer);
-/* tests / A-B measurements: force the tcgen05 GEMM variant: 0 automatic, 1 one CTA per 128x128 tile, 2 CTA pairs
- * (cta_group::2) with 256x128 tiles, 3 CTA pairs with 256x256 tiles (2 and 3 apply when M > 128); < 0 restores the
- * PHK_GEMM_MODE environment default. */
+/* tests: GEMM variant selector, kept for ABI compatibility: modes <= 3 are accepted and every mode runs the one
+ * 128x128-tile wgmma kernel (the CTA-pair variants of modes 2 and 3 need an MMA Hopper does not have). */
 int phk_debug_gemm_mode(int32_t mode);
 /* tests / A-B measurements: declare (1) or withdraw (0), for the calling thread, that the W operands of the following
  * phk_gemm_bf16* calls are not written by earlier kernels of the stream -- the kernel then requests their first tiles before
  * its programmatic-dependent-launch wait.  The forward drivers (phk_cvivit_*, phk_maskgit_*) set this themselves. */
 int phk_debug_static_weights(int32_t on);
-/* tests / A-B measurements: phk_attention_tc* variant -- 0 probabilities through a shared-memory tile (two CTAs per SM),
- * 1 probabilities in tensor memory as the TMEM A operand of P.V (three CTAs per SM); < 0 restores the default. */
+/* tests: phk_attention_tc* variant selector, kept for ABI compatibility: values <= 1 are accepted and one kernel serves
+ * all of them (probabilities stay in registers as the A operand of P.V). */
 int phk_debug_attention_tc_variant(int32_t variant);
 
 /* GEGLU (attention.py:40-43): out[r, j] = gelu_erf(h[r, inner + j]) * h[r, j] */
@@ -271,8 +270,8 @@ int phk_attention(const float* q, const float* kv, const float* null_kv, const f
                   const float* k_scale, const float* bias, const uint8_t* key_mask,
                   const float* alibi_slopes, void* out, const phk_attn_geom_t* g, phk_stream_t s);
 
-/* Tensor-core (tcgen05) attention core for self-attention sequences of n >= 64 tokens, dim_head 64, no null-kv / key
- * mask / causal (those take phk_attention): S = QK^T and O = PV on tcgen05, S and P never leave the SM.
+/* Tensor-core (wgmma) attention core for self-attention sequences of n >= 64 tokens, dim_head 64, no null-kv / key
+ * mask / causal (those take phk_attention): S = QK^T and O = PV on wgmma, S and P never leave the SM.
  * phk_attention_tc_bf16: operands as phk_gemm_bf16_qkv writes them -- Qn bf16 [n_seq*n, ld_q], KVn bf16 [n_seq*n, ld_kv]
  *   (token-major; 4-D tensor maps pick one head's tile, V is an MN-major operand: no head-major or transposed copy);
  *   bias fp32 [heads, n, n] or NULL -> out bf16 [n_seq*n, heads*64].
@@ -324,7 +323,7 @@ int phk_layernorm_lfq(const float* x, const float* gamma, const float* beta, con
 /* Cosine-sim VectorQuantize ids (cvivit.py:321, :568-570 with lookup_free_quantization=False; oracle/lfq.py):
  * ids[r] = argmax_c l2norm(x[r]) . codebook[c] = argmax_c x[r] . codebook[c] (unit codebook rows), first maximum on ties.
  * PHK_PREC_F32: x fp32 [rows, dim], fp32 FFMA similarities strip by strip; PHK_PREC_BF16: x bf16 [rows, dim], the fused
- * tcgen05 head at temperature 0 (dim <= 512): the [rows, K] similarities are never stored. */
+ * wgmma head at temperature 0 (dim <= 512): the [rows, K] similarities are never stored. */
 int64_t phk_vq_cosine_scratch_bytes(int64_t rows, int32_t K, int32_t prec);
 int phk_vq_cosine_ids(const void* x, const float* codebook, const void* codebook_h, int64_t* ids, int64_t rows,
                       int32_t dim, int32_t K, void* scratch, int64_t scratch_bytes, int32_t prec, phk_stream_t s);
@@ -476,9 +475,9 @@ int phk_maskgit_forward(const phk_maskgit_t* m, const int64_t* ids, int32_t b, i
 int phk_layernorm_cfg(const float* x_cond, const float* x_null, const float* gamma, const float* beta,
                       float cond_scale, void* out_bf16, int64_t rows, int32_t dim, phk_stream_t s);
 
-/* Fused logits head for the sampling loop (phenaki_pytorch.py:213 + 83-93 + 506-509 + 547-550): a tcgen05 GEMM whose
+/* Fused logits head for the sampling loop (phenaki_pytorch.py:213 + 83-93 + 506-509 + 547-550): a wgmma GEMM whose
  * epilogue applies bias and gumbel noise (in-kernel Philox, same counter layout as phk_sample_tokens with u == NULL)
- * and reduces argmax / online softmax over the vocabulary straight out of TMEM, so the (b, n, V) logits never exist
+ * and reduces argmax / online softmax over the vocabulary straight out of the accumulator registers, so the (b, n, V) logits never exist
  * in memory.  emb bf16 [emb_rows >= n_tokens, dim <= 512] = guided embeddings (phk_layernorm_cfg, or plain norm_out
  * rows when there is no guidance); the 128-token A panel stays resident in shared memory, W streams through TMA.
  * Outputs as phk_sample_tokens. */
@@ -606,7 +605,7 @@ int phk_debug_step_graph(int32_t on);
  * The gradient-shrink trick (:199) scales the embedding gradients by shrink_alpha, as autograd does.  cond_drop_prob is
  * 0 in the reference's training forward (:594 overwrites the argument), so there is no text dropout.
  * prec: PHK_PREC_F32 = fp32 FFMA products (parity with the fp32 reference); PHK_PREC_BF16 = the forward, dgrad and
- * wgrad product of every nn.Linear on the tcgen05 GEMM (phk_gemm_bf16) with operands converted on the fly from the
+ * wgrad product of every nn.Linear on the wgmma GEMM (phk_gemm_bf16) with operands converted on the fly from the
  * fp32 activations / master weights (the dtype flow of torch.autocast(bfloat16)); LayerNorm, softmax, GEGLU, the
  * attention core and all gradients of non-matrix parameters stay fp32 in both modes. */
 int64_t phk_maskgit_train_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L, int32_t bce_head,

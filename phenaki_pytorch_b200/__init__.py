@@ -1,4 +1,4 @@
-"""phenaki-pytorch hot path, B200-native (sm_100a).  Drop-in names of the reference package
+"""phenaki-pytorch hot path, H100-native (sm_90a).  Drop-in names of the reference package
 (/root/reference/phenaki_pytorch/__init__.py:1-4) for the C-ViViT encode + MaskGIT sampling path."""
 from .cvivit import CViViT
 from .modules import invalidate_weights

@@ -9,14 +9,14 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PHK_LIB") or os.path.join(_HERE, "libphk.so")  # PHK_LIB: an A/B build of the same ABI (tools/ only)
 
 PREC_F32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
-LN_STAT_BYTES, LN_COUNTERS = 2 * 148 * 128 * 8, 160   # phk_gemm_bf16_ln_ws scratch (include/phk.h)
+LN_STAT_BYTES, LN_COUNTERS = 2 * 132 * 128 * 8, 160   # phk_gemm_bf16_ln_ws scratch (include/phk.h)
 
 
 def default_precision():
     """Precision mode new modules start in: `PHK_PREC` = f32 | bf16 | bf16x3 (unset: the module default below).
     f32    fp32 FFMA products -- the reference's fp32 arithmetic, token ids identical (slowest)
-    bf16x3 split-bf16 products on tcgen05 -- ids identical at the same bars, 4.3x faster than f32
-    bf16   bf16 products on tcgen05 -- the reference's autocast(bfloat16) dtype flow, 3x faster again (benchmarked mode)
+    bf16x3 split-bf16 products on wgmma -- ids identical at the same bars, 4.3x faster than f32
+    bf16   bf16 products on wgmma -- the reference's autocast(bfloat16) dtype flow, 3x faster again (benchmarked mode)
     `model.precision = _lib.PREC_*` switches a module at any time."""
     name = os.environ.get("PHK_PREC", DEFAULT_PRECISION_NAME).lower()
     return {"f32": PREC_F32, "fp32": PREC_F32, "bf16": PREC_BF16, "bf16x3": PREC_BF16X3}.get(name, PREC_BF16X3)

@@ -1,4 +1,4 @@
-"""Builds libphk.so (hand-written sm_100a CUDA + the C ABI of include/phk.h) in-tree with nvcc."""
+"""Builds libphk.so (hand-written sm_90a CUDA + the C ABI of include/phk.h) in-tree with nvcc."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libphk.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr", "-Xptxas", "-warn-spills"]
 
 
@@ -44,7 +44,7 @@ def build(force=False, verbose=False):
             failed = True
     if failed:
         raise RuntimeError("libphk build failed")
-    subprocess.check_call([NVCC, "-shared", "-o", LIB, *objs, "-lcudart", "-lcuda"])
+    subprocess.check_call([NVCC, *FLAGS[:2], "-shared", "-o", LIB, *objs, "-lcudart", "-lcuda"])
     return LIB
 
 

@@ -107,7 +107,7 @@ static inline bool known_prec(int prec) { return prec == PHK_PREC_F32 || prec ==
 
 // y = act @ W^T (+bias)(+residual) in the selected contraction type.  `act` is fp32 (parity / split-bf16 modes) or bf16.
 //   PHK_PREC_BF16X3: `act` fp32 is split into [hi | hi | lo] bf16 and multiplied with the [hi | lo | hi] weight pack
-//   (w16, ld 3 * Kp) by ONE tcgen05 GEMM over K' = 3 Kp: fp32-grade products on the tensor cores.
+//   (w16, ld 3 * Kp) by ONE wgmma GEMM over K' = 3 Kp: fp32-grade products on the tensor cores.
 static int linear(const Lin& ln, const void* act, int64_t lda, const float* w32, const void* w16, int64_t ldw, float* C,
                   int64_t ldc, int64_t M, int N, int K, const float* bias, const float* residual, phk_stream_t s) {
   if (ln.prec == PHK_PREC_BF16) {
@@ -129,14 +129,13 @@ static int linear(const Lin& ln, const void* act, int64_t lda, const float* w32,
 //   parity mode : every buffer fp32, FFMA GEMMs.
 //   bf16 mode   : residual stream / LayerNorm / softmax fp32; LayerNorm emits bf16 GEMM operands (plus the
 //                 un-normalised bf16 row for the self-attention k,v projection, attention.py:140-144); GEMMs on
-//                 tcgen05 with fp32 accumulation; FF first linear fused with GEGLU; attention output bf16.
+//                 wgmma with fp32 accumulation; FF first linear fused with GEGLU; attention output bf16.
 static int transformer_forward(const TfCall& c, Arena scratch, float* out, void* out_h, cudaStream_t st) {
   const phk_transformer_t* T = c.T;
   const bool h16 = c.prec == PHK_PREC_BF16;
-  // (StaticWeightsScope -- requesting the first weight tiles BEFORE the programmatic-dependent-launch wait -- measured
-  //  slower on the B200: 8.8 vs 7.6 us for the 4608x512x512 product, 14.3 vs 11.8 us at K = 1408,
-  //  profiles/r02/op_bench_c8.txt; griddepcontrol.wait appears to drain the thread's outstanding bulk copies first, so the
-  //  activation tiles are requested a full TMA latency later.  The hint stays available through phk_debug_static_weights.)
+  // (StaticWeightsScope -- requesting the first weight tiles BEFORE the programmatic-dependent-launch wait -- is not used
+  //  here: griddepcontrol.wait appears to drain the thread's outstanding bulk copies first, so the activation tiles would
+  //  be requested a full TMA latency later.  The hint stays available through phk_debug_static_weights.)
   PHK_REQUIRE(c.prec == PHK_PREC_F32 || c.prec == PHK_PREC_BF16X3 || h16, PHK_E_ARG, "transformer: unknown precision mode");
   PHK_REQUIRE(c.lin.prec == c.prec, PHK_E_ARG, "transformer: contraction descriptor not initialised");
   const int D = T->dim, H = T->heads, DH = T->dim_head, I = H * DH;
@@ -160,9 +159,8 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
   // bf16 mode, opt-in (PHK_FUSE_LN=1): the LayerNorm that follows a residual GEMM (out-projection -> cross-attention /
   // feed-forward norm, feed-forward -> the next layer's attention norm when no PEG sits in between) computed by that
   // GEMM's epilogue (phk_gemm_bf16_ln: row statistics summed over a cluster of N / 128 CTAs through distributed shared
-  // memory).  Correct (tests/test_gpu_fused_qkv.py) but NOT faster on the B200 at dim 512: a cluster of 4 full-SM CTAs
-  // needs 4 free SMs of one GPC, only ~32 such clusters are resident at once and the 36 row tiles of 4608 tokens take two
-  // waves -- 30.3 us against 12.2 us (GEMM) + 4.7 us (LayerNorm kernel), profiles/r02/encode_bf16_launches_c4_fuse_ln.txt.
+  // memory).  Correct (tests/test_gpu_fused_qkv.py); off by default because a cluster of 4 full-SM CTAs needs 4 free SMs
+  // of one GPC, so few clusters are resident at once and the row tiles of 4608 tokens take two waves.
   // PHK_FUSE_LN=2: the same fusion without clusters -- the CTAs of a row tile exchange the statistics through global
   // memory (phk_gemm_bf16_ln_ws; one set of arrival counters per fused launch, cleared together by one memset here).
   static const int fuse_ln_env = [] { const char* e = std::getenv("PHK_FUSE_LN"); return e && e[0] >= '0' && e[0] <= '2' ? e[0] - '0' : kFuseLnDefault; }();
@@ -253,8 +251,8 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
       // 16 < n <= 64 (the spatial transformer's 8 x 8 frames): warp-level MMAs, all (sequence, head) CTAs resident at once
       bool mid_ok = false;
 #ifndef PHK_CUDA_EMU
-      // (at exactly 64 tokens the tcgen05 kernel is faster -- 8.9 vs 11.6 us at 72 sequences x 8 heads,
-      //  profiles/r02/op_bench_c17.txt -- so the MMA kernel takes 17..63 tokens, which used to fall back to the fp32 kernel;
+      // (at exactly 64 tokens the wgmma kernel is used, so the MMA kernel takes 17..63 tokens, which used to fall back to
+      //  the fp32 kernel;
       //  PHK_MID_ATTN_MMA=1 forces it for 64 as well, =0 disables it)
       static const int mid_env = [] { const char* e = std::getenv("PHK_MID_ATTN_MMA"); return e ? (e[0] == '0' ? 0 : 2) : 1; }();
       mid_ok = mid_env != 0 && plain && !T->causal && c.seq.n_inner == 1 && c.seq.tok == 1 && c.seq.outer == c.seq.n_tok &&
@@ -281,7 +279,7 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
           PHK_TRY(linear(c.lin, xn, D, A.wq, A.wq_h, D, q, I, Rl, I, D, nullptr, nullptr, s));
           PHK_TRY(linear(c.lin, h16 ? xraw : (const void*)x, D, A.wkv, A.wkv_h, D, kv, 2 * I, Rl, 2 * I, D, nullptr, nullptr, s));
         }
-        if (tc_ok) {  // tcgen05 path from fp32 projections (PHK_FUSE_QKV=0): operands prepared by attention_prep_kernel
+        if (tc_ok) {  // wgmma path from fp32 projections (PHK_FUSE_QKV=0): operands prepared by attention_prep_kernel
           const int64_t ab = phk_attention_tc_scratch_bytes(n_outer, c.seq.n_tok, H);
           Arena tmp = scratch;
           void* asc = tmp.take(ab);

@@ -859,7 +859,7 @@ __global__ void __launch_bounds__(MMA_WARPS * 32) attention_small_mma_kernel(con
 // ------------------------------------------------------------------------------------------
 // Self-attention of short sequences (16 < n <= 64: the spatial transformer's 8 x 8 token frames) on the pre-normalised
 // token-major bf16 operands, warp-level MMAs: one CTA of four warps per (sequence, head), every warp owns 16 query rows.
-// The tcgen05 kernel (attention_tc_kernel) spends its life in prologue / barrier round trips at this size -- one 64-key
+// The wgmma kernel (attention_tc_kernel) spends its life in prologue / barrier round trips at this size -- one 64-key
 // chunk, half of its 128-row tile empty, 576 CTAs on 296 resident slots = two rounds (8.9 us at 72 x 64 x 8 heads);
 // here 576 CTAs of 128 threads and 27 KB are resident at once and a CTA is a 24 KB copy + 64 MMAs per warp.
 // Position bias fp32 [heads, n, n] or NULL; no masks, not causal (those take phk_attention).  [not on the CPU executor]

@@ -1,5 +1,5 @@
 // Tensor-core cosine-sim attention for long sequences (MaskGit self-attention, attention.py:146-181 with the 3-D
-// continuous position bias, n = T'H'W' = 576..1024 tokens, dim_head 64), sm_100a only.
+// continuous position bias, n = T'H'W' = 576..1024 tokens, dim_head 64), sm_90a (wgmma).
 //
 //   operands           : bf16, TOKEN-major as the projections write them: Qn [rows, heads*64] (l2-normalised, * q_scale * 8),
 //                        KVn [rows, 2*heads*64] (keys normalised * k_scale | values) -- produced directly by the q / k,v
@@ -7,16 +7,14 @@
 //                        4-D tensor maps (d, head, token, sequence) pick one head's tile out of the token-major rows, so no
 //                        head-major copy exists; V is consumed as an MN-major B operand (rows = keys), so no transposed
 //                        copy either.
-//   phk_attention_tc   : one CTA per (128-query tile, head, sequence); keys streamed in chunks of 64.
-//       warp 0      TMA producer (3-D tensor maps, SWIZZLE_128B; out-of-range rows zero-filled)
-//       warp 1      tcgen05.mma issuer: S[128x64] = Q K^T (4 x K=16) into TMEM cols 0..63,
-//                   O[128x64] += P V (4 x K=16) into TMEM cols 64..127
-//       warps 2..5  softmax, one query row per thread: tcgen05.ld S -> + bias -> online max/sum (fp32) ->
-//                   P = exp(s - m) as bf16 into a SWIZZLE_128B smem tile (the A operand of the PV MMA);
-//                   O is rescaled in TMEM (tcgen05.ld / tcgen05.st) when the running max moves.
-//   S and P never touch HBM; 48 KB smem + 128 TMEM columns per CTA -> several CTAs per SM overlap MMA and softmax.
+//   phk_attention_tc   : one CTA per (64-query tile, head, sequence); keys streamed in chunks of 64 through a two-deep ring.
+//       warps 0..3  one warpgroup: S[64x64] = Q K^T (wgmma, both operands in shared memory) into registers, + bias,
+//                   online max / sum (fp32, a row shared by the four lanes of a quad), P = exp(s - m) packed to bf16
+//                   in registers and used directly as the A operand of O[64x64] += P V (wgmma, A from registers).
+//       warp 4      TMA producer (SWIZZLE_128B; out-of-range rows zero-filled).
+//   S and P never leave the registers; 40 KB shared memory per CTA -> several CTAs per SM overlap MMA and softmax.
 #include "phk_common.cuh"
-#include "phk_sm100.cuh"
+#include "phk_sm90.cuh"
 #include <cstdlib>
 #include <mutex>
 #include <unordered_map>
@@ -24,276 +22,166 @@
 namespace phk {
 namespace {
 
-constexpr int AQ = 128;   // queries per CTA (UMMA M)
-constexpr int AKC = 64;   // keys per chunk (UMMA N for S, K extent for PV)
+constexpr int AQ = 64;    // queries per CTA (wgmma M)
+constexpr int AKC = 64;   // keys per chunk (N of S, K extent of PV)
 constexpr int ADH = 64;   // dim_head
-constexpr int ATHREADS = 64 + 256;  // TMA producer, MMA issuer, eight softmax warps
-constexpr int SQ_BYTES = AQ * ADH * 2, SK_BYTES = AKC * ADH * 2, SV_BYTES = ADH * AKC * 2, SP_BYTES = AQ * AKC * 2;
-constexpr int SB_BYTES = 2 * AQ * 128;  // bias tile: two [128 rows x 32 fp32] SWIZZLE_128B boxes
-constexpr int SMX_BYTES = 4 * AQ * 4;  // row-maximum exchange [2 buffers][2 halves][128 rows]
-constexpr int ATT_SMEM = SQ_BYTES + SK_BYTES + SV_BYTES + SP_BYTES + SB_BYTES + 128 + SMX_BYTES + 1024;
-// PT variant (probabilities in tensor memory): no P tile in shared memory -> 69 KB, three CTAs per SM
-constexpr int ATT_SMEM_PT = SQ_BYTES + SK_BYTES + SV_BYTES + SB_BYTES + 128 + SMX_BYTES + 1024;
-
+constexpr int ATHREADS = 128 + 32;  // one MMA / softmax warpgroup + the TMA producer warp
+constexpr int ASTAGES = 2;
+constexpr int SQ_BYTES = AQ * ADH * 2, SK_BYTES = AKC * ADH * 2, SV_BYTES = ADH * AKC * 2;
+constexpr int ATT_SMEM = SQ_BYTES + ASTAGES * (SK_BYTES + SV_BYTES) + 128 + 1024;
 
 struct AttTcParams {
   const float* bias;        // [heads, n_q, n_k] fp32 or NULL
   __nv_bfloat16* out;       // [.., heads*64] bf16; token i of sequence s at (s*o_seq + i*o_tok) elements
   int n_q, n_k, heads;
   int64_t o_seq, o_tok;
-  int bias_tma;  // 1: the bias tile arrives through TMA (tmB) into shared memory, 0: direct loads
 };
 
-// PT = true: the probabilities never leave tensor memory -- the softmax warps tcgen05.st their bf16 P row into 32 extra
-// TMEM columns and P.V reads its A operand from there (tcgen05.mma with a TMEM A operand).  Without the 16 KB P tile a
-// CTA needs 69 KB of shared memory and (at <= 64 registers) THREE fit on an SM: the 320 CTAs of the MaskGit shape
-// (5 query tiles x 8 heads x 8 sequences) are resident at once instead of 296 + a 24-CTA tail wave that cost a whole
-// second CTA lifetime (ncu r2c7: 38 us, warps active 28 %).
-template <bool PT>
-__global__ void __launch_bounds__(ATHREADS, PT ? 3 : 2) attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ,
-                                                                            const __grid_constant__ CUtensorMap tmK,
-                                                                            const __grid_constant__ CUtensorMap tmV,
-                                                                            const __grid_constant__ CUtensorMap tmB,
-                                                                            AttTcParams p) {
+__global__ void __launch_bounds__(ATHREADS) attention_tc_kernel(const __grid_constant__ CUtensorMap tmQ,
+                                                                const __grid_constant__ CUtensorMap tmK,
+                                                                const __grid_constant__ CUtensorMap tmV,
+                                                                AttTcParams p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
-  constexpr int SPB = PT ? 0 : SP_BYTES;  // no P tile in the TMEM variant
-  const uint32_t sQ = base, sK = sQ + SQ_BYTES, sV = sK + SK_BYTES, sP = sV + SV_BYTES;
-  uint8_t* sP_ptr = base_ptr + SQ_BYTES + SK_BYTES + SV_BYTES;
-  const uint32_t sBias = sP + SPB;
-  const uint8_t* sBias_ptr = sP_ptr + SPB;
-  const uint32_t bars = sBias + SB_BYTES;
-  float* s_mx = reinterpret_cast<float*>(base_ptr + SQ_BYTES + SK_BYTES + SV_BYTES + SPB + SB_BYTES + 128);
-  const uint32_t b_qfull = bars, b_kfull = bars + 8, b_kempty = bars + 16, b_vfull = bars + 24, b_vempty = bars + 32,
-                 b_sfull = bars + 40, b_sempty = bars + 48, b_pfull = bars + 56, b_pvdone = bars + 64,
-                 b_bfull = bars + 72, b_bempty = bars + 80, tmem_slot = bars + 88;
+  const uint32_t sQ = base, sK = sQ + SQ_BYTES, sV = sK + ASTAGES * SK_BYTES;
+  const uint32_t bars = sV + ASTAGES * SV_BYTES;
+  const uint32_t b_q = bars, b_full = bars + 8, b_empty = b_full + 8 * ASTAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int q0 = blockIdx.x * AQ, h = blockIdx.y, seq = blockIdx.z;
   const int nch = (p.n_k + AKC - 1) / AKC;
 
   if (threadIdx.x == 0) {
+    mbar_init(b_q, 1);
+    for (int s = 0; s < ASTAGES; ++s) { mbar_init(b_full + 8 * s, 1); mbar_init(b_empty + 8 * s, 4); }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  if (threadIdx.x == 128) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmQ) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmK) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmV) : "memory");
-    mbar_init(b_qfull, 1); mbar_init(b_kfull, 1); mbar_init(b_kempty, 1); mbar_init(b_vfull, 1);
-    mbar_init(b_vempty, 1); mbar_init(b_sfull, 1); mbar_init(b_sempty, 8); mbar_init(b_pfull, 8);
-    mbar_init(b_pvdone, 1); mbar_init(b_bfull, 1); mbar_init(b_bempty, 8);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(128) : "memory");
-    if (PT)  // second allocation: 32 columns for the bf16 probabilities (128 + 32 per CTA, three CTAs = 480 of 512)
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot + 4), "n"(32) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
-  const uint32_t tS = tmem_base, tO = tmem_base + AKC;
-  uint32_t tP = 0;
-  if (PT) asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tP) : "r"(tmem_slot + 4));
   pdl_wait();  // prologue above overlapped the previous kernel
 
-  if (warp == 0) {
+  if (warp == 4) {
     if (lane == 0) {
-      mbar_expect_tx(b_qfull, SQ_BYTES);
-      tma_load_4d(&tmQ, b_qfull, sQ, 0, h, q0, seq);
+      mbar_expect_tx(b_q, SQ_BYTES);
+      tma_load_4d(&tmQ, b_q, sQ, 0, h, q0, seq);
       for (int j = 0; j < nch; ++j) {
-        if (p.bias_tma) {  // bias tile of this (head, query tile, key chunk): rows h*n_q + q0.., two 32-column boxes
-          mbar_wait(b_bempty, (j & 1) ^ 1);
-          mbar_expect_tx(b_bfull, SB_BYTES);
-          tma_load_2d(&tmB, b_bfull, sBias, j * AKC, h * p.n_q + q0);
-          tma_load_2d(&tmB, b_bfull, sBias + AQ * 128, j * AKC + 32, h * p.n_q + q0);
-        }
-        mbar_wait(b_kempty, (j & 1) ^ 1);
-        mbar_expect_tx(b_kfull, SK_BYTES);
-        tma_load_4d(&tmK, b_kfull, sK, 0, h, j * AKC, seq);
-        mbar_wait(b_vempty, (j & 1) ^ 1);
-        mbar_expect_tx(b_vfull, SV_BYTES);
-        tma_load_4d(&tmV, b_vfull, sV, 0, h, j * AKC, seq);   // [64 keys][64 d]: rows = keys (MN-major B operand of P.V)
+        const int s = j % ASTAGES;
+        mbar_wait(b_empty + 8 * s, ((j / ASTAGES) & 1) ^ 1);
+        mbar_expect_tx(b_full + 8 * s, SK_BYTES + SV_BYTES);
+        tma_load_4d(&tmK, b_full + 8 * s, sK + s * SK_BYTES, 0, h, j * AKC, seq);
+        tma_load_4d(&tmV, b_full + 8 * s, sV + s * SV_BYTES, 0, h, j * AKC, seq);  // [64 keys][64 d]: MN-major B of P.V
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // M=128, N=64, bf16 x bf16 -> f32, both K-major (cute::UMMA::InstrDescriptor)
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(AKC >> 3) << 17) | ((uint32_t)(AQ >> 4) << 24);
-      const uint32_t idesc_pv = idesc | (1u << 16);  // B (= V) MN-major: N = 64 dims contiguous, K = keys along rows
-      mbar_wait(b_qfull, 0);
-      // software pipeline: S(j+1) = Q K(j+1)^T is issued BEFORE waiting for the probabilities of chunk j, so the score
-      // product and its commit / barrier round trip hide behind the softmax of chunk j (S is free as soon as the
-      // softmax warps have pulled S(j) into registers, long before they finish with it)
-      auto issue_qk = [&](int j) {
-        mbar_wait(b_kfull, j & 1);
-        mbar_wait(b_sempty, (j & 1) ^ 1);  // softmax has read S of the previous chunk
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t dq = umma_desc(sQ), dk = umma_desc(sK);
-#pragma unroll
-        for (int k = 0; k < ADH / 16; ++k) umma_f16(tS, dq + 2 * k, dk + 2 * k, idesc, k != 0);
-        umma_commit(b_kempty);
-        umma_commit(b_sfull);
-      };
-      issue_qk(0);
-      for (int j = 0; j < nch; ++j) {
-        if (j + 1 < nch) issue_qk(j + 1);
-        mbar_wait(b_pfull, j & 1);          // P written (and O rescaled) by the softmax warps
-        mbar_wait(b_vfull, j & 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint64_t dp = umma_desc(sP), dv = umma_desc_mn(sV);
-#pragma unroll
-        for (int k = 0; k < AKC / 16; ++k) {  // 16 keys = two 8-row atoms of V = 2048 B (128 descriptor units) per step
-          if (PT) umma_f16_ts(tO, tP + 8 * k, dv + 128 * k, idesc_pv, (j | k) != 0);  // 16 bf16 keys = 8 TMEM columns
-          else umma_f16(tO, dp + 2 * k, dv + 128 * k, idesc_pv, (j | k) != 0);
-        }
-        umma_commit(b_vempty);
-        umma_commit(b_pvdone);
-      }
-    }
-  } else {
-    // softmax: EIGHT warps, thread = (query row, half of the chunk's 64 keys).  A warp may only touch the TMEM lanes of
-    // its lane group (warp % 4), so the two warps of a lane group split the columns.  One row per thread (four warps)
-    // made the per-chunk math a 64-element serial chain per thread -- the kernel's critical path (ncu: tensor pipe 18 %
-    // active at n = 576); halves cut that chain and the register footprint in two.  Only the running MAXIMUM has to be
-    // agreed on per chunk (exchanged through shared memory); each half keeps its own partial sum until the end.
-    const int sw = warp - 2;            // 0..7
-    const int lg = warp & 3;            // TMEM lane group
-    const int hf = sw >> 2;             // which 32 of the 64 keys of a chunk / which 32 of the 64 output dims
-    const int r = lg * 32 + lane;       // query row inside the tile == TMEM lane
-    const int qi = q0 + r;
-    const bool valid = qi < p.n_q;
-    const uint32_t lane_off = (uint32_t)(lg * 32) << 16;
-    const float* brow = (p.bias && valid) ? p.bias + ((int64_t)h * p.n_q + qi) * p.n_k : nullptr;
-    const bool bias_vec = (p.n_k % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.bias) & 15) == 0);
-    constexpr int HC = AKC / 2;         // 32 columns per thread
-    constexpr float LOG2E = 1.4426950408889634f;
-    float m_run = -INFINITY, l_run = 0.f;
-    for (int j = 0; j < nch; ++j) {
-      const int k0 = j * AKC + hf * HC;
-      float sc[HC];  // scores of this thread's 32 keys (logit + bias), then reused by the exponentials
-      mbar_wait(b_sfull, j & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      {
-        uint32_t sv[HC];
-        tmem_ld32(tS + lane_off + hf * HC, sv);
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        __syncwarp();
-        if (lane == 0) mbar_arrive(b_sempty);  // S may be overwritten by the next QK^T (8 arrivals)
-        if (p.bias_tma) {
-          // this row of the TMA-staged tile (box `hf` = this half's 32 columns): 16-byte chunk c of row r sits at chunk
-          // (c ^ (r & 7)) (SWIZZLE_128B); added straight into the score registers
-          mbar_wait(b_bfull, j & 1);
-          const uint8_t* rowp = sBias_ptr + hf * (AQ * 128) + r * 128;
-#pragma unroll
-          for (int c = 0; c < 8; ++c) {
-            const float4 t = *reinterpret_cast<const float4*>(rowp + ((c ^ (r & 7)) << 4));
-            sc[4 * c] = __uint_as_float(sv[4 * c]) + t.x; sc[4 * c + 1] = __uint_as_float(sv[4 * c + 1]) + t.y;
-            sc[4 * c + 2] = __uint_as_float(sv[4 * c + 2]) + t.z; sc[4 * c + 3] = __uint_as_float(sv[4 * c + 3]) + t.w;
-          }
-          __syncwarp();
-          if (lane == 0) mbar_arrive(b_bempty);  // tile consumed (values are in registers)
-        } else if (brow && bias_vec && k0 + HC <= p.n_k) {
-          // direct path (a bias whose row pitch TMA cannot address)
-#pragma unroll
-          for (int c = 0; c < HC / 4; ++c) {
-            const float4 t = __ldg(reinterpret_cast<const float4*>(brow + k0) + c);
-            sc[4 * c] = __uint_as_float(sv[4 * c]) + t.x; sc[4 * c + 1] = __uint_as_float(sv[4 * c + 1]) + t.y;
-            sc[4 * c + 2] = __uint_as_float(sv[4 * c + 2]) + t.z; sc[4 * c + 3] = __uint_as_float(sv[4 * c + 3]) + t.w;
-          }
-        } else {
-#pragma unroll
-          for (int c = 0; c < HC; ++c) sc[c] = __uint_as_float(sv[c]) + ((brow && k0 + c < p.n_k) ? __ldg(brow + k0 + c) : 0.f);
-        }
-      }
-      float mx = -INFINITY;
-      if (k0 + HC <= p.n_k) {  // this half inside the sequence (warp-uniform): no per-element bounds tests
-#pragma unroll
-        for (int c = 0; c < HC; ++c) mx = fmaxf(mx, sc[c]);
-      } else {
-#pragma unroll
-        for (int c = 0; c < HC; ++c) {
-          if (k0 + c >= p.n_k) sc[c] = -INFINITY;  // zero-filled padding keys
-          mx = fmaxf(mx, sc[c]);
-        }
-      }
-      // the row maximum of the chunk over both halves (double-buffered exchange: a thread may be one chunk ahead)
-      s_mx[((j & 1) * 2 + hf) * AQ + r] = mx;
-      asm volatile("bar.sync 2, 256;" ::: "memory");
-      mx = fmaxf(mx, s_mx[((j & 1) * 2 + (hf ^ 1)) * AQ + r]);
-      const float m_new = fmaxf(m_run, mx);
-      const float alpha = fast_ex2((m_run - m_new) * LOG2E);  // 0 on the first chunk (m_run = -inf); m_new is finite:
-      const float m2 = m_new * LOG2E;                          // the first half of every chunk holds valid keys
-      float lsum = 0.f;
-      uint32_t pk[HC / 2];
-#pragma unroll
-      for (int c = 0; c < HC; c += 2) {
-        const float p0 = fast_ex2(fmaf(sc[c], LOG2E, -m2)), p1 = fast_ex2(fmaf(sc[c + 1], LOG2E, -m2));
-        lsum += p0 + p1;
-        pk[c >> 1] = pack_bf16x2(p0, p1);
-      }
-      l_run = l_run * alpha + lsum;
-      m_run = m_new;
-      if (j > 0) {
-        mbar_wait(b_pvdone, (j - 1) & 1);  // previous P.V finished: P buffer free, O stable
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (__any_sync(0xffffffffu, alpha != 1.0f)) {  // rescale this thread's half of the running output in TMEM
-#pragma unroll
-          for (int part = 0; part < 2; ++part) {  // 16 columns at a time: the packed probabilities stay live meanwhile
-            uint32_t ov[16];
-            tmem_ld16(tO + lane_off + hf * 32 + part * 16, ov);
-            tmem_ld_wait();
-#pragma unroll
-            for (int c = 0; c < 16; ++c) ov[c] = __float_as_uint(__uint_as_float(ov[c]) * alpha);
-            tmem_st16(tO + lane_off + hf * 32 + part * 16, ov);
-          }
-        }
-      }
-      if (PT) {
-        // this half of the P row -> TMEM columns [hf*16, hf*16+16) of the probability block (two bf16 keys per column)
-        tmem_st16(tP + lane_off + hf * (HC / 2), pk);
-      } else {
-        // this half of the P row -> SWIZZLE_128B K-major tile: 16-byte chunk c of row r lives at chunk (c ^ (r & 7))
-        uint8_t* prow = sP_ptr + r * 128;
-#pragma unroll
-        for (int c = 0; c < 4; ++c)
-          *reinterpret_cast<uint4*>(prow + (((hf * 4 + c) ^ (r & 7)) << 4)) = make_uint4(pk[4 * c], pk[4 * c + 1], pk[4 * c + 2], pk[4 * c + 3]);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the MMA
-      }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(b_pfull);  // (8 arrivals)
-    }
-    // total row sum = the two halves' partial sums (same running maximum on both sides); exchanged through the buffer the
-    // LAST chunk did not use (a partner may still be reading that chunk's maxima)
-    s_mx[((nch & 1) * 2 + hf) * AQ + r] = l_run;
-    asm volatile("bar.sync 2, 256;" ::: "memory");
-    const float inv = 1.f / (l_run + s_mx[((nch & 1) * 2 + (hf ^ 1)) * AQ + r]);
-    mbar_wait(b_pvdone, (nch - 1) & 1);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    __nv_bfloat16* orow = p.out + (int64_t)seq * p.o_seq + (int64_t)qi * p.o_tok + h * ADH;
-    {
-      uint32_t ov[32];
-      tmem_ld32(tO + lane_off + hf * 32, ov);
-      if (valid) {
-#pragma unroll
-        for (int c = 0; c < 32; c += 8) {
-          uint32_t w[4];
-#pragma unroll
-          for (int e = 0; e < 4; ++e)
-            w[e] = pack_bf16x2(__uint_as_float(ov[c + 2 * e]) * inv, __uint_as_float(ov[c + 2 * e + 1]) * inv);
-          *reinterpret_cast<uint4*>(orow + hf * 32 + c) = make_uint4(w[0], w[1], w[2], w[3]);
-        }
-      }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
+    return;
   }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(128) : "memory");
-    if (PT) asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tP), "n"(32) : "memory");
+  // ---- MMA / softmax warpgroup: lane l of warp w holds rows 16w + l/4 (index 0) and + 8 (index 1) of the tile and
+  // columns 8j + 2(l%4) + {0, 1}, j = 0..7, of S and O (wgmma accumulator fragment)
+  const int t4 = lane & 3;
+  const int rows[2] = {q0 + 16 * warp + (lane >> 2), q0 + 16 * warp + (lane >> 2) + 8};
+  const float* brow[2];
+#pragma unroll
+  for (int i = 0; i < 2; ++i) brow[i] = (p.bias && rows[i] < p.n_q) ? p.bias + ((int64_t)h * p.n_q + rows[i]) * p.n_k : nullptr;
+  const bool bias_vec = (p.n_k % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.bias) & 7) == 0);
+  constexpr float LOG2E = 1.4426950408889634f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  mbar_wait(b_q, 0);
+  const uint64_t dq = gmma_desc(sQ);
+  for (int j = 0; j < nch; ++j) {
+    const int s = j % ASTAGES;
+    mbar_wait(b_full + 8 * s, (j / ASTAGES) & 1);
+    float sc[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) sc[i] = 0.f;
+    const uint64_t dk = gmma_desc(sK + s * SK_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < ADH / 16; ++k) wgmma_m64n64k16_ss<0>(sc, dq + 2 * k, dk + 2 * k, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    // + bias, padding keys -> -inf, chunk maximum per row
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      const int key = j * AKC + 8 * jj + 2 * t4;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float& a = sc[4 * jj + 2 * i];
+        float& b = sc[4 * jj + 2 * i + 1];
+        if (brow[i]) {
+          if (bias_vec && key + 1 < p.n_k) {
+            const float2 t = __ldg(reinterpret_cast<const float2*>(brow[i] + key));
+            a += t.x; b += t.y;
+          } else {
+            if (key < p.n_k) a += __ldg(brow[i] + key);
+            if (key + 1 < p.n_k) b += __ldg(brow[i] + key + 1);
+          }
+        }
+        if (key >= p.n_k) a = -INFINITY;  // zero-filled padding keys
+        if (key + 1 >= p.n_k) b = -INFINITY;
+        mx[i] = fmaxf(mx[i], fmaxf(a, b));
+      }
+    }
+    float alpha[2], m2[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+      mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+      const float m_new = fmaxf(m_run[i], mx[i]);  // finite: every chunk starts with a valid key
+      alpha[i] = fast_ex2((m_run[i] - m_new) * LOG2E);  // 0 on the first chunk (m_run = -inf)
+      m2[i] = m_new * LOG2E;
+      m_run[i] = m_new;
+    }
+    // P = exp(s - m) -> bf16 A fragments of the P.V product (four K = 16 steps of 16 keys)
+    uint32_t pa[4][4];
+    float lsum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const float p0 = fast_ex2(fmaf(sc[4 * jj + 2 * i], LOG2E, -m2[i]));
+        const float p1 = fast_ex2(fmaf(sc[4 * jj + 2 * i + 1], LOG2E, -m2[i]));
+        lsum[i] += p0 + p1;
+        pa[jj >> 1][(jj & 1) * 2 + i] = pack_bf16x2(p0, p1);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) l_run[i] = l_run[i] * alpha[i] + lsum[i];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) {
+      o[4 * jj] *= alpha[0]; o[4 * jj + 1] *= alpha[0];
+      o[4 * jj + 2] *= alpha[1]; o[4 * jj + 3] *= alpha[1];
+    }
+    const uint64_t dv = gmma_desc_mn(sV + s * SV_BYTES);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < AKC / 16; ++k)  // 16 keys = two 8-row atoms of V = 2048 B (128 descriptor units) per step
+      wgmma_m64n64k16_rs<1>(o, pa[k], dv + 128 * k, 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    __syncwarp();
+    if (lane == 0) mbar_arrive(b_empty + 8 * s);  // this warp is done with K and V of the slot
+  }
+  // row sums over the quad, normalise, bf16 out
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    l_run[i] += __shfl_xor_sync(0xffffffffu, l_run[i], 1);
+    l_run[i] += __shfl_xor_sync(0xffffffffu, l_run[i], 2);
+  }
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    if (rows[i] >= p.n_q) continue;
+    const float inv = 1.f / l_run[i];
+    __nv_bfloat16* orow = p.out + (int64_t)seq * p.o_seq + (int64_t)rows[i] * p.o_tok + h * ADH;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj)
+      *reinterpret_cast<uint32_t*>(orow + 8 * jj + 2 * t4) = pack_bf16x2(o[4 * jj + 2 * i] * inv, o[4 * jj + 2 * i + 1] * inv);
   }
 }
 
@@ -329,22 +217,6 @@ __global__ void __launch_bounds__(256) attention_prep_kernel(const float* __rest
 }
 
 
-// bf16 [d2][d1][d0] with d0 contiguous; box [1][b1][64]; SWIZZLE_128B; zero OOB fill
-// fp32 [rows][cols] bias, box [128 rows][32 cols = 128 B], SWIZZLE_128B, zero OOB fill
-int make_map_bias(const float* ptr, int64_t rows, int64_t cols, CUtensorMap* out) {
-  EncodeTiledFn fn = encode_fn();
-  PHK_REQUIRE(fn, PHK_E_UNSUPPORTED, "cuTensorMapEncodeTiled not available from the driver");
-  const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  const cuuint64_t gstride[1] = {(cuuint64_t)cols * 4};
-  const cuuint32_t box[2] = {32, (cuuint32_t)AQ};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(ptr), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  PHK_REQUIRE(r == CUDA_SUCCESS, PHK_E_ARG, "cuTensorMapEncodeTiled rejected the attention bias");
-  return 0;
-}
-
 // one head's [tokens, 64] tile out of a token-major bf16 matrix [n_seq * n rows, ld elements]: dims (d, head, token,
 // sequence), box [64 d][1][box_tok tokens][1], SWIZZLE_128B; tokens >= n are zero-filled (never the next sequence's)
 int make_map_4d(const void* ptr, int64_t n, int64_t heads, int64_t n_seq, int64_t ld, int box_tok, CUtensorMap* out) {
@@ -361,9 +233,6 @@ int make_map_4d(const void* ptr, int64_t n, int64_t heads, int64_t n_seq, int64_
   PHK_REQUIRE(r == CUDA_SUCCESS, PHK_E_ARG, "cuTensorMapEncodeTiled rejected an attention operand");
   return 0;
 }
-
-constexpr int kTmemVariantFromTokens = 256;  // sequences at least this long take the TMEM-probabilities variant by default
-int g_attn_variant = -1;                // phk_debug_attention_tc_variant
 
 }  // namespace
 }  // namespace phk
@@ -391,36 +260,17 @@ extern "C" int phk_attention_tc_bf16(const void* Qn, int64_t ld_q, const void* K
   PHK_TRY(make_map_4d(Qn, n, heads, n_seq, ld_q, AQ, &tq));
   PHK_TRY(make_map_4d(KVn, n, heads, n_seq, ld_kv, AKC, &tk));
   PHK_TRY(make_map_4d(reinterpret_cast<const __nv_bfloat16*>(KVn) + I, n, heads, n_seq, ld_kv, AKC, &tv));
-  static unsigned long long configured_mask = 0;
-  const bool configured = device_configured(&configured_mask);
-  if (!configured) {
-    PHK_CUDA(cudaFuncSetAttribute(attention_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM));
-    PHK_CUDA(cudaFuncSetAttribute(attention_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATT_SMEM_PT));
-    mark_configured(&configured_mask);
-  }
-  const int bias_tma = bias && (n % 4 == 0) && ((reinterpret_cast<uintptr_t>(bias) & 15) == 0);
-  CUtensorMap tb = tq;  // placeholder when unused
-  if (bias_tma) PHK_TRY(make_map_bias(bias, (int64_t)heads * n, n, &tb));
-  AttTcParams p{bias, (__nv_bfloat16*)out_bf16, n, n, heads, (int64_t)n * heads * 64, (int64_t)heads * 64, bias_tma};
+  AttTcParams p{bias, (__nv_bfloat16*)out_bf16, n, n, heads, (int64_t)n * heads * 64, (int64_t)heads * 64};
   dim3 grid((unsigned)((n + AQ - 1) / AQ), (unsigned)heads, (unsigned)n_seq);
-  // default: probabilities in tensor memory (three CTAs per SM) for long sequences -- 24.2 vs 30.5 us at 8 x 576 tokens, where
-  // 320 CTAs no longer need a second wave; single-chunk sequences (n = 64: 8.9 vs 10.2 us) keep the shared-memory tile
-  // (profiles/r02/op_bench_c8.txt).  PHK_ATTN_P_TMEM=0/1 or phk_debug_attention_tc_variant force one.
-  static const int env_variant = [] { const char* e = std::getenv("PHK_ATTN_P_TMEM"); return e ? (e[0] != '0' ? 1 : 0) : -1; }();
-  const int variant = g_attn_variant >= 0 ? g_attn_variant : env_variant >= 0 ? env_variant : (n >= kTmemVariantFromTokens);
-  if (variant)
-    PHK_CUDA(launch_pdl(attention_tc_kernel<true>, dim3(grid), dim3(ATHREADS), (size_t)(ATT_SMEM_PT), st, tq, tk, tv, tb, p));
-  else
-    PHK_CUDA(launch_pdl(attention_tc_kernel<false>, dim3(grid), dim3(ATHREADS), (size_t)(ATT_SMEM), st, tq, tk, tv, tb, p));
+  PHK_CUDA(launch_pdl(attention_tc_kernel, dim3(grid), dim3(ATHREADS), (size_t)(ATT_SMEM), st, tq, tk, tv, p));
   PHK_LAUNCH_CHECK();
   return 0;
 }
 
-// tests / A-B measurements: 0 probabilities through a shared-memory tile (two CTAs per SM), 1 probabilities in tensor
-// memory (three CTAs per SM); < 0 restores the PHK_ATTN_P_TMEM environment default
+// tests: selected the probability path of an earlier tensor-memory design; accepted for ABI compatibility, the one
+// kernel above serves every value
 extern "C" int phk_debug_attention_tc_variant(int32_t variant) {
   PHK_REQUIRE(variant <= 1, PHK_E_ARG, "phk_debug_attention_tc_variant: 0, 1 or < 0");
-  g_attn_variant = variant;
   return 0;
 }
 
@@ -442,7 +292,7 @@ extern "C" int phk_attention_tc(const float* q, const float* kv, const float* q_
   {
     Prof prof_(FAM_ATTENTION, s, 0.0);
     const int64_t pairs = rows * heads;
-    const unsigned blocks = (unsigned)((pairs + 7) / 8 < 148 * 16 ? (pairs + 7) / 8 : 148 * 16);
+    const unsigned blocks = (unsigned)((pairs + 7) / 8 < kNumSMs * 16 ? (pairs + 7) / 8 : kNumSMs * 16);
     PHK_CUDA(launch_pdl(attention_prep_kernel, dim3(blocks), dim3(256), (size_t)(0), st, q, kv, q_scale, k_scale, Qn, KVn, rows,
                         (int)heads, scale));
     PHK_LAUNCH_CHECK();

@@ -1,7 +1,7 @@
 // fp32 FFMA GEMM for the parity mode: C[map(m), n] = sum_k A[m,k] * W[n,k] (+bias) (+residual).
 // nn.Linear semantics (attention.py:49-52, 120-126; cvivit.py:276, 283).  fp32 operands and
 // fp32 accumulation keep the C-ViViT token ids identical to the fp32 reference (SURVEY H1);
-// the tensor-core path lives in gemm_tcgen05.cu.
+// the tensor-core path lives in gemm_wgmma.cu.
 //
 // 128x128x16 CTA tile, 256 threads, 8x8 register micro-tile, double-buffered shared memory
 // (k-major so the inner loop reads two float4 per operand with no bank conflicts).

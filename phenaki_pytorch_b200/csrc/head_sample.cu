@@ -1,4 +1,4 @@
-// Fused logits head of the sampling loop (sm_100a): logits GEMM + bias + gumbel noise + argmax + online softmax,
+// Fused logits head of the sampling loop (sm_90a): logits GEMM + bias + gumbel noise + argmax + online softmax,
 // reduced over the vocabulary inside the kernel -- the (b, n, V) logits never exist in memory
 // (phenaki_pytorch.py:213 to_logits, :161 classifier-free guidance, :83-93 gumbel_sample, :506-509, :547-550).
 //
@@ -8,14 +8,15 @@
 // only A operand: half the FLOPs of the reference's two logits GEMMs and no cond/null pairing in the epilogue.
 //
 // One CTA owns 128 tokens and a contiguous slice of the vocabulary:
-//   warp 0      TMA: the 128 x dim A panel is loaded ONCE and stays resident in shared memory (dim <= 512: 128 KB);
-//               W tiles (128 vocabulary rows x 64) stream through a 4-stage ring -> L2 traffic is W only.
-//   warp 1      tcgen05.mma issuer, two 128-column TMEM accumulators (MMA of tile i+1 overlaps the math of tile i).
-//   warps 2..17 math: thread = (token, 32-column group); tcgen05.ld straight from TMEM (no smem staging), Philox4x32-7
-//               noise (phk_common.cuh; counter layout and gumbel transform of phk_sample_tokens), running (argmax of l/T + g, l at argmax, max l, sum exp).
+//   warpgroup 0     TMA (one thread): the 128 x dim A panel is loaded ONCE and stays resident in shared memory
+//                   (dim <= 512: 128 KB); W tiles (128 vocabulary rows x 64) stream through a 4-stage ring -> L2 traffic
+//                   is W only.
+//   warpgroups 1..4 each multiplies one 64-token x 64-column quadrant of the 128 x 128 logits tile (wgmma) and works on
+//                   its accumulator fragment in registers: Philox4x32-7 noise (phk_common.cuh; counter layout and gumbel
+//                   transform of phk_sample_tokens), running (argmax of l/T + g, l at argmax, max l, sum exp) per row.
 // Partials per (token, vocabulary slice) are merged by head_finalize_kernel (pred, 1 - softmax(l)[pred], mask).
 #include "phk_common.cuh"
-#include "phk_sm100.cuh"
+#include "phk_sm90.cuh"
 #include <mutex>
 
 namespace phk {
@@ -23,10 +24,10 @@ namespace {
 
 constexpr int HM = 128, HN = 128, HK = 64, HSTAGES = 4;
 constexpr int H_MATH_WARPS = 16;
-constexpr int HTHREADS = 64 + H_MATH_WARPS * 32;  // 576
+constexpr int HTHREADS = 128 + H_MATH_WARPS * 32;  // 640
 constexpr int HSTAGE_BYTES = HN * HK * 2;          // 16 KB
 constexpr int H_MAX_KB = 8;                        // dim <= 512
-constexpr int H_EX_BYTES = HM * 3 * 6 * 4;        // exchange buffer of the final 4-way merge
+constexpr int H_EX_BYTES = HM * 6 * 4;             // exchange buffer of the merge of the two column halves
 constexpr int H_SMEM = H_MAX_KB * HM * HK * 2 + HSTAGES * HSTAGE_BYTES + 256 + H_EX_BYTES + 1024;
 
 struct HeadParams {
@@ -39,6 +40,18 @@ struct HeadParams {
   int* part_i;     // [n_tokens, n_splits] argmax index
 };
 
+struct HeadRun {
+  float best, lbest, mx, ssum;
+  int bidx;
+};
+// merge of two partial states of one token: the larger perturbed logit (the smaller index on ties), log-sum-exp sums
+__device__ __forceinline__ void head_merge(HeadRun& a, float oy, float ol, float om, float os, int oi) {
+  if (oy > a.best || (oy == a.best && oi < a.bidx)) { a.best = oy; a.bidx = oi; a.lbest = ol; }
+  const float nm = fmaxf(a.mx, om);
+  a.ssum = a.ssum * __expf(a.mx - nm) + os * __expf(om - nm);
+  a.mx = nm;
+}
+
 __global__ void __launch_bounds__(HTHREADS, 1) head_sample_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                   const __grid_constant__ CUtensorMap tmB,
                                                                   HeadParams p) {
@@ -50,8 +63,7 @@ __global__ void __launch_bounds__(HTHREADS, 1) head_sample_kernel(const __grid_c
   const uint32_t sA = base;                                   // num_kb x [128 x 64] resident A panel
   const uint32_t sB = base + H_MAX_KB * HM * HK * 2;          // ring
   const uint32_t bars = sB + HSTAGES * HSTAGE_BYTES;
-  const uint32_t bar_afull = bars, bar_full = bars + 8, bar_empty = bar_full + 8 * HSTAGES,
-                 bar_tfull = bar_empty + 8 * HSTAGES, bar_tempty = bar_tfull + 16, tmem_slot = bar_tempty + 16;
+  const uint32_t bar_afull = bars, bar_full = bars + 8, bar_empty = bar_full + 8 * HSTAGES;
   float* ex = reinterpret_cast<float*>(base_ptr + H_MAX_KB * HM * HK * 2 + HSTAGES * HSTAGE_BYTES + 256);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tile = blockIdx.x / p.n_splits, split = blockIdx.x % p.n_splits;
@@ -62,23 +74,14 @@ __global__ void __launch_bounds__(HTHREADS, 1) head_sample_kernel(const __grid_c
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     mbar_init(bar_afull, 1);
-    for (int s = 0; s < HSTAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, 1); }
-    for (int a = 0; a < 2; ++a) { mbar_init(bar_tfull + 8 * a, 1); mbar_init(bar_tempty + 8 * a, H_MATH_WARPS); }
+    for (int s = 0; s < HSTAGES; ++s) { mbar_init(bar_full + 8 * s, 1); mbar_init(bar_empty + 8 * s, H_MATH_WARPS); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "n"(2 * HN) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  uint32_t tmem_base;
-  asm volatile("ld.shared.u32 %0, [%1];" : "=r"(tmem_base) : "r"(tmem_slot));
   pdl_wait();
 
-  if (warp == 0) {
-    if (lane == 0 && my_tiles > 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0 && my_tiles > 0) {
       mbar_expect_tx(bar_afull, (uint32_t)num_kb * HM * HK * 2);
       for (int kb = 0; kb < num_kb; ++kb) tma_load_2d(&tmA, bar_afull, sA + kb * HM * HK * 2, kb * HK, m_tile * HM);
       int stage = 0;
@@ -93,139 +96,107 @@ __global__ void __launch_bounds__(HTHREADS, 1) head_sample_kernel(const __grid_c
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0 && my_tiles > 0) {
-      const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(HN >> 3) << 17) | ((uint32_t)(HM >> 4) << 24);
-      mbar_wait(bar_afull, 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        const int acc = it & 1;
-        const uint32_t use = (uint32_t)(it >> 1);
-        mbar_wait(bar_tempty + 8 * acc, (use & 1) ^ 1);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t d_tmem = tmem_base + acc * HN;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(bar_full + 8 * stage, phase);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t da = umma_desc(sA + kb * HM * HK * 2);
-          const uint64_t db = umma_desc(sB + stage * HSTAGE_BYTES);
-#pragma unroll
-          for (int k = 0; k < HK / 16; ++k) umma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0);
-          umma_commit(bar_empty + 8 * stage);
-          if (++stage == HSTAGES) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(bar_tfull + 8 * acc);
-      }
-    }
   } else {
-    // ===================== math warps =====================
-    const int mw = warp - 2;
-    const int lg = warp & 3;     // TMEM lane group
-    const int cgrp = mw >> 2;    // 32-column group of the tile
-    const int tl = lg * 32 + lane;
-    const int tok = m_tile * HM + tl;
-    const bool valid = tok < p.n_tokens;
-    float best = -FLT_MAX, lbest = 0.f, mx = -FLT_MAX, ssum = 0.f;
-    int bidx = 0x7fffffff;
+    // ===================== MMA + math warps =====================
+    const int mw = warp - 4;
+    const int wg = mw >> 2, w = mw & 3;
+    const int rq = (wg & 1) * 64, cq = (wg >> 1) * 64;  // this warpgroup's quadrant of the tile
+    const int t4 = lane & 3;
+    int tl[2], tok[2];
+    unsigned long long ctr0[2];
     // noise key: by value, or read from device memory so that a captured CUDA graph draws fresh noise on every replay
     const unsigned long long seed = p.rng ? p.rng[0] : p.seed;
-    const unsigned long long ctr0 = (p.rng ? p.rng[1] : p.offset) + (unsigned long long)tok * (unsigned long long)((p.V + 3) / 4);
+    const unsigned long long off = p.rng ? p.rng[1] : p.offset;
+    HeadRun run[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      tl[i] = rq + 16 * w + (lane >> 2) + 8 * i;
+      tok[i] = m_tile * HM + tl[i];
+      ctr0[i] = off + (unsigned long long)tok[i] * (unsigned long long)((p.V + 3) / 4);
+      run[i] = HeadRun{-FLT_MAX, 0.f, -FLT_MAX, 0.f, 0x7fffffff};
+    }
+    constexpr float LOG2E = 1.4426950408889634f;
+    if (my_tiles > 0) mbar_wait(bar_afull, 0);
+    int stage = 0;
+    uint32_t phase = 0;
     for (int it = 0; it < my_tiles; ++it) {
-      const int acc = it & 1;
-      const uint32_t use = (uint32_t)(it >> 1);
-      const int v_base = (n_begin + it) * HN + cgrp * 32;
-      mbar_wait(bar_tfull + 8 * acc, use & 1);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      uint32_t raw[32];
-      tmem_ld32(tmem_base + acc * HN + cgrp * 32 + ((uint32_t)(lg * 32) << 16), raw);
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_tempty + 8 * acc);  // accumulator slice consumed
-      if (!valid || v_base >= p.V) continue;
-      constexpr float LOG2E = 1.4426950408889634f;
-      if (v_base + 32 <= p.V) {
-        // whole 32-column group inside the vocabulary (always, for V % 32 == 0): no per-element bounds tests.
-        // Issue-slot budget per logit (the kernel is bound by them, not by the MMA): Philox-7 ~9, gumbel 5 + 2 MUFU,
-        // perturbed arg-max 4, softmax 2 + 1 MUFU + the running maximum.
-        float mxs = mx * LOG2E;
+      float d[32];
 #pragma unroll
-        for (int c = 0; c < 32; c += 4) {
-          const int v0 = v_base + c;
-          float l4[4] = {__uint_as_float(raw[c]), __uint_as_float(raw[c + 1]), __uint_as_float(raw[c + 2]),
-                         __uint_as_float(raw[c + 3])};
-          if (p.bias) {
-            const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + v0));
-            l4[0] += b4.x; l4[1] += b4.y; l4[2] += b4.z; l4[3] += b4.w;
-          }
-          uint32_t rnd[4];
-          const unsigned long long ctr = ctr0 + (unsigned long long)(v0 >> 2);
-          philox4x32<kNoiseRounds>((uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), rnd);
+      for (int i = 0; i < 32; ++i) d[i] = 0.f;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(bar_full + 8 * stage, phase);
+        const uint64_t da = gmma_desc(sA + kb * HM * HK * 2 + rq * 128);
+        const uint64_t db = gmma_desc(sB + stage * HSTAGE_BYTES + cq * 128);
+        wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const float y = fmaf(l4[j], p.inv_T, gumbel_from_bits(rnd[j]));
-            if (y > best) { best = y; bidx = v0 + j; lbest = l4[j]; }
-          }
-          const float gm = fmaxf(fmaxf(l4[0], l4[1]), fmaxf(l4[2], l4[3]));
-          if (gm > mx) { ssum *= fast_ex2((mx - gm) * LOG2E); mx = gm; mxs = gm * LOG2E; }  // one rescale per 4 logits
-#pragma unroll
-          for (int j = 0; j < 4; ++j) ssum += fast_ex2(fmaf(l4[j], LOG2E, -mxs));
-        }
-        continue;
+        for (int k = 0; k < HK / 16; ++k) wgmma_m64n64k16_ss<0>(d, da + 2 * k, db + 2 * k, 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar_empty + 8 * stage);
+        if (++stage == HSTAGES) { stage = 0; phase ^= 1; }
       }
+      // columns v, v + 1 (v even) of each row, in increasing v: Philox block v / 4 supplies draws v % 4 and v % 4 + 1
+      // (the same (token, v) -> noise map as phk_sample_tokens)
+      const int v_tile = (n_begin + it) * HN + cq + 2 * t4;
 #pragma unroll
-      for (int c = 0; c < 32; c += 4) {
-        const int v0 = v_base + c;
-        if (v0 >= p.V) break;
-        float bb[4] = {0.f, 0.f, 0.f, 0.f};
-        if (p.bias) {
-          if (v0 + 3 < p.V) { const float4 b4 = __ldg(reinterpret_cast<const float4*>(p.bias + v0)); bb[0] = b4.x; bb[1] = b4.y; bb[2] = b4.z; bb[3] = b4.w; }
-          else { for (int j = 0; j < 4; ++j) if (v0 + j < p.V) bb[j] = __ldg(p.bias + v0 + j); }
+      for (int jj = 0; jj < 8; ++jj) {
+        const int v = v_tile + 8 * jj;
+        if (v >= p.V) break;
+        const bool in1 = v + 1 < p.V;
+        float bb[2] = {0.f, 0.f};
+        if (p.bias) { bb[0] = __ldg(p.bias + v); if (in1) bb[1] = __ldg(p.bias + v + 1); }
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          if (tok[i] >= p.n_tokens) continue;
+          uint32_t rnd[4];
+          const unsigned long long ctr = ctr0[i] + (unsigned long long)(v >> 2);
+          philox4x32<kNoiseRounds>((uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), rnd);
+          const uint32_t r0 = (v & 2) ? rnd[2] : rnd[0], r1 = (v & 2) ? rnd[3] : rnd[1];
+          const float l0 = d[4 * jj + 2 * i] + bb[0];
+          const float l1 = in1 ? d[4 * jj + 2 * i + 1] + bb[1] : -FLT_MAX;
+          HeadRun& a = run[i];
+          const float y0 = fmaf(l0, p.inv_T, gumbel_from_bits(r0));
+          if (y0 > a.best) { a.best = y0; a.bidx = v; a.lbest = l0; }
+          if (in1) {
+            const float y1 = fmaf(l1, p.inv_T, gumbel_from_bits(r1));
+            if (y1 > a.best) { a.best = y1; a.bidx = v + 1; a.lbest = l1; }
+          }
+          const float gm = fmaxf(l0, l1);
+          if (gm > a.mx) { a.ssum *= fast_ex2((a.mx - gm) * LOG2E); a.mx = gm; }
+          const float mxs = a.mx * LOG2E;
+          a.ssum += fast_ex2(fmaf(l0, LOG2E, -mxs));
+          if (in1) a.ssum += fast_ex2(fmaf(l1, LOG2E, -mxs));
         }
-        uint32_t rnd[4];
-        const unsigned long long ctr = ctr0 + (unsigned long long)(v0 >> 2);
-        philox4x32<kNoiseRounds>((uint32_t)ctr, (uint32_t)(ctr >> 32), 0u, 0u, (uint32_t)seed, (uint32_t)(seed >> 32), rnd);
-        float l4[4];
-        float gm = -FLT_MAX;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const bool in = v0 + j < p.V;
-          l4[j] = in ? __uint_as_float(raw[c + j]) + bb[j] : -FLT_MAX;
-          gm = fmaxf(gm, l4[j]);
-          const float y = fmaf(l4[j], p.inv_T, gumbel_from_bits(rnd[j]));
-          if (in && y > best) { best = y; bidx = v0 + j; lbest = l4[j]; }
-        }
-        if (gm > mx) { ssum *= fast_ex2((mx - gm) * LOG2E); mx = gm; }  // one rescale per 4 logits
-        const float mxs = mx * LOG2E;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) ssum += fast_ex2(fmaf(l4[j], LOG2E, -mxs));
       }
     }
-    // merge the four column groups of every token, then one partial per (token, vocabulary slice)
-    if (cgrp > 0) {
-      float* e = ex + (tl * 3 + cgrp - 1) * 6;
-      e[0] = best; e[1] = lbest; e[2] = mx; e[3] = ssum; e[4] = __int_as_float(bidx);
+    // merge the four lanes of a quad (same rows), then the two column halves of every token
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+#pragma unroll
+      for (int o = 1; o <= 2; o <<= 1) {
+        const float oy = __shfl_xor_sync(0xffffffffu, run[i].best, o), ol = __shfl_xor_sync(0xffffffffu, run[i].lbest, o);
+        const float om = __shfl_xor_sync(0xffffffffu, run[i].mx, o), os = __shfl_xor_sync(0xffffffffu, run[i].ssum, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, run[i].bidx, o);
+        head_merge(run[i], oy, ol, om, os, oi);
+      }
+      if (cq == 64 && t4 == 0) {
+        float* e = ex + tl[i] * 6;
+        e[0] = run[i].best; e[1] = run[i].lbest; e[2] = run[i].mx; e[3] = run[i].ssum; e[4] = __int_as_float(run[i].bidx);
+      }
     }
     asm volatile("bar.sync 1, %0;" ::"n"(H_MATH_WARPS * 32) : "memory");
-    if (cgrp == 0 && valid) {
-      for (int qq = 0; qq < 3; ++qq) {
-        const float* e = ex + (tl * 3 + qq) * 6;
-        const float oy = e[0], ol = e[1], om = e[2], os = e[3];
-        const int oi = __float_as_int(e[4]);
-        if (oy > best || (oy == best && oi < bidx)) { best = oy; bidx = oi; lbest = ol; }
-        const float nm = fmaxf(mx, om);
-        ssum = ssum * __expf(mx - nm) + os * __expf(om - nm);
-        mx = nm;
+    if (cq == 0 && t4 == 0) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        if (tok[i] >= p.n_tokens) continue;
+        const float* e = ex + tl[i] * 6;
+        head_merge(run[i], e[0], e[1], e[2], e[3], __float_as_int(e[4]));
+        const int64_t slot = (int64_t)tok[i] * p.n_splits + split;
+        p.part_f[slot] = make_float4(run[i].best, run[i].lbest, run[i].mx, run[i].ssum);
+        p.part_i[slot] = run[i].bidx;
       }
-      const int64_t slot = (int64_t)tok * p.n_splits + split;
-      p.part_f[slot] = make_float4(best, lbest, mx, ssum);
-      p.part_i[slot] = bidx;
     }
-  }
-  __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(2 * HN) : "memory");
   }
 }
 

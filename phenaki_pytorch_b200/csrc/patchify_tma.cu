@@ -7,7 +7,7 @@
 // (107 MB at cfg2) keeps streaming instead of stalling on the two block-wide reductions of every token.  gamma / beta
 // are staged once per CTA.  Falls back to patchify_ln_reg_kernel (rowops.cu) when the shape does not fit a box.
 #include "phk_common.cuh"
-#include "phk_sm100.cuh"
+#include "phk_sm90.cuh"
 #include <cstdlib>
 #include <mutex>
 #include <unordered_map>

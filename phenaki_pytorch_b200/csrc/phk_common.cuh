@@ -1,4 +1,4 @@
-// Shared device/host helpers for libphk (sm_100a only).
+// Shared device/host helpers for libphk (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -8,8 +8,8 @@
 #include "../../include/phk.h"
 #include <cstdlib>
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libphk is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libphk is written for sm_90a (H100) only"
 #endif
 
 namespace phk {
@@ -35,7 +35,7 @@ int patchify_ln_tma_launch(const float* video, int B, int C, int F, int H, int W
 
 static inline cudaStream_t to_stream(phk_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
 
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;  // H100 SXM
 
 // One-time per-DEVICE kernel configuration (cudaFuncSetAttribute is a per-device setting; a process may drive several
 // devices): `mask` is a call-site static, bit d = "done on device d".
@@ -62,7 +62,7 @@ struct Prof {
 // Programmatic dependent launch (PDL): every kernel of the library is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization, triggers its dependents immediately and waits for its
 // predecessors right before its first global-memory access.  The next kernel's launch latency, block scheduling and
-// prologue (barrier init, tensor-map prefetch, TMEM allocation) then overlap the tail of the running kernel.
+// prologue (barrier init, tensor-map prefetch) then overlap the tail of the running kernel.
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_prologue() { pdl_trigger(); pdl_wait(); }
@@ -160,7 +160,7 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
 }
 
 // inference drivers bracket their GEMM calls with this: the W operands are weights that no kernel of the stream rewrites,
-// so the tcgen05 GEMM may request their first tiles before its programmatic-dependent-launch wait (gemm_tcgen05.cu)
+// so the tensor-core GEMM may request their first tiles before its programmatic-dependent-launch wait (gemm_wgmma.cu)
 void gemm_static_weights(bool on);
 struct StaticWeightsScope {
   StaticWeightsScope() { gemm_static_weights(true); }

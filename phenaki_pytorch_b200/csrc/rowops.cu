@@ -1,4 +1,4 @@
-// Row-wise / memory-bound kernels of the phenaki hot path (sm_100a).
+// Row-wise / memory-bound kernels of the phenaki hot path (sm_90a).
 // Every kernel cites the reference code it replaces (paths relative to
 // /root/reference/phenaki_pytorch/).  All are HBM/L2-bound: coalesced 16-byte accesses,
 // no tensor cores on purpose.

@@ -9,7 +9,7 @@
 //
 //   mask_compact      index[b*k]   <- positions of the masked tokens of each sequence, in order
 //   ln_cfg_gather     emb[b*k, D]  <- norm_out(x_null) + s * (norm_out(x_cond) - norm_out(x_null)) of those rows (bf16)
-//   phk_head_sample   on b*k rows  (tcgen05 GEMM + gumbel argmax + confidence, head_sample.cu; logits never stored)
+//   phk_head_sample   on b*k rows  (wgmma GEMM + gumbel argmax + confidence, head_sample.cu; logits never stored)
 //   scatter           ids / pred / score of the masked rows; score = -1e4 and ids untouched elsewhere
 //
 // Plain kernels (no tensor cores): they also run under tests/cuda_emu.

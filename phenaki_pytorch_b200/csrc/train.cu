@@ -11,9 +11,9 @@
 // phk_peg3d, phk_geglu, phk_token_embed, phk_cpb_bias) and keeps every layer's activations.  The backward kernels are
 // deliberately plain (one warp per row, coalesced, no tensor cores): this is the parity path that pins the gradient
 // math against the reference's autograd; every formula is restated on the CPU in tests/train_mirror.py and checked
-// against the reference there.  The tcgen05 (bf16) backward GEMMs are the next step on top of it.
-// STATUS: written after the round's GPU budget was spent -- compiled for sm_100a and executed on the CPU by tests/cuda_emu
-// (this very source, g++-compiled) against the reference's gradients; not yet run on a GPU.
+// against the reference there.  In bf16 mode the products run on the tensor-core GEMM instead (see below).
+// Checked against the reference's gradients on the CPU by tests/cuda_emu (this very source, g++-compiled) and on the GPU
+// by tests/test_gpu_train.py.
 #include "phk_common.cuh"
 #include <cstdlib>
 // the kernels of this file are ordinary stream-ordered launches (they do not use programmatic dependent launch)
@@ -261,7 +261,7 @@ int colsum(const float* x, int64_t rows, int cols, int64_t ld, float* out, cudaS
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// bf16 mode (PHK_PREC_BF16): the three products of every nn.Linear run on the tcgen05 GEMM of gemm_tcgen05.cu
+// bf16 mode (PHK_PREC_BF16): the three products of every nn.Linear run on the wgmma GEMM of gemm_wgmma.cu
 // (C = A.W^T, bf16 operands K-major, fp32 accumulate -- the dtype flow of torch.autocast(bfloat16)); the operands are
 // converted on the fly from the fp32 activations / master weights:
 //   forward  Y[M,N]  = X.W^T          A = bf16(X) [M,K]        W = bf16(W) [N,K]
@@ -1144,7 +1144,7 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   const int64_t R = (int64_t)b * n, CR = (int64_t)b * L;
   Arena ar{(char*)workspace, workspace_bytes, 0};
   TcScratch tc{nullptr, nullptr, 0};
-  if (prec == PHK_PREC_BF16) {  // operand buffers of the tcgen05 products (activations stay fp32 everywhere else)
+  if (prec == PHK_PREC_BF16) {  // operand buffers of the wgmma products (activations stay fp32 everywhere else)
     tc.elems = tc_scratch_elems(m, R, CR, bce);
     tc.a = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
     tc.b = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));

@@ -5,7 +5,7 @@
 // arg-max rows of the product x . embed^T -- (tokens x K x dim), 309 GFLOP at BASELINE configs[1], more than the encoder.
 //   fp32 (parity):  phk_gemm_f32 into a [rows, K] strip of the caller's scratch + argmax_rows_kernel (first maximum wins,
 //                   like torch.argmax), strip by strip so the similarities never need more than the scratch holds;
-//   bf16:           the fused tcgen05 head (phk_head_sample at temperature 0 = pure argmax, phenaki_pytorch.py:493): the
+//   bf16:           the fused wgmma head (phk_head_sample at temperature 0 = pure argmax, phenaki_pytorch.py:493): the
 //                   [tokens, K] similarities never leave the SM.
 #include "phk_common.cuh"
 

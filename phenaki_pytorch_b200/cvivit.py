@@ -365,7 +365,7 @@ class CViViT(nn.Module):
             recon = self.decode_from_codebook_indices(self.encode_ids(video))
             return recon.squeeze(2) if is_image else recon
         raise NotImplementedError("C-ViViT training losses (reconstruction / GAN / perceptual, cvivit.py:576-671) "
-                                  "are out of scope of the B200 hot path (SURVEY.md section 2 row 8)")
+                                  "are out of scope of the H100 hot path (SURVEY.md section 2 row 8)")
 
     def _decode(self, ids, tokens, b, tp, device, taps=None):
         lib = L.lib()

@@ -138,7 +138,7 @@ class Keep:
         return o
 
     def h(self, tensor):
-        """bf16 copy (the tcgen05 GEMM operand); leading dimension must be a multiple of 8 for TMA."""
+        """bf16 copy (the wgmma GEMM operand); leading dimension must be a multiple of 8 for TMA."""
         if not tensor.is_cuda:
             raise L.PhkError("module parameters must be on a CUDA device (no CPU path): call .cuda() first")
         t = tensor.detach().to(torch.bfloat16).contiguous()

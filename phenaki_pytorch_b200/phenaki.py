@@ -245,7 +245,7 @@ class _TokenTransformer(nn.Module):
                    text_mask=None, video_mask=None, loss_scale=1.0, keep_logits=False, head=None, owner=None,
                    overlap_all_reduce=False):
         """One forward + loss + backward in libphk (phk_maskgit_train_step; ``self.precision`` selects fp32 FFMA or
-        tcgen05 bf16 products, everything else is fp32 in both modes): returns (loss 0-d tensor,
+        wgmma bf16 products, everything else is fp32 in both modes): returns (loss 0-d tensor,
         GradKeep with d(loss_scale * loss)/d(parameter), logits or None).  ``labels`` given: Linear(dim, 1) head + BCE
         with logits (TokenCritic; or ``head`` = SelfCritic.to_pred on this MaskGit, gradients laid out for
         ``owner.parameters()``); otherwise masked cross entropy against ``targets`` at ``token_mask``."""
@@ -651,7 +651,7 @@ class Phenaki(nn.Module):
         self.sync_gradients = True
         # bf16 mode, no critic: ONE C call per demasking iteration with all state in device memory
         # (phk_maskgit_demask_iteration), replayed as ONE CUDA-graph launch per iteration from the third sample() with the
-        # same shapes on (BASELINE north_star: one launch per decode iteration).  Validated on the B200 against the
+        # same shapes on (BASELINE north_star: one launch per decode iteration).  Validated on the H100 against the
         # per-step loop (identical ids: same noise counters).  PHK_STEP_GRAPH=0 restores the per-step loop.
         self.iteration_call = os.environ.get("PHK_STEP_GRAPH", "1") != "0"
         self._iter_bufs = {}
@@ -957,7 +957,7 @@ class Phenaki(nn.Module):
         The returned scalar is connected to the parameters through ``_TrainStepFn``: ``loss.backward()`` fills
         ``p.grad`` with the gradients the hand-written backward kernels computed (phk_maskgit_train_step).
         ``draw_fn(shape, tag)`` (tests) injects the draws 'rand_step' (b,), 'perm' (b, n) and 'gumbel' (b, n, V).
-        ``maskgit.precision`` selects fp32 (parity) or bf16 tensor-core products.  Validated on the B200 against the
+        ``maskgit.precision`` selects fp32 (parity) or bf16 tensor-core products.  Validated on the H100 against the
         reference's autograd loss and every parameter gradient (tests/test_gpu_train.py, both precision modes)."""
         assert not (only_train_generator and only_train_critic)
         assert (videos is not None) ^ (video_codebook_ids is not None), "either raw video or codebook ids"

@@ -1,5 +1,5 @@
 // TEST INFRASTRUCTURE: fiber scheduler of cuda_emu.h.  The kernels themselves are the product's sources (csrc/train.cu,
-// rowops.cu, gemm_simt.cu, attention.cu) compiled by g++; the only stand-in is the tcgen05 GEMM (tensor cores cannot be
+// rowops.cu, gemm_simt.cu, attention.cu) compiled by g++; the only stand-in is the wgmma GEMM (tensor cores cannot be
 // emulated thread by thread), stated below from its include/phk.h contract.
 #include "cuda_emu.h"
 #include <setjmp.h>
@@ -192,7 +192,7 @@ int patchify_ln_tma_launch(const float*, int, int, int, int, int, int, int, int,
                            int, cudaStream_t) { return 1; }
 }  // namespace phk
 // ---------------------------------------------------------------------------------------------------------------------
-// The tcgen05 / TMA entry points (gemm_tcgen05.cu, attention_tc.cu, head_sample.cu) cannot be executed thread by thread;
+// The wgmma / TMA entry points (gemm_wgmma.cu, attention_tc.cu, head_sample.cu) cannot be executed thread by thread;
 // they are represented by their include/phk.h CONTRACTS so that the bf16-mode drivers (weight packing, buffer wiring,
 // the CFG-pair sharing, the masked-rows tail) can run end to end on the CPU.  Numerics: bf16 operands, fp32 accumulation.
 // ---------------------------------------------------------------------------------------------------------------------
@@ -336,7 +336,7 @@ extern "C" int phk_gemm_bf16_qkv(const void* xn, const void* xraw, int64_t lda, 
   });
   return 0;
 }
-// phk_layernorm_cfg / phk_head_sample (head_sample.cu, tcgen05) from their include/phk.h contracts, for the drivers'
+// phk_layernorm_cfg / phk_head_sample (head_sample.cu, wgmma) from their include/phk.h contracts, for the drivers'
 // wiring tests: e = s * norm(x_cond) + (1 - s) * norm(x_null) in bf16; logits = e W^T + bias in fp32, then the REAL
 // phk_sample_tokens kernel (the documented equivalence: same Philox counter layout as phk_sample_tokens with u == NULL)
 extern "C" int phk_layernorm_cfg(const float* xc, const float* xn, const float* g, const float* b, float scale, void* out,
@@ -395,7 +395,7 @@ extern "C" int phk_head_sample(const void* emb, int64_t ld_emb, int64_t emb_rows
 // test hook: 0 = in-order schedule, otherwise the seed of the random block / thread order
 extern "C" void phk_emu_set_shuffle(uint64_t seed) { emu::set_schedule_seed(seed); }
 
-// tcgen05 GEMM contract (include/phk.h): bf16 operands K-major, fp32 accumulate; epilogue 0 fp32 (+bias, +residual, row
+// wgmma GEMM contract (include/phk.h): bf16 operands K-major, fp32 accumulate; epilogue 0 fp32 (+bias, +residual, row
 // map), 1 bf16 (+bias), 2 GEGLU over [64 value | 64 gate] row groups of W -> bf16 [M, N/2]
 extern "C" int phk_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t ldw, void* C, int64_t ldc, int64_t M,
                              int32_t N, int32_t K, const float* bias, const float* residual, int64_t seg_len,

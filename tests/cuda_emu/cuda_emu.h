@@ -170,7 +170,7 @@ void count_launch(int n = 1);
 #define PHK_CUDA(call) do { cudaError_t e__ = (call); if (e__ != cudaSuccess) return (int)e__; } while (0)
 #define PHK_TRY(call) do { int r__ = (call); if (r__ != 0) return r__; } while (0)
 static inline cudaStream_t to_stream(phk_stream_t s) { return reinterpret_cast<cudaStream_t>(s); }
-constexpr int kNumSMs = 148;
+constexpr int kNumSMs = 132;
 enum Family { FAM_PATCHIFY = 0, FAM_LAYERNORM, FAM_GEMM_F32, FAM_GEMM_BF16, FAM_ATTENTION, FAM_PEG, FAM_GEGLU,
               FAM_LFQ, FAM_EMBED, FAM_CPB, FAM_SAMPLE, FAM_TOPK, FAM_CRITIC, FAM_CFG, FAM_COUNT };
 struct Prof {  // defined in api.cu (per-family event timing; the events are no-ops here)

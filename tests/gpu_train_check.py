@@ -17,7 +17,7 @@ from tests import cases as C  # noqa: E402
 
 
 def check_case(name, verbose=True, bf16=False, device="cuda:0"):
-    """bf16=True: tcgen05 products (PHK_PREC_BF16); the bar is then closeness to the fp32 reference (5 % of each
+    """bf16=True: wgmma products (PHK_PREC_BF16); the bar is then closeness to the fp32 reference (5 % of each
     gradient tensor's largest entry), not parity."""
     case = C.TRAIN_CASES[name]
     g = torch.load(os.path.join(ROOT, "tests", "golden", f"train_{name}.pt"), weights_only=False)

@@ -23,7 +23,7 @@ def test_library_is_built_and_exports_every_declared_symbol():
     syms = header_symbols()
     assert len(syms) >= 20
     missing = [s for s in syms if not hasattr(raw, s)]
-    # phk_gemm_bf16 (tcgen05) lands with the tensor-core path; everything else must already resolve
+    # phk_gemm_bf16 (wgmma) lands with the tensor-core path; everything else must already resolve
     assert missing == []
 
 

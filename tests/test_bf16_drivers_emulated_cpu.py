@@ -1,8 +1,8 @@
 """CPU: the bf16-mode parity tests of tests/test_gpu_bf16_mode.py with the DRIVERS executed from the shipped source
-(csrc/api.cu, sample_tail.cu and every plain kernel they launch) and the tcgen05 / TMA kernels represented by their
+(csrc/api.cu, sample_tail.cu and every plain kernel they launch) and the wgmma / TMA kernels represented by their
 include/phk.h contracts (tests/cuda_emu/cuda_emu.cpp: bf16 operands, fp32 accumulation).  What this covers is the host
 logic of bf16 mode -- bf16 weight packing (GEGLU row interleave, padding), buffer wiring, the CFG-pair sharing of the
-first layer, the masked-rows tail of the demasking step -- not the tensor-core kernels themselves, which only the B200
+first layer, the masked-rows tail of the demasking step -- not the tensor-core kernels themselves, which only the H100
 run exercises."""
 import ctypes
 

@@ -1,4 +1,4 @@
-"""GPU: PHK_PREC_BF16 (tcgen05 GEMMs, bf16 operands, fp32 accumulation / residual / LayerNorm / softmax)
+"""GPU: PHK_PREC_BF16 (wgmma GEMMs, bf16 operands, fp32 accumulation / residual / LayerNorm / softmax)
 against the fp32 reference goldens.  This is the dtype flow of the reference under
 torch.autocast(bfloat16) (SURVEY.md H2), so the comparison is reference-fp32 vs bf16 contraction noise.
 
@@ -102,7 +102,7 @@ def test_layernorm_cfg_combination():
 
 @pytest.mark.parametrize("n_tokens,V,dim", [(300, 1000, 128), (2304, 4096, 512), (64, 130, 256)])
 def test_fused_head_kernel_matches_gemm_plus_sample_tokens(n_tokens, V, dim):
-    """phk_head_sample (logits only ever in TMEM) vs phk_gemm_bf16 -> logits -> phk_sample_tokens with the same
+    """phk_head_sample (logits only ever in registers) vs phk_gemm_bf16 -> logits -> phk_sample_tokens with the same
     Philox counters: identical sampled ids (same MMA arithmetic), confidence within 1e-4 (softmax summation order)."""
     lib = L.lib()
     emb = (C.seeded_randn((n_tokens, dim), 310)).bfloat16().to(DEV)

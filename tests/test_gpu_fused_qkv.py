@@ -1,6 +1,6 @@
 """GPU: the fused self-attention operand path of bf16 mode (round 2): phk_gemm_bf16_qkv (q / k,v projections whose
 epilogue writes the l2-normalised, scaled bf16 operands of the attention core, attention.py:146-157), consumed by
-phk_attention_tc_bf16 (4-D tensor maps over token-major rows, V as an MN-major tcgen05 operand) and
+phk_attention_tc_bf16 (4-D tensor maps over token-major rows, V as an MN-major wgmma operand) and
 phk_attention_small_bf16 (temporal transformer, one warp per (sequence, head)) -- against torch fp32 references of the
 same ops computed from the same bf16 inputs."""
 import ctypes as C
@@ -66,9 +66,8 @@ def _core_reference(qn, kvn, n_seq, n, heads, bias=None, causal_slopes=None):
 @pytest.mark.parametrize("n_seq,n,heads,with_bias", [(72, 64, 8, True), (2, 576, 8, True), (1, 200, 4, False), (3, 130, 2, True),
                                                      (8, 576, 8, True), (2, 1024, 8, True), (5, 199, 3, True)])
 def test_attention_tc_on_prenormalised_token_major_operands(n_seq, n, heads, with_bias, variant):
-    """variant 0: probabilities through a shared-memory tile (two CTAs per SM); 1: probabilities in tensor memory, read by
-    P.V as a TMEM A operand (three CTAs per SM).  (8, 576, 8): the MaskGit shape, 320 CTAs; n = 199: bias rows TMA cannot
-    address (direct loads) and a ragged last chunk."""
+    """variant 0 / 1: the values of phk_debug_attention_tc_variant (one kernel serves both).  (8, 576, 8): the MaskGit
+    shape; n = 199: odd bias rows (scalar loads) and a ragged last chunk."""
     L.check(L.lib().phk_debug_attention_tc_variant(variant))
     try:
         _attention_tc_case(n_seq, n, heads, with_bias)

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05/TMEM/TMA bf16 GEMM (phk_gemm_bf16) against torch fp32 matmul of the SAME bf16-rounded
+"""GPU: the wgmma/TMA bf16 GEMM (phk_gemm_bf16) against torch fp32 matmul of the SAME bf16-rounded
 operands (so the only difference is fp32 summation order: tolerance 2e-3 * sqrt(K/512) absolute on O(sqrt(K)) sums)."""
 import pytest
 import torch
@@ -85,7 +85,7 @@ def test_gemm_bf16_geglu_epilogue(M, inner, K):
 
 @pytest.mark.parametrize("n_seq,n,heads,with_bias", [(2, 576, 8, True), (3, 64, 2, True), (1, 200, 4, False), (2, 640, 8, True)])
 def test_attention_tensor_core_matches_oracle(n_seq, n, heads, with_bias):
-    """tcgen05 attention (bf16 operands, fp32 softmax) vs the fp32 oracle core: |err| <= 0.02 on O(1) outputs."""
+    """wgmma attention (bf16 operands, fp32 softmax) vs the fp32 oracle core: |err| <= 0.02 on O(1) outputs."""
     from oracle import phenaki_oracle as O
     dh, I = 64, heads * 64
     q, kv = TC.seeded_randn((n_seq, n, I), 200), TC.seeded_randn((n_seq, n, 2 * I), 201)
@@ -110,7 +110,7 @@ def test_attention_tensor_core_matches_oracle(n_seq, n, heads, with_bias):
 
 @pytest.fixture
 def gemm_mode():
-    """Forces one tcgen05 GEMM variant (1 one-CTA 128x128, 2 CTA pairs 256x128, 3 CTA pairs 256x256) for a test."""
+    """Forces one wgmma GEMM variant (1 one-CTA 128x128, 2 CTA pairs 256x128, 3 CTA pairs 256x256) for a test."""
     lib = L.lib()
     yield lambda m: L.check(lib.phk_debug_gemm_mode(m))
     lib.phk_debug_gemm_mode(-1)

@@ -2,7 +2,7 @@
 (tools/parity_report.py: the functional oracle -- bit-identical to the unmodified reference, tests/golden/make_golden.py
 -- executed on CUDA in eager fp32 and under torch.autocast(bfloat16), the reference's only bf16 path, SURVEY H2).
 
-Bars (measured values of round 2 in profiles/r02/parity_at_size_*.json; the report is also written to
+Bars (the measured values in parentheses are from an earlier build; the report is also written to
 gpurun_out/parity_at_size.json by this test):
   * fp32 parity mode: all 8 cfg2 videos -- LFQ ids identical (a flipped bit tolerated only below a 2e-5 reference margin;
     measured 0 of 73 728); cfg3 logits within 2e-5, identical arg-max; the whole 18-step demasking loop with injected
@@ -54,7 +54,7 @@ def test_cfg2_token_ids_of_all_8_videos_against_both_reference_dtypes():
 
 def test_cfg2_cosine_vq_tokenizer_at_full_codebook_size():
     """SURVEY 8f-3 at size: configs[1] encoder + cosine-sim VectorQuantize with K = 65536 codes (309 GFLOP nearest-code
-    search, fused tcgen05 head in bf16 mode), all 8 videos against the oracle on CUDA."""
+    search, fused wgmma head in bf16 mode), all 8 videos against the oracle on CUDA."""
     import parity_report as R
     rep = _REPORT["cfg2_cosine_vq_K65536"] = R.cfg2_cosine_vq_report(batch=8)
     _save()

@@ -1,7 +1,6 @@
 """GPU: the training step (Phenaki.forward -> phk_maskgit_train_step: forward, loss and the hand-written backward
 kernels of csrc/train.cu) against the reference's autograd loss and gradients (tests/golden/train_*.pt): fp32 mode at
-parity tolerances, bf16 mode (tcgen05 products) within 5 % of each gradient tensor's largest entry.  First run on a B200
-in round 2 (profiles/r02/train_checks_c1.txt, compute-sanitizer clean)."""
+parity tolerances, bf16 mode (wgmma products) within 5 % of each gradient tensor's largest entry."""
 import pytest
 
 from tests import cases as C

@@ -1,4 +1,4 @@
-"""GPU: PHK_PREC_BF16X3 -- fp32-grade nn.Linear products on the tcgen05 tensor cores (operands split into two bf16 terms,
+"""GPU: PHK_PREC_BF16X3 -- fp32-grade nn.Linear products on the wgmma tensor cores (operands split into two bf16 terms,
 one GEMM over K' = 3K) with the parity mode's fp32 LayerNorm / attention core / GEGLU around them.  Bars are the fp32
 parity mode's: token ids identical to the reference goldens, activations / logits / pixels within 2e-4 (+ 2e-4 |ref|).
 At configs[1] / configs[2] sizes: tests/test_gpu_parity_at_size.py."""
@@ -15,7 +15,7 @@ DEV = "cuda"
 
 @pytest.mark.parametrize("M,N,K", [(300, 200, 512), (129, 96, 77), (4608, 512, 1365)])
 def test_split_gemm_matches_fp64_product_to_fp32_grade(M, N, K):
-    """phk_split3 on both sides + one tcgen05 GEMM over 3 Kp == A W^T to ~1e-5 of the row scale (bf16 alone: ~4e-3)."""
+    """phk_split3 on both sides + one wgmma GEMM over 3 Kp == A W^T to ~1e-5 of the row scale (bf16 alone: ~4e-3)."""
     from phenaki_pytorch_b200.modules import split3_weight
     a, w = C.seeded_randn((M, K), 500), C.seeded_randn((N, K), 501) / K ** 0.5
     ref = (a.double() @ w.double().t()).float()

@@ -18,7 +18,7 @@ DEV = "cuda"
 @pytest.mark.parametrize("b,n,k,dim,V", [(4, 576, 100, 512, 4096), (2, 48, 17, 128, 300), (3, 30, 1, 256, 130),
                                          (4, 576, 441, 512, 1024)])
 def test_sample_tail_on_the_masked_rows_only(b, n, k, dim, V):
-    """phk_sample_tail (csrc/sample_tail.cu + the tcgen05 head on the compact rows) against plain torch arithmetic; the
+    """phk_sample_tail (csrc/sample_tail.cu + the wgmma head on the compact rows) against plain torch arithmetic; the
     same body runs on the CPU executor in tests/test_sample_tail_emulated_cpu.py."""
     from tests import tail_cases
     tail_cases.check_exact_k(L.lib(), torch.device(DEV), b, n, k, dim, V, sync=torch.cuda.synchronize)
@@ -58,7 +58,7 @@ def test_fused_sample_step_on_masked_rows_equals_the_all_rows_step():
 
 
 def test_cosine_vq_ids_in_bf16_mode_against_fp32_reference_golden(golden):
-    """lookup_free_quantization=False in bf16 mode: the nearest-code search runs on the fused tcgen05 head at temperature 0
+    """lookup_free_quantization=False in bf16 mode: the nearest-code search runs on the fused wgmma head at temperature 0
     (phk_vq_cosine_ids).  An id may differ from the fp32 reference's only where the reference's similarities of the two
     candidates are within bf16 noise (0.03 in cosine units), and at least 85 % of the ids agree."""
     case, g = C.CVIVIT_CASES["cosine_vq"], golden("cvivit_cosine_vq")

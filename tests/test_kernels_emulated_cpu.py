@@ -2,7 +2,7 @@
 gemm_simt.cu, attention.cu) run a second time with the kernels EXECUTED ON THE CPU by tests/cuda_emu.  Same test
 bodies, same oracle comparisons, same tolerances -- only the device string and the library handle are swapped.
 
-Two purposes: (1) these kernels are validated on the B200 by the -m gpu suite, so their passing here is the check of the
+Two purposes: (1) these kernels are validated on the H100 by the -m gpu suite, so their passing here is the check of the
 executor itself (the training-step tests rely on it); (2) the CPU-only container gets kernel-level coverage of the
 shipped sources (indexing, barriers, edge tiles) before any GPU time is spent."""
 import pytest

@@ -1,6 +1,6 @@
 """CPU: tests/test_gpu_masks_and_self_critic.py a second time with the whole fp32 product path (classes, ctypes tables,
 csrc drivers, every kernel incl. the training step's backward kernels) executed by tests/cuda_emu -- the same bodies and
-bars as on the B200."""
+bars as on the H100."""
 import pytest
 import torch
 

@@ -1,10 +1,10 @@
 """CPU: the module-granularity parity tests of tests/test_gpu_models.py and tests/test_gpu_decode.py (fp32 parity mode)
 run a second time with the WHOLE product path executed on the CPU: the reference-facing classes, the ctypes tables, the
 drivers of csrc/api.cu and every kernel they launch (rowops.cu, gemm_simt.cu, attention.cu), compiled by g++ against
-tests/cuda_emu.  Same test bodies and bars as on the B200: C-ViViT token ids identical to the reference's, logits /
+tests/cuda_emu.  Same test bodies and bars as on the H100: C-ViViT token ids identical to the reference's, logits /
 critic scores / reconstructions within 2e-4, the full demasking loop (with the reference's noise replayed) identical.
 
-What only the GPU run covers: bf16 mode (tcgen05 / TMA kernels), pinned-memory pipelines, CUDA-graph replay, speed."""
+What only the GPU run covers: bf16 mode (wgmma / TMA kernels), pinned-memory pipelines, CUDA-graph replay, speed."""
 import pytest
 import torch
 

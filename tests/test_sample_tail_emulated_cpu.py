@@ -1,7 +1,7 @@
 """CPU (tests/cuda_emu): the masked-rows-only tail of a demasking iteration (csrc/sample_tail.cu: compaction, gathered
 norm_out + guidance, head on the compact rows, scatter) executed from the shipped source, against plain torch
-arithmetic.  The tcgen05 head itself (phk_head_sample) is represented by its contract here -- a bf16-operand product
-followed by the REAL phk_sample_tokens kernel; on the B200 the same checks run through the real head
+arithmetic.  The wgmma head itself (phk_head_sample) is represented by its contract here -- a bf16-operand product
+followed by the REAL phk_sample_tokens kernel; on the H100 the same checks run through the real head
 (tests/test_gpu_zz_after_last_gpu_call.py)."""
 import pytest
 import torch

@@ -2,7 +2,7 @@
 gemm_simt.cu, attention.cu) -- compiled by g++ against tests/cuda_emu (every CUDA thread a fiber, __syncthreads / warp
 shuffles as barriers) and EXECUTED on the CPU through the product's own Python path (MaskGit.train_step -> ctypes
 tables -> phk_maskgit_train_step), against the reference's autograd loss and gradients (tests/golden/train_*.pt).
-Every kernel of the fp32 step is the shipped source; the one stand-in is the tcgen05 GEMM of the bf16 mode (its
+Every kernel of the fp32 step is the shipped source; the one stand-in is the wgmma GEMM of the bf16 mode (its
 include/phk.h contract stated on the CPU).  That the GPU-validated forward kernels give the reference's numbers here
 too is the evidence that the executor is faithful."""
 import pytest
@@ -135,7 +135,7 @@ def test_emulated_step_with_a_gradient_scale_and_without_text(golden, on_cpu):
 
 @pytest.mark.parametrize("name", ["generator", "with_critic"])
 def test_emulated_bf16_mode_step_tracks_the_fp32_reference(golden, on_cpu, name):
-    """PHK_PREC_BF16: forward / dgrad / wgrad products through the tcgen05 GEMM contract (here its CPU stand-in: bf16
+    """PHK_PREC_BF16: forward / dgrad / wgrad products through the wgmma GEMM contract (here its CPU stand-in: bf16
     operands, fp32 accumulation) with operands cast / transposed on the fly by the shipped kernels.  The dtype flow is
     torch.autocast's, so the bar is closeness to the fp32 reference: loss within 2 %, every gradient tensor within 5 % of
     its largest entry and at a cosine similarity above 0.995."""

@@ -1,5 +1,5 @@
 """CPU: PHK_PREC_BF16X3 (split-bf16 tensor-core mode) through the product path on the CPU executor: weight packs
-[hi | lo | hi], the activation split kernel [hi | hi | lo] (rowops.cu, executed) and the drivers' wiring; the tcgen05
+[hi | lo | hi], the activation split kernel [hi | hi | lo] (rowops.cu, executed) and the drivers' wiring; the wgmma
 GEMM itself is represented by its contract (bf16 operands, fp32 accumulation).  Bars: the fp32 parity mode's -- token ids
 identical to the reference's, logits within 2e-4 -- because hi + lo carries 16 mantissa bits of every operand."""
 import pytest

@@ -1,4 +1,4 @@
-"""Per-phase clock64 stamps of the tcgen05 GEMM (debug): python tools/gemm_trace.py M N K [epilogue]"""
+"""Per-phase clock64 stamps of the wgmma GEMM (debug): python tools/gemm_trace.py M N K [epilogue]"""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch

@@ -1,4 +1,4 @@
-"""The same-box GPU bar (SURVEY 2a / 8d, BASELINE.md 4.4): the reference's own PyTorch path on the B200 -- the oracle
+"""The same-box GPU bar (SURVEY 2a / 8d, BASELINE.md 4.4): the reference's own PyTorch path on the GPU -- the oracle
 port (same ATen ops as the reference modules; /root/reference does not exist on the GPU box) on CUDA, eager fp32 (torch
 defaults) and under torch.autocast(bfloat16) -- for configs[1] (C-ViViT encode) and configs[2] (18-step demasking loop).
 bench.py imports `encode_leg` / `maskgit_leg`; standalone:  python tools/ref_gpu_bench.py
