@@ -348,9 +348,15 @@ int phk_token_embed(const int64_t* ids, const float* tok, const float* pos, floa
 /* CFG + gumbel argmax + confidence, one pass over the vocabulary
  * (phenaki_pytorch.py:161, 83-93, 506-509, 547-550):
  *   l = null + (cond-null)*cond_scale   (null==NULL or cond_scale==1: l = cond)
- *   pred = argmax_v( l/max(T,1e-10) - log(-log(u+1e-10)+1e-10) ), first index on ties
+ *   pred = argmax_v( l/max(T,1e-10) + g ), first index on ties
  *   ids = mask ? pred : ids ;  score = mask ? 1 - softmax(l)[pred] : -1e4
- * u: uniform draws [rows, V] (parity mode) or NULL -> in-kernel Philox4x32-10(seed, offset).
+ * u: uniform draws [rows, V] (parity mode): g = -log(-log(u+1e-10)+1e-10), the reference's guarded op sequence; or
+ * u == NULL: in-kernel gumbel noise, draw v of token row r:
+ *   Philox4x32 with 7 rounds (Salmon et al., SC'11; multipliers 0xD2511F53 / 0xCD9E8D57, key increments
+ *   0x9E3779B9 / 0xBB67AE85), key = (seed lo 32, seed hi 32), counter = (c lo 32, c hi 32, 0, 0),
+ *   c = offset + r*ceil(V/4) + v/4 (64-bit, wrapping); the draw is output word v % 4;
+ *   u = (2*(draw >> 9) + 1) / 2^24 (the top 23 bits, strictly inside (0, 1), no guards); g = -ln(-ln(u)), evaluated
+ *   in fp32 with lg2.approx.  One call uses the counters [offset, offset + rows*ceil(V/4)).
  * seg_*: token row r reads logits row (r/seg_len)*seg_stride + seg_off + r%seg_len, i.e. the
  * `logits[:, prime_len:]` slice of a primed sample (:503-504); seg_len<=0: identity. */
 int phk_sample_tokens(const float* cond, const float* null_logits, int64_t ld, const float* u,
@@ -476,7 +482,8 @@ int phk_layernorm_cfg(const float* x_cond, const float* x_null, const float* gam
                       float cond_scale, void* out_bf16, int64_t rows, int32_t dim, phk_stream_t s);
 
 /* Fused logits head for the sampling loop (phenaki_pytorch.py:213 + 83-93 + 506-509 + 547-550): a wgmma GEMM whose
- * epilogue applies bias and gumbel noise (in-kernel Philox, same counter layout as phk_sample_tokens with u == NULL)
+ * epilogue applies bias and gumbel noise (the in-kernel noise of phk_sample_tokens with u == NULL, token row r = row r
+ * of emb: the same (seed, offset, r, v) gives the same draw)
  * and reduces argmax / online softmax over the vocabulary straight out of the accumulator registers, so the (b, n, V) logits never exist
  * in memory.  emb bf16 [emb_rows >= n_tokens, dim <= 512] = guided embeddings (phk_layernorm_cfg, or plain norm_out
  * rows when there is no guidance); the 128-token A panel stays resident in shared memory, W streams through TMA.
@@ -546,7 +553,9 @@ int phk_rng_advance(uint64_t* rng_state, uint64_t stride, phk_stream_t s);
 /* One WHOLE demasking iteration (phenaki_pytorch.py:485-509, 547-550) as one call:
  *   [k_remask > 0:  mask = scatter(topk(scores, k_remask)); ids = where(mask, mask_id, ids)]      (phk_topk_mask)
  *   -> MaskGit forward of the CFG pair on ids -> tail on the masked rows -> ids, pred, scores updated IN PLACE
- *   -> rng_state[1] += b*n*ceil(V/4) + 1 (the noise counters the iteration consumed).
+ *   -> rng_state[1] += round_up(b*n*ceil(V/4) + 1, 4) (the noise counters of one V-wide draw over all b*n tokens, one
+ *      more, rounded up to the multiple of 4 torch's generator offsets take; the tail draws on compact row i*k + j,
+ *      i.e. within the first b*k*ceil(V/4) of them).
  * k_remask == 0 is the first iteration (every token masked: mask must be all ones).  rng_state: device uint64[2]
  * {seed, offset}.  With PHK_STEP_GRAPH=1 the launch sequence is captured into a CUDA graph the second time the same
  * arguments are seen (same table contents, pointers, shape, scalars) and later calls are ONE cudaGraphLaunch -- the

@@ -118,9 +118,10 @@ __device__ __forceinline__ float gelu_erf(float x) {
 }
 
 // ---- in-kernel sampling noise (statistical mode of the demasking loop: phk_sample_tokens without injected draws, the
-// fused logits head).  Counter-based: Philox4x32 keyed by the torch CUDA seed, counter = noise offset + (token, v / 4).
+// fused logits head), as include/phk.h (phk_sample_tokens) defines it.  Counter-based: Philox4x32 keyed by the torch CUDA
+// seed, counter = noise offset + token * ceil(V / 4) + v / 4, draw v % 4 of the block.
 // 7 rounds: the smallest count the Random123 authors report as passing BigCrush (10 is their safety-margin default); the
-// generator sits in the logits head's epilogue, which is instruction-bound (ncu, profiles/), at 4 IMAD + 2 LOP3 per round.
+// generator sits in the logits head's epilogue, which is instruction-bound, at 4 IMAD + 2 LOP3 per round.
 constexpr int kNoiseRounds = 7;
 template <int ROUNDS>
 __device__ __forceinline__ void philox4x32(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1,
