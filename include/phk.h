@@ -524,70 +524,58 @@ int phk_sample_tail_rows(const float* x_cond, const float* x_null, const float* 
                          const uint8_t* mask, int64_t* ids, int64_t* pred_out, float* score_out, int32_t src_stride,
                          int32_t src_off, void* scratch, int64_t scratch_bytes, phk_stream_t s);
 
-/* One demasking iteration's network half for the sampling loop (phenaki_pytorch.py:495-509, 547-550): MaskGit forward
- * of the CFG pair (as phk_maskgit_forward with cfg_pair=1) + phk_head_sample.  bf16 weights required, cond_scale != 1,
- * no priming.  ids_in (b,n) = current (partly masked) ids; ids/pred_out/score_out/mask as phk_sample_tokens.
+/* One demasking iteration's network half for the sampling loop (phenaki_pytorch.py:493-509, 547-550): MaskGit forward
+ * of the CFG pair (as phk_maskgit_forward with cfg_pair=1) + phk_head_sample.  bf16 weights required, cond_scale != 1.
+ * ids_in (b, n) = current (partly masked) ids; with a prime prefix (Phenaki.sample(prime_frames=...), the scene chains
+ * of make_video) the prime_len prime ids come first, n = prime_len + sampled tokens.  mask / ids / pred_out / score_out
+ * (b, n - prime_len) cover the sampled tokens, as phk_sample_tokens.
  * masked_per_seq: the number of set mask entries of EVERY sequence when the caller knows it (the k it gave
- * phk_topk_mask), else 0.  With 0 < masked_per_seq < n the final LayerNorm, the guidance and the logits head run on the
- * masked rows only (phk_sample_tail); pred_out is then the current id at unmasked positions. */
+ * phk_topk_mask), else 0; prime_len > 0 requires it.  With 0 < masked_per_seq < n the final LayerNorm, the guidance and
+ * the logits head run on the masked rows only (phk_sample_tail); pred_out is then the current id at unmasked positions. */
 int64_t phk_maskgit_sample_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L);
 int phk_maskgit_sample_step(const phk_maskgit_t* m, const int64_t* ids_in, int32_t b, int32_t n, int32_t pt,
                             int32_t ph, int32_t pw, const float* ctx_kv, int32_t L, const uint8_t* text_mask,
-                            const uint8_t* video_mask, const float* pos_bias, float cond_scale, float temperature,
-                            uint64_t seed, uint64_t offset, const uint8_t* mask, int64_t* ids, int64_t* pred_out,
-                            float* score_out, int32_t masked_per_seq, void* workspace, int64_t workspace_bytes,
+                            const float* pos_bias, float cond_scale, float temperature, uint64_t seed, uint64_t offset,
+                            const uint8_t* mask, int64_t* ids, int64_t* pred_out, float* score_out,
+                            int32_t masked_per_seq, int32_t prime_len, void* workspace, int64_t workspace_bytes,
                             phk_stream_t s);
-/* With a prime prefix (Phenaki.sample(prime_frames=...), the scene chains of make_video): ids_in (b, n) = prime ids
- * followed by the tokens being sampled, n = prime_len + sampled tokens; mask / ids / pred_out / score_out
- * (b, n - prime_len) cover the sampled tokens; masked_per_seq > 0 is required (the head runs on the masked rows only). */
-int phk_maskgit_sample_step_primed(const phk_maskgit_t* m, const int64_t* ids_in, int32_t b, int32_t n, int32_t pt,
-                                   int32_t ph, int32_t pw, const float* ctx_kv, int32_t L, const uint8_t* text_mask,
-                                   const float* pos_bias, float cond_scale, float temperature, uint64_t seed,
-                                   uint64_t offset, const uint8_t* mask, int64_t* ids, int64_t* pred_out, float* score_out,
-                                   int32_t masked_per_seq, int32_t prime_len, void* workspace, int64_t workspace_bytes,
-                                   phk_stream_t s);
 
 /* rng_state[1] += stride on the stream (device-resident noise key, see phk_head_sample_rng) */
 int phk_rng_advance(uint64_t* rng_state, uint64_t stride, phk_stream_t s);
 
-/* One WHOLE demasking iteration (phenaki_pytorch.py:485-509, 547-550) as one call:
+/* One WHOLE demasking iteration (phenaki_pytorch.py:478-550) as one call, for every kind of sample: no critic, a
+ * TokenCritic, a SelfCritic, each with or without a prime prefix (make_video's scene chains):
  *   [k_remask > 0:  mask = scatter(topk(scores, k_remask)); ids = where(mask, mask_id, ids)]      (phk_topk_mask)
- *   -> MaskGit forward of the CFG pair on ids -> tail on the masked rows -> ids, pred, scores updated IN PLACE
+ *   -> ids copied behind the prime ids in token_in -> MaskGit forward of the CFG pair -> tail on the masked rows
+ *      -> ids, pred, scores updated IN PLACE
  *   -> rng_state[1] += round_up(b*n*ceil(V/4) + 1, 4) (the noise counters of one V-wide draw over all b*n tokens, one
  *      more, rounded up to the multiple of 4 torch's generator offsets take; the tail draws on compact row i*k + j,
  *      i.e. within the first b*k*ceil(V/4) of them).
+ *   -> unless skip_critic: ids -> token_in, critic forward of the CFG pair, scores = head(cond, null, cond_scale) +
+ *      noise_K * (u - 0.5) * noise_mult (:534-545).
+ * skip_critic: 1: no critic half (the final iteration, or a sample without a critic).
+ * No critic: skip_critic = 1 on every call; scores stay the MaskGit's logit confidence (:547-550).
+ * TokenCritic: critic is a TokenCritic table (is_critic, the MaskGit's width), ctx via critic_ctx_kv (or NULL: no cross
+ * attention), head_w / head_b its own.
+ * SelfCritic: critic == NULL, the MaskGit's own embeddings under head_w / head_b (fp32 [dim], [1]).
+ * critic_noise: [b, n] uniform draws the caller refreshes before every call (device buffer at a stable address), or NULL.
+ * Prime prefix: token_in [b, prime_len + n] int64 holds the prime ids in the first prime_len columns (written once by the
+ * caller); with prime_len == 0 pass token_in == ids.  pt*ph*pw == prime_len + n.
  * k_remask == 0 is the first iteration (every token masked: mask must be all ones).  rng_state: device uint64[2]
  * {seed, offset}.  With PHK_STEP_GRAPH=1 the launch sequence is captured into a CUDA graph the second time the same
  * arguments are seen (same table contents, pointers, shape, scalars) and later calls are ONE cudaGraphLaunch -- the
  * noise key and the token state live in device memory, so nothing that changes between calls is baked in.  Buffers
- * must therefore be stable across calls.  bf16 weights, cond_scale != 1, no priming (as phk_maskgit_sample_step). */
-int phk_maskgit_demask_iteration(const phk_maskgit_t* m, int64_t* ids, uint8_t* mask, float* scores, int64_t* pred,
-                                 int32_t b, int32_t n, int32_t pt, int32_t ph, int32_t pw, const float* ctx_kv, int32_t L,
+ * must therefore be stable across calls.  bf16 weights, cond_scale != 1 (as phk_maskgit_sample_step). */
+int64_t phk_maskgit_demask_iteration_workspace_bytes(const phk_maskgit_t* m, const phk_maskgit_t* critic, int32_t b,
+                                                     int32_t n_total, int32_t L);
+int phk_maskgit_demask_iteration(const phk_maskgit_t* m, const phk_maskgit_t* critic, const float* head_w,
+                                 const float* head_b, int64_t* token_in, int64_t* ids, uint8_t* mask, float* scores,
+                                 int64_t* pred, int32_t b, int32_t n, int32_t prime_len, int32_t pt, int32_t ph,
+                                 int32_t pw, const float* ctx_kv, const float* critic_ctx_kv, int32_t L,
                                  const uint8_t* text_mask, const float* pos_bias, float cond_scale, float temperature,
-                                 uint64_t* rng_state, int32_t k_remask, void* workspace, int64_t workspace_bytes,
+                                 uint64_t* rng_state, int32_t k_remask, const float* critic_noise, float noise_K,
+                                 float noise_mult, int32_t skip_critic, void* workspace, int64_t workspace_bytes,
                                  phk_stream_t s);
-
-/* The iteration of a sample WITH a critic and / or a prime prefix (phenaki_pytorch.py:478-550; make_video's scene chains),
- * one call, replayed as a CUDA graph like phk_maskgit_demask_iteration:
- *   [k_remask > 0: phk_topk_mask on `scores`] -> ids copied behind the prime ids in token_in -> MaskGit forward of the CFG
- *   pair + tail on the masked rows: ids / pred / scores updated in place -> rng_state[1] += stride
- *   -> unless `last`: ids -> token_in, critic forward of the CFG pair, scores = head(cond, null, cond_scale) +
- *      noise_K * (u - 0.5) * noise_mult (:534-545).
- * token_in [b, prime_len + n] int64: prime ids in the first prime_len columns (written once by the caller); with
- * prime_len == 0 pass token_in == ids.  pt*ph*pw == prime_len + n.  critic: a TokenCritic table (is_critic), ctx via
- * critic_ctx_kv (or NULL: no cross attention); critic == NULL: SelfCritic -- the MaskGit's own embeddings under head_w /
- * head_b (fp32 [dim], [1]).  critic_noise: [b, n] uniform draws the caller refreshes before every call (device buffer at a
- * stable address), or NULL.  Same buffer-stability rule as phk_maskgit_demask_iteration; bf16 weights, cond_scale != 1. */
-int64_t phk_maskgit_demask_iteration_critic_workspace_bytes(const phk_maskgit_t* m, const phk_maskgit_t* critic, int32_t b,
-                                                            int32_t n_total, int32_t L);
-int phk_maskgit_demask_iteration_critic(const phk_maskgit_t* m, const phk_maskgit_t* critic, const float* head_w,
-                                        const float* head_b, int64_t* token_in, int64_t* ids, uint8_t* mask, float* scores,
-                                        int64_t* pred, int32_t b, int32_t n, int32_t prime_len, int32_t pt, int32_t ph,
-                                        int32_t pw, const float* ctx_kv, const float* critic_ctx_kv, int32_t L,
-                                        const uint8_t* text_mask, const float* pos_bias, float cond_scale, float temperature,
-                                        uint64_t* rng_state, int32_t k_remask, const float* critic_noise, float noise_K,
-                                        float noise_mult, int32_t last, void* workspace, int64_t workspace_bytes,
-                                        phk_stream_t s);
 
 /* tests / A-B runs: 1 = phk_maskgit_demask_iteration replays a CUDA graph, 0 = eager, < 0 = the PHK_STEP_GRAPH default */
 int phk_debug_step_graph(int32_t on);

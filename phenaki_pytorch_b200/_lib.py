@@ -160,14 +160,12 @@ PROTOTYPES = {
     "phk_layernorm_cfg": [vp, vp, vp, vp, f32, vp, i64, i32, vp],
     "phk_head_sample": [vp, i64, i64, vp, i64, vp, i32, i32, i32, f32, u64, u64, vp, vp, vp, vp, vp, i64, vp],
     "phk_maskgit_sample_workspace_bytes": [C.POINTER(MaskgitT), i32, i32, i32],
-    "phk_maskgit_demask_iteration_critic_workspace_bytes": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), i32, i32, i32],
-    "phk_maskgit_sample_step": [C.POINTER(MaskgitT), vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, vp, f32, f32, u64,
-                                u64, vp, vp, vp, vp, i32, vp, i64, vp],
+    "phk_maskgit_demask_iteration_workspace_bytes": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), i32, i32, i32],
+    "phk_maskgit_sample_step": [C.POINTER(MaskgitT), vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, f32, f32, u64, u64, vp,
+                                vp, vp, vp, i32, i32, vp, i64, vp],
     "phk_sample_tail_scratch_bytes": [i32, i32, i32],
     "phk_sample_tail_rows": [vp, vp, vp, vp, f32, vp, i64, vp, i32, i32, i32, i32, i32, f32, u64, u64, vp, vp, vp, vp, vp, i32,
                              i32, vp, i64, vp],
-    "phk_maskgit_sample_step_primed": [C.POINTER(MaskgitT), vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, f32, f32, u64, u64,
-                                       vp, vp, vp, vp, i32, i32, vp, i64, vp],
     "phk_sample_tail": [vp, vp, vp, vp, f32, vp, i64, vp, i32, i32, i32, i32, i32, f32, u64, u64, vp, vp, vp, vp, vp, vp,
                         i64, vp],
     "phk_head_sample_rng": [vp, i64, i64, vp, i64, vp, i32, i32, i32, f32, u64, u64, vp, vp, vp, vp, vp, vp, i64, vp],
@@ -175,10 +173,8 @@ PROTOTYPES = {
     "phk_debug_step_graph": [i32],
     "phk_vq_cosine_scratch_bytes": [i64, i32, i32],
     "phk_vq_cosine_ids": [vp, vp, vp, vp, i64, i32, i32, vp, i64, i32, vp],
-    "phk_maskgit_demask_iteration": [C.POINTER(MaskgitT), vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, f32, f32,
-                                     vp, i32, vp, i64, vp],
-    "phk_maskgit_demask_iteration_critic": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), vp, vp, vp, vp, vp, vp, vp, i32, i32, i32,
-                                            i32, i32, i32, vp, vp, i32, vp, vp, f32, f32, vp, i32, vp, f32, f32, i32, vp, i64, vp],
+    "phk_maskgit_demask_iteration": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), vp, vp, vp, vp, vp, vp, vp, i32, i32, i32,
+                                     i32, i32, i32, vp, vp, i32, vp, vp, f32, f32, vp, i32, vp, f32, f32, i32, vp, i64, vp],
     "phk_maskgit_forward": [C.POINTER(MaskgitT), vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, i32, i32, vp, vp,
                             vp, i64, i32, vp],
     "phk_maskgit_train_workspace_bytes": [C.POINTER(MaskgitT), i32, i32, i32, i32, i32],
@@ -186,7 +182,7 @@ PROTOTYPES = {
                                vp, vp, f32, vp, vp, vp, i64, i32, vp],
 }
 _RESTYPES = {"phk_attention_tc_scratch_bytes": i64, "phk_head_sample_scratch_bytes": i64,
-             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_critic_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
+             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
              "phk_cvivit_workspace_bytes": i64, "phk_cvivit_decode_workspace_bytes": i64, "phk_maskgit_workspace_bytes": i64}
 
 FAMILIES = ["patchify_ln", "layernorm", "gemm_f32", "gemm_bf16", "attention", "peg", "geglu", "lfq", "embed",

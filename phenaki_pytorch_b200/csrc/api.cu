@@ -392,7 +392,7 @@ static int check_transformer(const phk_transformer_t* T) {
 
 using namespace phk;
 
-extern "C" int phk_version(void) { return 100; }
+extern "C" int phk_version(void) { return 101; }
 extern "C" const char* phk_last_error(void) { return g_err; }
 extern "C" int64_t phk_launch_count(void) { return g_launches.load(); }
 
@@ -970,10 +970,10 @@ extern "C" int phk_maskgit_forward(const phk_maskgit_t* m, const int64_t* ids, i
   return 0;
 }
 
-// One demasking iteration's network half, fully fused for the sampling loop (phenaki_pytorch.py:495-509, 547-550):
+// One demasking iteration's network half, fully fused for the sampling loop (phenaki_pytorch.py:493-509, 547-550):
 // MaskGit forward for the CFG pair, then logits head + CFG + gumbel argmax + confidence in ONE GEMM kernel whose
-// epilogue reduces over the vocabulary -- the (2b, n, V) logits are never written.  bf16 mode, cond_scale != 1,
-// no priming (those cases use phk_maskgit_forward + phk_sample_tokens).
+// epilogue reduces over the vocabulary -- the (2b, n, V) logits are never written.  bf16 mode, cond_scale != 1; with a
+// prime prefix the head runs on the sampled tokens only.
 extern "C" int64_t phk_maskgit_sample_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L) {
   if (!m || b <= 0 || n <= 0) return -1;
   const int64_t tokens = (int64_t)b * n;
@@ -986,7 +986,7 @@ extern "C" int64_t phk_maskgit_sample_workspace_bytes(const phk_maskgit_t* m, in
 
 static int sample_step_impl(const phk_maskgit_t* m, const int64_t* ids_in, int32_t b, int32_t n, int32_t pt,
                             int32_t ph, int32_t pw, const float* ctx_kv, int32_t L,
-                            const uint8_t* text_mask, const uint8_t* video_mask, const float* pos_bias,
+                            const uint8_t* text_mask, const float* pos_bias,
                             float cond_scale, float temperature, uint64_t seed, uint64_t offset, const uint64_t* rng_state,
                             const uint8_t* mask, int64_t* ids, int64_t* pred_out, float* score_out,
                             int32_t masked_per_seq, int32_t prime_len, void* workspace, int64_t workspace_bytes,
@@ -1036,7 +1036,6 @@ static int sample_step_impl(const phk_maskgit_t* m, const int64_t* ids_in, int32
   c.seq = SeqView{2 * b, 1, n, n, 0, 1};
   c.pegB = 2 * b; c.pegT = pt; c.pegH = ph; c.pegW = pw; c.peg_layout = 0;
   c.attn_bias = m->has_bias ? pos_bias : nullptr;
-  c.self_mask = video_mask; c.self_mask_mod = b;
   c.ctx_kv = ctx_kv; c.ctx_b = b; c.ctx_L = L; c.ctx_mask = text_mask; c.ctx_mask_off_from = b;
   c.prec = PHK_PREC_BF16; c.lin = Lin{PHK_PREC_BF16, nullptr, 0}; c.out_cfg = emb_h; c.cfg_scale = cond_scale;
   c.dup_halves = 1;  // phk_token_embed wrote the same embeddings for both halves
@@ -1051,26 +1050,16 @@ static int sample_step_impl(const phk_maskgit_t* m, const int64_t* ids_in, int32
                              seed, offset, rng_state, mask, ids, pred_out, score_out, hsc, hb, s);
 }
 
+// ids_in (b, n) = prime ids followed by the tokens being sampled (prime_len == 0: no prefix; prime_len > 0:
+// Phenaki.sample(prime_frames=...), make_video's scene chains); mask / ids / pred_out / score_out (b, n - prime_len) cover
+// the sampled tokens.
 extern "C" int phk_maskgit_sample_step(const phk_maskgit_t* m, const int64_t* ids_in, int32_t b, int32_t n, int32_t pt,
-                                       int32_t ph, int32_t pw, const float* ctx_kv, int32_t L,
-                                       const uint8_t* text_mask, const uint8_t* video_mask, const float* pos_bias,
-                                       float cond_scale, float temperature, uint64_t seed, uint64_t offset,
-                                       const uint8_t* mask, int64_t* ids, int64_t* pred_out, float* score_out,
-                                       int32_t masked_per_seq, void* workspace, int64_t workspace_bytes,
-                                       phk_stream_t s) {
-  return sample_step_impl(m, ids_in, b, n, pt, ph, pw, ctx_kv, L, text_mask, video_mask, pos_bias, cond_scale, temperature,
-                          seed, offset, nullptr, mask, ids, pred_out, score_out, masked_per_seq, 0, workspace, workspace_bytes, s);
-}
-
-// The same with a prime prefix (Phenaki.sample(prime_frames=...), make_video's scene chains): ids_in (b, n) = prime ids
-// followed by the tokens being sampled; mask / ids / pred_out / score_out (b, n - prime_len) cover the sampled tokens.
-extern "C" int phk_maskgit_sample_step_primed(const phk_maskgit_t* m, const int64_t* ids_in, int32_t b, int32_t n, int32_t pt,
-                                              int32_t ph, int32_t pw, const float* ctx_kv, int32_t L,
-                                              const uint8_t* text_mask, const float* pos_bias, float cond_scale,
-                                              float temperature, uint64_t seed, uint64_t offset, const uint8_t* mask,
-                                              int64_t* ids, int64_t* pred_out, float* score_out, int32_t masked_per_seq,
-                                              int32_t prime_len, void* workspace, int64_t workspace_bytes, phk_stream_t s) {
-  return sample_step_impl(m, ids_in, b, n, pt, ph, pw, ctx_kv, L, text_mask, nullptr, pos_bias, cond_scale, temperature, seed,
+                                       int32_t ph, int32_t pw, const float* ctx_kv, int32_t L, const uint8_t* text_mask,
+                                       const float* pos_bias, float cond_scale, float temperature, uint64_t seed,
+                                       uint64_t offset, const uint8_t* mask, int64_t* ids, int64_t* pred_out,
+                                       float* score_out, int32_t masked_per_seq, int32_t prime_len, void* workspace,
+                                       int64_t workspace_bytes, phk_stream_t s) {
+  return sample_step_impl(m, ids_in, b, n, pt, ph, pw, ctx_kv, L, text_mask, pos_bias, cond_scale, temperature, seed,
                           offset, nullptr, mask, ids, pred_out, score_out, masked_per_seq, prime_len, workspace,
                           workspace_bytes, s);
 }
@@ -1079,17 +1068,11 @@ extern "C" int phk_maskgit_sample_step_primed(const phk_maskgit_t* m, const int6
 // Everything that changes between calls lives in device memory (ids / mask / scores / pred are updated in place, the
 // noise key is rng_state), so the launch sequence is a pure function of the arguments and a captured graph stays valid:
 // same scheme as phk_cvivit_encode (first sighting of a key eager, second captured, then one cudaGraphLaunch).
-static int demask_iteration_impl(const phk_maskgit_t* m, int64_t* ids, uint8_t* mask, float* scores, int64_t* pred,
-                                 int32_t b, int32_t n, int32_t pt, int32_t ph, int32_t pw, const float* ctx_kv, int32_t L,
-                                 const uint8_t* text_mask, const float* pos_bias, float cond_scale, float temperature,
-                                 uint64_t* rng_state, int32_t k_remask, void* workspace, int64_t workspace_bytes,
-                                 phk_stream_t s) {
-  if (k_remask > 0) PHK_TRY(phk_topk_mask(scores, b, n, k_remask, mask, ids, (int64_t)m->num_tokens, s));
-  PHK_TRY(sample_step_impl(m, ids, b, n, pt, ph, pw, ctx_kv, L, text_mask, nullptr, pos_bias, cond_scale, temperature, 0, 0,
-                           rng_state, mask, ids, pred, scores, k_remask > 0 ? k_remask : n, 0, workspace, workspace_bytes, s));
-  // counters of one V-wide draw, rounded up to a multiple of 4 (phenaki.py: _noise_stride)
-  const uint64_t stride = ((uint64_t)b * (uint64_t)n * (uint64_t)((m->num_tokens + 3) / 4) + 1 + 3) / 4 * 4;
-  return phk_rng_advance(rng_state, stride, s);
+
+// Philox counters one iteration reserves: one V-wide draw over all b*n sampled tokens, one more, rounded up to the
+// multiple of 4 torch's generator offsets take.  phenaki.py:_noise_stride is the same formula on the host side.
+static uint64_t noise_stride(int32_t b, int32_t n, int32_t V) {
+  return ((uint64_t)b * (uint64_t)n * (uint64_t)((V + 3) / 4) + 1 + 3) / 4 * 4;
 }
 
 static std::atomic<int> g_step_graph{-1};  // -1: PHK_STEP_GRAPH from the environment; 0 / 1: phk_debug_step_graph
@@ -1103,7 +1086,7 @@ static int step_graphs_enabled() {
 // tests / A-B runs: 1 replays phk_maskgit_demask_iteration as a CUDA graph, 0 keeps it eager, < 0 back to PHK_STEP_GRAPH
 extern "C" int phk_debug_step_graph(int32_t on) { g_step_graph.store(on < 0 ? -1 : (on ? 1 : 0)); return 0; }
 
-// Launch-sequence cache shared by the iteration entries: `key` identifies the call (table contents, every pointer and
+// Launch-sequence cache of phk_maskgit_demask_iteration: `key` identifies the call (table contents, every pointer and
 // scalar), `run(stream)` issues the launches.  First sighting of a key: eager; second: captured; later: one cudaGraphLaunch.
 template <typename Run>
 static int replay_or_capture(uint64_t key, phk_stream_t s, Run&& run) {
@@ -1155,61 +1138,33 @@ static int replay_or_capture(uint64_t key, phk_stream_t s, Run&& run) {
   return 0;
 }
 
-extern "C" int phk_maskgit_demask_iteration(const phk_maskgit_t* m, int64_t* ids, uint8_t* mask, float* scores,
-                                            int64_t* pred, int32_t b, int32_t n, int32_t pt, int32_t ph, int32_t pw,
-                                            const float* ctx_kv, int32_t L, const uint8_t* text_mask, const float* pos_bias,
-                                            float cond_scale, float temperature, uint64_t* rng_state, int32_t k_remask,
-                                            void* workspace, int64_t workspace_bytes, phk_stream_t s) {
-  PHK_REQUIRE(m && ids && mask && scores && pred && rng_state && workspace, PHK_E_ARG, "maskgit_demask_iteration: null pointer");
-  PHK_REQUIRE(k_remask >= 0 && k_remask <= n, PHK_E_ARG, "maskgit_demask_iteration: k_remask out of range");
-  auto run = [&](phk_stream_t st) {
-    return demask_iteration_impl(m, ids, mask, scores, pred, b, n, pt, ph, pw, ctx_kv, L, text_mask, pos_bias, cond_scale,
-                                 temperature, rng_state, k_remask, workspace, workspace_bytes, st);
-  };
-  if (!step_graphs_enabled() || !pos_bias || g_prof_on.load(std::memory_order_relaxed)) return run(s);
-  int dev = 0;
-  PHK_CUDA(cudaGetDevice(&dev));
-  // key: table contents + every pointer and scalar of the call (a 64-bit FNV of them; the values behind the pointers
-  // -- token state, noise key, weights -- are read at replay time)
-  uint64_t key = fnv(m, sizeof(*m), 0xcbf29ce484222325ull);
-  key = hash_transformer(m->transformer, key);
-  const void* ptrs[] = {ids, mask, scores, pred, ctx_kv, text_mask, pos_bias, rng_state, workspace};
-  key = fnv(ptrs, sizeof(ptrs), key);
-  const int64_t ints[] = {b, n, pt, ph, pw, L, k_remask, dev, workspace_bytes};
-  key = fnv(ints, sizeof(ints), key);
-  const float fl[] = {cond_scale, temperature};
-  key = fnv(fl, sizeof(fl), key);
-  return replay_or_capture(key, s, run);
-}
-
-// ---- the iteration of a sample with a critic and / or a prime prefix (phenaki_pytorch.py:478-550; make_video's scenes) ----
+// ---- the iteration of a sample (phenaki_pytorch.py:478-550; make_video's scenes) -------------------------------------
 // token_in [b, prime_len + n]: the MaskGit / critic input -- the prime ids in the first prime_len columns (written once by
-// the caller), the sampled tokens copied in by the call (prime_len == 0: token_in may be `ids` itself).
+// the caller), the sampled tokens copied in by the call (prime_len == 0: token_in is `ids` itself).
 //   [k_remask > 0: re-mask the k_remask lowest-confidence... (phk_topk_mask on `scores`)]
 //   -> ids -> token_in -> MaskGit CFG pair + tail on the masked rows -> ids / pred / scores (logit confidence) in place
-//   -> rng_state[1] += stride
-//   -> unless `last`: ids -> token_in -> critic forward of the CFG pair (critic: a TokenCritic table; NULL: the MaskGit's own
-//      embeddings, SelfCritic) -> scores = critic head with guidance + noise_K * (u - 0.5) * noise_mult  (:534-545)
-extern "C" int64_t phk_maskgit_demask_iteration_critic_workspace_bytes(const phk_maskgit_t* m, const phk_maskgit_t* critic,
-                                                                       int32_t b, int32_t n_total, int32_t L) {
+//   -> rng_state[1] += noise_stride(b, n, V)
+//   -> unless `skip_critic`: ids -> token_in -> critic forward of the CFG pair (critic: a TokenCritic table; NULL: the
+//      MaskGit's own embeddings, SelfCritic) -> scores = critic head with guidance + noise_K * (u - 0.5) * noise_mult  (:534-545)
+extern "C" int64_t phk_maskgit_demask_iteration_workspace_bytes(const phk_maskgit_t* m, const phk_maskgit_t* critic,
+                                                                int32_t b, int32_t n_total, int32_t L) {
   if (!m || b <= 0 || n_total <= 0) return -1;
   const int64_t a = phk_maskgit_sample_workspace_bytes(m, b, n_total, L);
   const int64_t c = phk_maskgit_workspace_bytes(critic ? critic : m, b, n_total, L, 1, PHK_PREC_BF16);
   return (a > c ? a : c) + 2 * (int64_t)b * n_total * m->dim * 4 + 512;
 }
 
-static int demask_iteration_critic_impl(const phk_maskgit_t* m, const phk_maskgit_t* critic, const float* head_w,
-                                        const float* head_b, int64_t* token_in, int64_t* ids, uint8_t* mask, float* scores,
-                                        int64_t* pred, int32_t b, int32_t n, int32_t prime_len, int32_t pt, int32_t ph,
-                                        int32_t pw, const float* ctx_kv, const float* critic_ctx_kv, int32_t L,
-                                        const uint8_t* text_mask, const float* pos_bias, float cond_scale, float temperature,
-                                        uint64_t* rng_state, int32_t k_remask, const float* critic_noise, float noise_K,
-                                        float noise_mult, int32_t last, void* workspace, int64_t workspace_bytes,
-                                        phk_stream_t s) {
+static int demask_iteration_impl(const phk_maskgit_t* m, const phk_maskgit_t* critic, const float* head_w,
+                                 const float* head_b, int64_t* token_in, int64_t* ids, uint8_t* mask, float* scores,
+                                 int64_t* pred, int32_t b, int32_t n, int32_t prime_len, int32_t pt, int32_t ph, int32_t pw,
+                                 const float* ctx_kv, const float* critic_ctx_kv, int32_t L, const uint8_t* text_mask,
+                                 const float* pos_bias, float cond_scale, float temperature, uint64_t* rng_state,
+                                 int32_t k_remask, const float* critic_noise, float noise_K, float noise_mult,
+                                 int32_t skip_critic, void* workspace, int64_t workspace_bytes, phk_stream_t s) {
   cudaStream_t st = to_stream(s);
   const int32_t nt = prime_len + n;
-  const int64_t need = phk_maskgit_demask_iteration_critic_workspace_bytes(m, critic, b, nt, L);
-  PHK_REQUIRE(workspace_bytes >= need, PHK_E_WORKSPACE, "maskgit_demask_iteration_critic: workspace too small");
+  const int64_t need = phk_maskgit_demask_iteration_workspace_bytes(m, critic, b, nt, L);
+  PHK_REQUIRE(workspace_bytes >= need, PHK_E_WORKSPACE, "maskgit_demask_iteration: workspace too small");
   const int64_t emb_bytes = 2 * (int64_t)b * nt * m->dim * 4;
   float* emb = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + ((workspace_bytes - emb_bytes) & ~(int64_t)255));
   const int64_t body_bytes = reinterpret_cast<char*>(emb) - reinterpret_cast<char*>(workspace);
@@ -1221,11 +1176,10 @@ static int demask_iteration_critic_impl(const phk_maskgit_t* m, const phk_maskgi
   };
   if (k_remask > 0) PHK_TRY(phk_topk_mask(scores, b, n, k_remask, mask, ids, (int64_t)m->num_tokens, s));
   PHK_TRY(ids_to_input());
-  PHK_TRY(sample_step_impl(m, token_in, b, nt, pt, ph, pw, ctx_kv, L, text_mask, nullptr, pos_bias, cond_scale, temperature, 0, 0,
+  PHK_TRY(sample_step_impl(m, token_in, b, nt, pt, ph, pw, ctx_kv, L, text_mask, pos_bias, cond_scale, temperature, 0, 0,
                            rng_state, mask, ids, pred, scores, k_remask > 0 ? k_remask : n, prime_len, workspace, body_bytes, s));
-  const uint64_t stride = ((uint64_t)b * (uint64_t)n * (uint64_t)((m->num_tokens + 3) / 4) + 1 + 3) / 4 * 4;
-  PHK_TRY(phk_rng_advance(rng_state, stride, s));
-  if (last) return 0;
+  PHK_TRY(phk_rng_advance(rng_state, noise_stride(b, n, m->num_tokens), s));
+  if (skip_critic) return 0;
   PHK_TRY(ids_to_input());
   const phk_maskgit_t* net = critic ? critic : m;
   PHK_TRY(phk_maskgit_forward(net, token_in, b, nt, pt, ph, pw, critic ? critic_ctx_kv : ctx_kv, L,
@@ -1236,32 +1190,34 @@ static int demask_iteration_critic_impl(const phk_maskgit_t* m, const phk_maskgi
                            (int64_t)b * n, m->dim, prime_len ? n : 0, prime_len ? nt : 0, prime_len ? prime_len : 0, s);
 }
 
-extern "C" int phk_maskgit_demask_iteration_critic(const phk_maskgit_t* m, const phk_maskgit_t* critic, const float* head_w,
-                                                   const float* head_b, int64_t* token_in, int64_t* ids, uint8_t* mask,
-                                                   float* scores, int64_t* pred, int32_t b, int32_t n, int32_t prime_len,
-                                                   int32_t pt, int32_t ph, int32_t pw, const float* ctx_kv,
-                                                   const float* critic_ctx_kv, int32_t L, const uint8_t* text_mask,
-                                                   const float* pos_bias, float cond_scale, float temperature,
-                                                   uint64_t* rng_state, int32_t k_remask, const float* critic_noise,
-                                                   float noise_K, float noise_mult, int32_t last, void* workspace,
-                                                   int64_t workspace_bytes, phk_stream_t s) {
+extern "C" int phk_maskgit_demask_iteration(const phk_maskgit_t* m, const phk_maskgit_t* critic, const float* head_w,
+                                            const float* head_b, int64_t* token_in, int64_t* ids, uint8_t* mask,
+                                            float* scores, int64_t* pred, int32_t b, int32_t n, int32_t prime_len,
+                                            int32_t pt, int32_t ph, int32_t pw, const float* ctx_kv,
+                                            const float* critic_ctx_kv, int32_t L, const uint8_t* text_mask,
+                                            const float* pos_bias, float cond_scale, float temperature,
+                                            uint64_t* rng_state, int32_t k_remask, const float* critic_noise,
+                                            float noise_K, float noise_mult, int32_t skip_critic, void* workspace,
+                                            int64_t workspace_bytes, phk_stream_t s) {
   PHK_REQUIRE(m && token_in && ids && mask && scores && pred && rng_state && workspace, PHK_E_ARG,
-              "maskgit_demask_iteration_critic: null pointer");
+              "maskgit_demask_iteration: null pointer");
   PHK_REQUIRE(n > 0 && prime_len >= 0 && k_remask >= 0 && k_remask <= n, PHK_E_ARG,
-              "maskgit_demask_iteration_critic: prime_len / k_remask out of range");
+              "maskgit_demask_iteration: prime_len / k_remask out of range");
   PHK_REQUIRE(prime_len > 0 || token_in == ids, PHK_E_ARG,
-              "maskgit_demask_iteration_critic: without a prime prefix the input buffer is the id buffer");
-  PHK_REQUIRE(last || (head_w && head_b), PHK_E_ARG, "maskgit_demask_iteration_critic: critic head missing");
+              "maskgit_demask_iteration: without a prime prefix the input buffer is the id buffer");
+  PHK_REQUIRE(skip_critic || (head_w && head_b), PHK_E_ARG, "maskgit_demask_iteration: critic head missing");
   PHK_REQUIRE(!critic || (critic->is_critic && critic->dim == m->dim), PHK_E_ARG,
-              "maskgit_demask_iteration_critic: the critic table must be a TokenCritic of the MaskGit's width");
+              "maskgit_demask_iteration: the critic table must be a TokenCritic of the MaskGit's width");
   auto run = [&](phk_stream_t st) {
-    return demask_iteration_critic_impl(m, critic, head_w, head_b, token_in, ids, mask, scores, pred, b, n, prime_len, pt, ph, pw,
-                                        ctx_kv, critic_ctx_kv, L, text_mask, pos_bias, cond_scale, temperature, rng_state,
-                                        k_remask, critic_noise, noise_K, noise_mult, last, workspace, workspace_bytes, st);
+    return demask_iteration_impl(m, critic, head_w, head_b, token_in, ids, mask, scores, pred, b, n, prime_len, pt, ph, pw,
+                                 ctx_kv, critic_ctx_kv, L, text_mask, pos_bias, cond_scale, temperature, rng_state,
+                                 k_remask, critic_noise, noise_K, noise_mult, skip_critic, workspace, workspace_bytes, st);
   };
   if (!step_graphs_enabled() || !pos_bias || g_prof_on.load(std::memory_order_relaxed)) return run(s);
   int dev = 0;
   PHK_CUDA(cudaGetDevice(&dev));
+  // key: table contents + every pointer and scalar of the call (a 64-bit FNV of them; the values behind the pointers
+  // -- token state, noise key, weights -- are read at replay time)
   uint64_t key = fnv(m, sizeof(*m), 0xcbf29ce484222325ull);
   key = hash_transformer(m->transformer, key);
   if (critic) {
@@ -1271,7 +1227,7 @@ extern "C" int phk_maskgit_demask_iteration_critic(const phk_maskgit_t* m, const
   const void* ptrs[] = {head_w, head_b, token_in, ids, mask, scores, pred, ctx_kv, critic_ctx_kv, text_mask, pos_bias, rng_state,
                         critic_noise, workspace};
   key = fnv(ptrs, sizeof(ptrs), key);
-  const int64_t ints[] = {b, n, prime_len, pt, ph, pw, L, k_remask, last, dev, workspace_bytes, 0x63726974 /* "crit" */};
+  const int64_t ints[] = {b, n, prime_len, pt, ph, pw, L, k_remask, skip_critic, dev, workspace_bytes};
   key = fnv(ints, sizeof(ints), key);
   const float fl[] = {cond_scale, temperature, noise_K, noise_mult};
   key = fnv(fl, sizeof(fl), key);

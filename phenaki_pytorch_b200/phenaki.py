@@ -45,7 +45,7 @@ def _rng_take(dev, seed, count):
 def _noise_stride(rows, vocab):
     """Philox counters one V-wide gumbel draw over `rows` tokens consumes (4 uniforms per counter), rounded up to a
     multiple of 4 (the granularity of torch's generator offset); phk_maskgit_demask_iteration advances the device-side
-    counter by the same amount."""
+    counter by the same amount (csrc/api.cu: noise_stride)."""
     return (rows * ((vocab + 3) // 4) + 1 + 3) // 4 * 4
 
 
@@ -189,18 +189,11 @@ class _TokenTransformer(nn.Module):
             if text_mask is not None:
                 text_mask = L.require_cuda(text_mask.to(torch.uint8), "text mask")
             pt, ph, pw = (int(v) for v in patch_shape)
-            if prime_len:  # ids_in = prime ids + the tokens being sampled; mask / ids / pred / scores cover the latter
-                L.check(lib.phk_maskgit_sample_step_primed(C.byref(table), L.ptr(ids_in), b, n, pt, ph, pw, L.ptr(ctx_kv),
-                                                           ctx_len, L.ptr(text_mask), L.ptr(bias), float(cond_scale),
-                                                           float(temperature), seed, offset, L.ptr(mask), L.ptr(ids),
-                                                           L.ptr(pred), L.ptr(scores), int(masked_per_seq), int(prime_len),
-                                                           L.ptr(ws), ws.numel(), L.stream_ptr()),
-                        "phk_maskgit_sample_step_primed")
-                return
+            # ids_in = prime ids + the tokens being sampled; mask / ids / pred / scores cover the latter
             L.check(lib.phk_maskgit_sample_step(C.byref(table), L.ptr(ids_in), b, n, pt, ph, pw, L.ptr(ctx_kv), ctx_len,
-                                                L.ptr(text_mask), None, L.ptr(bias), float(cond_scale),
-                                                float(temperature), seed, offset, L.ptr(mask), L.ptr(ids), L.ptr(pred),
-                                                L.ptr(scores), int(masked_per_seq), L.ptr(ws), ws.numel(),
+                                                L.ptr(text_mask), L.ptr(bias), float(cond_scale), float(temperature), seed,
+                                                offset, L.ptr(mask), L.ptr(ids), L.ptr(pred), L.ptr(scores),
+                                                int(masked_per_seq), int(prime_len), L.ptr(ws), ws.numel(),
                                                 L.stream_ptr()),
                     "phk_maskgit_sample_step")
 
@@ -649,7 +642,7 @@ class Phenaki(nn.Module):
         # training under torch.distributed: average the gradient bucket over the ranks in backward() (what the
         # reference gets from Accelerate's DDP wrapper, phenaki_trainer.py); no-op without a process group
         self.sync_gradients = True
-        # bf16 mode, no critic: ONE C call per demasking iteration with all state in device memory
+        # bf16 mode: ONE C call per demasking iteration with all state in device memory
         # (phk_maskgit_demask_iteration), replayed as ONE CUDA-graph launch per iteration from the third sample() with the
         # same shapes on (BASELINE north_star: one launch per decode iteration).  Validated on the H100 against the
         # per-step loop (identical ids: same noise counters).  PHK_STEP_GRAPH=0 restores the per-step loop.
@@ -703,17 +696,16 @@ class Phenaki(nn.Module):
             have_scores = False
             iterations = (self.iteration_call and self.fused_head and mg.precision == L.PREC_BF16 and noise_fn is None
                           and cond_scale != 1 and trace is None and self._fused_step_supported())
-            if iterations and plen == 0 and self.critic is None:
-                return self._sample_by_iterations(b, n, patch_shape, ctx_kv, ctx_len, text_mask, cond_scale,
-                                                  starting_temperature, ks, seed, vocab, dev)
-            critic_ok = self.critic is None or isinstance(self.critic, SelfCritic) or (
-                isinstance(self.critic, TokenCritic) and self.critic.precision == L.PREC_BF16)
-            if iterations and critic_ok and self.critic_noise_anneal_schedule in ("fixed", "decay", "increase"):
-                return self._sample_by_critic_iterations(b, n, plen, prime_token_ids, patch_shape, ctx_kv, critic_kv, ctx_len,
-                                                         text_mask, cond_scale, starting_temperature, noise_K, ks, seed,
-                                                         vocab, dev)
+            # an unknown anneal schedule takes the per-step loop, which raises on it
+            critic_ok = self.critic is None or (
+                self.critic_noise_anneal_schedule in ("fixed", "decay", "increase")
+                and (isinstance(self.critic, SelfCritic)
+                     or (isinstance(self.critic, TokenCritic) and self.critic.precision == L.PREC_BF16)))
+            if iterations and critic_ok:
+                return self._sample_by_iterations(b, n, plen, prime_token_ids, patch_shape, ctx_kv, critic_kv, ctx_len,
+                                                  text_mask, cond_scale, starting_temperature, noise_K, ks, seed, vocab, dev)
             # the whole sample's V-wide noise counters are reserved up front (iteration s uses first + s * stride), as the
-            # iteration entries do: the critic's torch.rand draws then follow them in the generator stream on every path
+            # iteration path does: the critic's torch.rand draws then follow them in the generator stream on every path
             stride = _noise_stride(b * n, vocab)
             first_offset = _rng_take(dev, seed, stride * steps)
             for step in range(steps):
@@ -785,57 +777,16 @@ class Phenaki(nn.Module):
                     trace[-1]["scores"] = scores.clone()
         return ids
 
-    def _sample_by_iterations(self, b, n, patch_shape, ctx_kv, ctx_len, text_mask, cond_scale, starting_temperature,
-                              ks, seed, vocab, dev):
-        """The demasking loop as ``steps`` calls of phk_maskgit_demask_iteration.  Token state, mask, scores, the text
-        keys / values and the noise key live in buffers that persist across ``sample`` calls, so the library sees the
-        same arguments at iteration s of every sample and can replay one captured CUDA graph per iteration."""
-        lib, mg, steps = L.lib(), self.maskgit, self.steps
-        key = (b, n, ctx_len, dev)
-        bufs = self._iter_bufs.get(key)
-        if bufs is None:
-            bufs = self._iter_bufs[key] = dict(
-                ids=torch.empty((b, n), dtype=torch.int64, device=dev), mask=torch.empty((b, n), dtype=torch.uint8, device=dev),
-                scores=torch.empty((b, n), dtype=torch.float32, device=dev), pred=torch.empty((b, n), dtype=torch.int64, device=dev),
-                rng=torch.empty((2,), dtype=torch.int64, device=dev),
-                ctx_kv=None if ctx_kv is None else torch.empty_like(ctx_kv),
-                text_mask=None if text_mask is None else torch.empty(text_mask.shape, dtype=torch.uint8, device=dev))
-        bufs["ids"].fill_(self.mask_id)
-        bufs["mask"].fill_(1)
-        bufs["scores"].zero_()
-        if ctx_kv is not None:
-            bufs["ctx_kv"].copy_(ctx_kv)
-            bufs["text_mask"].copy_(text_mask.to(torch.uint8))
-        stride = _noise_stride(b * n, vocab)
-        as_i64 = lambda v: v - (1 << 64) if v >= (1 << 63) else v  # uint64 bit pattern in an int64 tensor
-        first = _rng_take(dev, seed, stride * steps)  # the library advances the device-side counter by `stride` per iteration
-        # two scalar fills, not a host tensor: a pageable H2D copy synchronises the stream first, which stalled the host at the
-        # start of every sample until the previous scene's decode had drained (make_video was host-bound through it)
-        bufs["rng"][0].fill_(as_i64(seed & (2 ** 64 - 1)))
-        bufs["rng"][1].fill_(as_i64(first))
-        with torch.cuda.device(dev):
-            table = mg._table()
-            ws = mg._ws.get(lib.phk_maskgit_sample_workspace_bytes(C.byref(table), b, n, ctx_len), dev)
-            bias = mg._pos_bias(table, patch_shape, dev)
-            pt, ph, pw = (int(v) for v in patch_shape)
-            for step in range(steps):
-                temperature = starting_temperature * ((steps - (step + 1)) / steps)
-                L.check(lib.phk_maskgit_demask_iteration(
-                    C.byref(table), L.ptr(bufs["ids"]), L.ptr(bufs["mask"]), L.ptr(bufs["scores"]), L.ptr(bufs["pred"]),
-                    b, n, pt, ph, pw, L.ptr(bufs["ctx_kv"]), ctx_len, L.ptr(bufs["text_mask"]), L.ptr(bias),
-                    float(cond_scale), float(temperature), L.ptr(bufs["rng"]), 0 if step == 0 else ks[step - 1],
-                    L.ptr(ws), ws.numel(), L.stream_ptr()), "phk_maskgit_demask_iteration")
-        return bufs["ids"].clone()
-
-    def _sample_by_critic_iterations(self, b, n, plen, prime_token_ids, patch_shape, ctx_kv, critic_kv, ctx_len, text_mask,
-                                     cond_scale, starting_temperature, noise_K, ks, seed, vocab, dev):
-        """The demasking loop with a critic and / or a prime prefix as ``steps`` calls of
-        phk_maskgit_demask_iteration_critic: re-mask, MaskGit CFG pair + tail, critic CFG pair + scores are ONE launch
-        sequence per iteration that the library replays as a CUDA graph (every per-call value lives in the persistent
-        buffers below; temperature, k and the critic-noise multiplier of iteration s are the same in every sample)."""
+    def _sample_by_iterations(self, b, n, plen, prime_token_ids, patch_shape, ctx_kv, critic_kv, ctx_len, text_mask,
+                              cond_scale, starting_temperature, noise_K, ks, seed, vocab, dev):
+        """The demasking loop as ``steps`` calls of phk_maskgit_demask_iteration: re-mask, MaskGit CFG pair + tail and,
+        with a critic, critic CFG pair + scores are ONE launch sequence per iteration.  Token state, mask, scores, the
+        text keys / values and the noise key live in buffers that persist across ``sample`` calls, so the library sees
+        the same arguments at iteration s of every sample (temperature, k and the critic-noise multiplier of iteration s
+        are the same in every sample) and can replay one captured CUDA graph per iteration."""
         lib, mg, steps, critic = L.lib(), self.maskgit, self.steps, self.critic
         token_critic = isinstance(critic, TokenCritic)
-        key = ("critic", b, n, plen, ctx_len, dev, None if critic is None else id(critic),
+        key = (b, n, plen, ctx_len, dev, None if critic is None else id(critic),
                None if critic_kv is None else tuple(critic_kv.shape))
         bufs = self._iter_bufs.get(key)
         if bufs is None:
@@ -858,8 +809,8 @@ class Phenaki(nn.Module):
         if critic_kv is not None:
             bufs["critic_kv"].copy_(critic_kv)
         stride = _noise_stride(b * n, vocab)
-        as_i64 = lambda v: v - (1 << 64) if v >= (1 << 63) else v
-        first = _rng_take(dev, seed, stride * steps)
+        as_i64 = lambda v: v - (1 << 64) if v >= (1 << 63) else v  # uint64 bit pattern in an int64 tensor
+        first = _rng_take(dev, seed, stride * steps)  # the library advances the device-side counter by `stride` per iteration
         # two scalar fills, not a host tensor: a pageable H2D copy synchronises the stream first, which stalled the host at the
         # start of every sample until the previous scene's decode had drained (make_video was host-bound through it)
         bufs["rng"][0].fill_(as_i64(seed & (2 ** 64 - 1)))
@@ -875,26 +826,27 @@ class Phenaki(nn.Module):
                         L.require_cuda(critic.to_pred[0].bias.detach(), "to_pred.bias", torch.float32))
                 head_w, head_b = L.ptr(keep[0]), L.ptr(keep[1])
             cref = C.byref(ctable) if ctable is not None else None
-            nbytes = lib.phk_maskgit_demask_iteration_critic_workspace_bytes(C.byref(table), cref, b, plen + n, ctx_len)
+            nbytes = lib.phk_maskgit_demask_iteration_workspace_bytes(C.byref(table), cref, b, plen + n, ctx_len)
             ws = mg._ws.get(nbytes, dev)
             bias = mg._pos_bias(table, patch_shape, dev)
             pt, ph, pw = (int(v) for v in patch_shape)
             inp = bufs["inp"] if plen else bufs["ids"]
             for step in range(steps):
-                last = step == steps - 1
                 til_x0 = steps - (step + 1)
                 temperature = starting_temperature * (til_x0 / steps)
-                mult = {"fixed": 1.0, "decay": til_x0 / steps, "increase": (step + 1) / steps}[self.critic_noise_anneal_schedule]
-                with_critic = critic is not None and not last
+                with_critic = critic is not None and step < steps - 1
+                mult = 0.0
                 if with_critic:
+                    mult = {"fixed": 1.0, "decay": til_x0 / steps, "increase": (step + 1) / steps}[
+                        self.critic_noise_anneal_schedule]
                     bufs["noise"].uniform_()  # torch.rand((b, n)) of the per-step loop, drawn into the stable buffer
-                L.check(lib.phk_maskgit_demask_iteration_critic(
+                L.check(lib.phk_maskgit_demask_iteration(
                     C.byref(table), cref, head_w, head_b, L.ptr(inp), L.ptr(bufs["ids"]), L.ptr(bufs["mask"]),
                     L.ptr(bufs["scores"]), L.ptr(bufs["pred"]), b, n, plen, pt, ph, pw, L.ptr(bufs["ctx_kv"]),
                     L.ptr(bufs["critic_kv"]) if token_critic else None, ctx_len, L.ptr(bufs["text_mask"]), L.ptr(bias),
                     float(cond_scale), float(temperature), L.ptr(bufs["rng"]), 0 if step == 0 else ks[step - 1],
                     L.ptr(bufs["noise"]) if with_critic else None, float(noise_K), float(mult), int(not with_critic),
-                    L.ptr(ws), ws.numel(), L.stream_ptr()), "phk_maskgit_demask_iteration_critic")
+                    L.ptr(ws), ws.numel(), L.stream_ptr()), "phk_maskgit_demask_iteration")
         return bufs["ids"].clone()
 
     @torch.no_grad()

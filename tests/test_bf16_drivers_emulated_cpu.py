@@ -76,7 +76,7 @@ def test_demasking_iterations_as_replayed_graphs_equal_the_default_loop(_emu_lib
 
 @pytest.mark.parametrize("critic_kind,primed", [("token", True), ("self", False), (None, True), ("token", False)])
 def test_critic_and_primed_iterations_as_replayed_graphs_equal_the_per_step_loop(_emu_lib, critic_kind, primed):
-    """phk_maskgit_demask_iteration_critic (re-mask + MaskGit CFG pair + tail + critic CFG pair + scores per call; prime ids
+    """phk_maskgit_demask_iteration (re-mask + MaskGit CFG pair + tail + critic CFG pair + scores per call; prime ids
     ahead of the sampled tokens) against the per-step Python loop: three consecutive samples (eager, captured, replayed),
     fresh V-wide noise and fresh critic noise per call -- a value wrongly baked into a graph shows up as a difference."""
     from phenaki_pytorch_b200 import _lib as L

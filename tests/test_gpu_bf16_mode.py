@@ -219,7 +219,7 @@ def test_one_graph_launch_per_iteration_equals_the_per_step_loop():
 
 @pytest.mark.parametrize("critic_kind,primed", [("token", True), ("self", False), (None, True)])
 def test_critic_and_primed_iterations_equal_the_per_step_loop(critic_kind, primed):
-    """phk_maskgit_demask_iteration_critic (re-mask + MaskGit CFG pair + tail + critic CFG pair + scores in ONE launch
+    """phk_maskgit_demask_iteration (re-mask + MaskGit CFG pair + tail + critic CFG pair + scores in ONE launch
     sequence per iteration, replayed as a graph from the third sample on; make_video's primed scenes) against the per-step
     loop: same V-wide noise counters and the same torch generator draws for the critic noise -> identical ids, four
     consecutive samples."""

@@ -119,8 +119,8 @@ def test_cfg3_masked_rows_step_equals_all_rows_step_at_full_size(k):
 
 
 def test_primed_fused_sample_step_equals_the_unprimed_step_on_the_same_rows():
-    """phk_maskgit_sample_step_primed (scene chains of make_video, phenaki_pytorch.py:493, 503-504): with a prime prefix of
-    `plen` ids the head runs on the masked rows of the sampled tokens only.  The step sees the same network input whether
+    """phk_maskgit_sample_step with prime_len > 0 (scene chains of make_video, phenaki_pytorch.py:493, 503-504): with a
+    prime prefix of `plen` ids the head runs on the masked rows of the sampled tokens only.  The step sees the same network input whether
     the prefix is declared as prime or the whole sequence is treated as sampled with the prefix unmasked, so at temperature
     0 both calls must produce the same ids / confidences on the sampled tokens."""
     torch.manual_seed(9)
