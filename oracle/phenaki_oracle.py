@@ -6,7 +6,8 @@ MaskGIT iterative masked sampling loop.  Purely functional: every function
 takes the reference ``state_dict`` (plain ``{name: tensor}``) and a key prefix,
 so it shares no code or structure with either the reference modules or the
 product.  Each function cites the reference file:line it follows
-(paths relative to /root/reference/phenaki_pytorch/).
+(paths relative to /root/reference/phenaki_pytorch/).  The MaskGit / critic functions compute in
+the dtype of the state dict they are given: tests/train_at_size_cases.py runs them in float64.
 
 Pinning: ``tests/golden/make_golden.py`` runs this file against the UNMODIFIED
 reference modules imported in the build container (oracle/reference_loader.py)
@@ -130,12 +131,11 @@ def attention(x, sd, p, *, heads, causal=False, num_null_kv=0, mask=None, contex
 
 def continuous_position_bias(sd, p, dims):
     """attention.py:229-275 -> (heads, n, n), n = prod(dims).  Weight-only function."""
-    dev = sd[p + "net.0.0.weight"].device
-    pos = [torch.arange(d, device=dev) for d in dims]
+    w0 = sd[p + "net.0.0.weight"]
+    pos = [torch.arange(d, device=w0.device) for d in dims]
     grid = torch.stack(torch.meshgrid(*pos, indexing="ij")).reshape(len(dims), -1).t()
-    rel = grid[:, None, :] - grid[None, :, :]
-    rel = torch.sign(rel) * torch.log(rel.abs() + 1)
-    h = rel.float()
+    rel = (grid[:, None, :] - grid[None, :, :]).to(w0.dtype)  # the weights' dtype (fp32: the same values as before)
+    h = torch.sign(rel) * torch.log(rel.abs() + 1)
     n_layers = len({k[len(p):].split(".")[1] for k in sd if k.startswith(p + "net.")})
     for li in range(n_layers - 1):
         h = F.leaky_relu(F.linear(h, sd[f"{p}net.{li}.0.weight"], sd[f"{p}net.{li}.0.bias"]), 0.1)
@@ -508,7 +508,7 @@ def critic_train_loss(ids, pred_ids, token_mask, critic_sd, *, video_patch_shape
     critic_input = torch.where(token_mask, pred_ids, ids)
     scores = critic_forward(critic_input, critic_sd, video_patch_shape=video_patch_shape, heads=heads,
                             context=context, text_mask=text_mask, video_mask=video_mask, p=p)
-    labels = (ids != pred_ids).float()
+    labels = (ids != pred_ids).to(scores.dtype)
     return F.binary_cross_entropy_with_logits(scores, labels)
 
 
@@ -523,4 +523,4 @@ def self_critic_train_loss(ids, pred_ids, token_mask, maskgit_sd, to_pred_w, to_
     emb = maskgit_forward(critic_input, maskgit_sd, video_patch_shape=video_patch_shape, heads=heads, context=context,
                           text_mask=text_mask, video_mask=video_mask, return_embeds=True)
     scores = F.linear(emb, to_pred_w, to_pred_b).squeeze(-1)
-    return F.binary_cross_entropy_with_logits(scores, (ids != pred_ids).float())
+    return F.binary_cross_entropy_with_logits(scores, (ids != pred_ids).to(scores.dtype))
