@@ -604,14 +604,34 @@ int phk_debug_step_graph(int32_t on);
  * prec: PHK_PREC_F32 = fp32 FFMA products (parity with the fp32 reference); PHK_PREC_BF16 = the forward, dgrad and
  * wgrad product of every nn.Linear on the wgmma GEMM (phk_gemm_bf16) with operands converted on the fly from the
  * fp32 activations / master weights (the dtype flow of torch.autocast(bfloat16)); LayerNorm, softmax, GEGLU, the
- * attention core and all gradients of non-matrix parameters stay fp32 in both modes. */
+ * attention core and all gradients of non-matrix parameters stay fp32 in both modes.
+ * dropout: NULL, or both probabilities 0, is the step without dropout (no mask is drawn).  Otherwise the step applies the
+ *   reference's nn.Dropout in training mode: attn_p to the softmax probabilities of every self- and cross-attention,
+ *   null-key columns included, before attn @ v (attention.py:177); ff_p to the GEGLU output before the second Linear
+ *   (attention.py:51).  0 <= p <= 1 (else PHK_E_ARG); p = 1 drops everything (zeros, as torch).  The masks are a
+ *   counter-based contract on the sampling noise's generator (phk_sample_tokens, u == NULL):
+ *     element e of a site is kept iff u >= p (p in fp32) and then scaled by 1 / (1 - p), where u = (2*(draw >> 9) + 1)
+ *     / 2^24 (exact in fp32) and draw = word e % 4 of Philox4x32-7(key = (seed lo 32, seed hi 32),
+ *     counter = (c lo 32, c hi 32, 0, 0)), c = base + e / 4.
+ *   Sites, in order, for each layer: the self-attention probabilities [b, heads, n, n]; the cross-attention
+ *   probabilities [b, heads, n, num_null_kv + L] (null keys first), only when the layer runs cross-attention (context
+ *   given); the FF hidden [b*n, inner].  e is the row-major index in that shape.  The first site's base is offset, the
+ *   next base is base + ceil(count / 4).  Every site takes its counters whatever the probabilities, so one step uses
+ *   phk_maskgit_train_dropout_counters(m, b, n, L) counters from offset on (L = 0 without a context; -1 on bad
+ *   arguments).  The workspace is the same with and without dropout. */
+typedef struct phk_dropout {
+  float attn_p, ff_p;
+  uint64_t seed, offset;
+} phk_dropout_t;
 int64_t phk_maskgit_train_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L, int32_t bce_head,
                                           int32_t prec);
+int64_t phk_maskgit_train_dropout_counters(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L);
 int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_t* grads, const int64_t* ids_in,
                            const int64_t* targets, const uint8_t* token_mask, const float* labels, int32_t b, int32_t n,
                            int32_t pt, int32_t ph, int32_t pw, const float* context, int32_t L,
                            const uint8_t* text_mask, const uint8_t* video_mask, float loss_scale, float* loss_out,
-                           float* logits_out, void* workspace, int64_t workspace_bytes, int32_t prec, phk_stream_t s);
+                           float* logits_out, void* workspace, int64_t workspace_bytes, int32_t prec, phk_stream_t s,
+                           const phk_dropout_t* dropout);
 /* Data-parallel overlap: `events` (cudaEvent_t handles, count >= depth + 2) are recorded by the NEXT phk_maskgit_train_step
  * call of the calling thread, on its stream, as gradient groups become final: events[0] head + norm_out, events[1 + k]
  * transformer layer depth-1-k, events[depth + 1] embeddings + position-bias MLP (= all).  One-shot; NULL clears. */

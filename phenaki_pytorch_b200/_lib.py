@@ -100,6 +100,10 @@ class AttnGeomT(C.Structure):
                 ("out_bf16", C.c_int32), ("scale", C.c_float), ("_pad", C.c_int32)]
 
 
+class DropoutT(C.Structure):
+    _fields_ = [("attn_p", C.c_float), ("ff_p", C.c_float), ("seed", C.c_uint64), ("offset", C.c_uint64)]
+
+
 i32, i64, f32, u64, vp = C.c_int32, C.c_int64, C.c_float, C.c_uint64, C.c_void_p
 
 # name -> argtypes (restype int unless listed in _RESTYPES); mirrors include/phk.h one to one
@@ -178,11 +182,12 @@ PROTOTYPES = {
     "phk_maskgit_forward": [C.POINTER(MaskgitT), vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, i32, i32, vp, vp,
                             vp, i64, i32, vp],
     "phk_maskgit_train_workspace_bytes": [C.POINTER(MaskgitT), i32, i32, i32, i32, i32],
+    "phk_maskgit_train_dropout_counters": [C.POINTER(MaskgitT), i32, i32, i32],
     "phk_maskgit_train_step": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, i32,
-                               vp, vp, f32, vp, vp, vp, i64, i32, vp],
+                               vp, vp, f32, vp, vp, vp, i64, i32, vp, C.POINTER(DropoutT)],
 }
 _RESTYPES = {"phk_attention_tc_scratch_bytes": i64, "phk_head_sample_scratch_bytes": i64,
-             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
+             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_maskgit_train_dropout_counters": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
              "phk_cvivit_workspace_bytes": i64, "phk_cvivit_decode_workspace_bytes": i64, "phk_maskgit_workspace_bytes": i64}
 
 FAMILIES = ["patchify_ln", "layernorm", "gemm_f32", "gemm_bf16", "attention", "peg", "geglu", "lfq", "embed",

@@ -12,6 +12,7 @@
 // deliberately plain (one warp per row, coalesced, no tensor cores): this is the parity path that pins the gradient
 // math against the reference's autograd; every formula is restated on the CPU in tests/train_mirror.py and checked
 // against the reference there.  In bf16 mode the products run on the tensor-core GEMM instead (see below).
+// With dropout (phk_dropout_t) the masks are regenerated from Philox counters wherever they are needed, never stored.
 // Checked against the reference's gradients on the CPU by tests/cuda_emu (this very source, g++-compiled) and on the GPU
 // by tests/test_gpu_train.py.
 #include "phk_common.cuh"
@@ -420,16 +421,46 @@ int ln_backward(const float* x, const float* g, const float* dy, float* dx, int 
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// GEGLU backward (attention.py:40-43; mirror geglu_bwd): h = [val | gate], g = gelu_erf(gate) * val
-//   dval = dg * gelu(gate) ; dgate = dg * val * (Phi(gate) + gate * phi(gate))
+// Dropout (include/phk.h, phk_dropout_t): element e of a site is kept iff u(base + e/4, word e % 4) >= p and then scaled
+// by 1/(1 - p); u is the sampling noise's uniform of that Philox4x32-7 block.  p == 0: the site is off.
 // ------------------------------------------------------------------------------------------------------------------
-__global__ void geglu_bwd_kernel(const float* __restrict__ h, const float* __restrict__ dg, float* __restrict__ dh,
-                                 int64_t rows, int inner) {
+struct DropSite { float p, scale; uint32_t k0, k1; uint64_t base; };
+
+__device__ __forceinline__ float drop_factor(const DropSite& d, uint64_t e) {
+  const uint64_t c = d.base + (e >> 2);
+  uint32_t r[4];
+  philox4x32<kNoiseRounds>((uint32_t)c, (uint32_t)(c >> 32), 0u, 0u, d.k0, d.k1, r);
+  const uint32_t k = (uint32_t)(e & 3);
+  const uint32_t w = k == 0 ? r[0] : (k == 1 ? r[1] : (k == 2 ? r[2] : r[3]));
+  const float u = (float)(2u * (w >> 9) + 1u) * (1.0f / 16777216.0f);  // exact: 2 (w >> 9) + 1 < 2^24
+  return u >= d.p ? d.scale : 0.f;                                      // p = 1 keeps nothing (u < 1): zeros, not NaN
+}
+
+// g = gelu(gate) * val * M / (1 - p): GEGLU followed by the FF dropout (attention.py:51), the dropped g is what W2 reads
+__global__ void geglu_dropout_kernel(const float* __restrict__ h, float* __restrict__ g, int64_t rows, int inner,
+                                     DropSite d) {
   const int64_t total = rows * inner;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = i / inner;
     const int j = (int)(i - r * inner);
-    const float val = h[r * 2 * inner + j], gate = h[r * 2 * inner + inner + j], d = dg[i];
+    const float m = drop_factor(d, (uint64_t)i);
+    g[i] = m != 0.f ? gelu_erf(h[r * 2 * inner + inner + j]) * h[r * 2 * inner + j] * m : 0.f;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// GEGLU backward (attention.py:40-43; mirror geglu_bwd): h = [val | gate], g = gelu_erf(gate) * val
+//   dval = dg * gelu(gate) ; dgate = dg * val * (Phi(gate) + gate * phi(gate))
+// With FF dropout (d.p > 0) the incoming gradient is that of the dropped g: dg is first multiplied by M / (1 - p).
+// ------------------------------------------------------------------------------------------------------------------
+__global__ void geglu_bwd_kernel(const float* __restrict__ h, const float* __restrict__ dg, float* __restrict__ dh,
+                                 int64_t rows, int inner, DropSite drop) {
+  const int64_t total = rows * inner;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / inner;
+    const int j = (int)(i - r * inner);
+    const float val = h[r * 2 * inner + j], gate = h[r * 2 * inner + inner + j];
+    const float d = drop.p > 0.f ? dg[i] * drop_factor(drop, (uint64_t)i) : dg[i];
     const float cdf = 0.5f * (1.0f + erff(gate * 0.70710678118654752440f));
     const float pdf = expf(-0.5f * gate * gate) * 0.39894228040143267794f;
     dh[r * 2 * inner + j] = d * gate * cdf;
@@ -487,11 +518,46 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const float* __restr
   }
 }
 
+// Forward with attention dropout, one warp per (sequence, head, query).  In: P holds the raw products qh.kh.
+// Out (in place): P = softmax(8 qh.kh + bias, masks) * M / (1 - p), element e = row * nkt + j of the site.
+__global__ void __launch_bounds__(256) attn_fwd_softmax_dropout_kernel(const float* __restrict__ bias,
+                                                                       const uint8_t* __restrict__ key_mask,
+                                                                       float* __restrict__ P, AttnBwdGeom g, DropSite d) {
+  const int lane = threadIdx.x & 31;
+  const int nkt = g.nnull + g.m;
+  const int64_t w = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (w >= (int64_t)g.b * g.H * g.n) return;
+  const int i = (int)(w % g.n);
+  const int h = (int)((w / g.n) % g.H);
+  const int bi = (int)(w / ((int64_t)g.n * g.H));
+  float* Pr = P + w * nkt;
+  float mx = -FLT_MAX;
+  for (int j = lane; j < nkt; j += 32) {
+    float s = Pr[j] * 8.0f;
+    if (bias && j >= g.nnull) s += bias[((int64_t)h * g.n + i) * g.m + (j - g.nnull)];
+    if (key_mask && j >= g.nnull && !key_mask[(int64_t)bi * g.m + (j - g.nnull)]) s = -FLT_MAX;
+    Pr[j] = s;
+    mx = fmaxf(mx, s);
+  }
+  mx = warp_max(mx);
+  float sum = 0.f;
+  for (int j = lane; j < nkt; j += 32) { const float e = expf(Pr[j] - mx); Pr[j] = e; sum += e; }
+  sum = warp_sum(sum);
+  const float inv = 1.0f / sum;
+  for (int j = lane; j < nkt; j += 32) {
+    const float m = drop_factor(d, (uint64_t)w * nkt + j);
+    Pr[j] = m != 0.f ? Pr[j] * inv * m : 0.f;
+  }
+}
+
 // one warp per (sequence, head, query).  In: P holds the raw products qh.kh (batched GEMM), dS holds dP = dO.vv.
 // Out (in place): P = softmax(8 qh.kh + bias, masks), dS = P * (dP - sum_j P dP).  Rows are contiguous: coalesced.
+// With attention dropout (d.p > 0) dS holds the gradient of the DROPPED probabilities: dP = dS * M / (1 - p) enters the
+// softmax backward, which differentiates the undropped P; P is then overwritten by the dropped P that the forward
+// multiplied V with (what dV = P^T.dO needs).
 __global__ void __launch_bounds__(256) attn_bwd_softmax_kernel(const float* __restrict__ bias,
                                                                const uint8_t* __restrict__ key_mask, float* __restrict__ P,
-                                                               float* __restrict__ dS, AttnBwdGeom g) {
+                                                               float* __restrict__ dS, AttnBwdGeom g, DropSite d) {
   const int lane = threadIdx.x & 31;
   const int nkt = g.nnull + g.m;
   const int64_t w = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -515,6 +581,20 @@ __global__ void __launch_bounds__(256) attn_bwd_softmax_kernel(const float* __re
   sum = warp_sum(sum);
   const float inv = 1.0f / sum;
   float dot = 0.f;
+  if (d.p > 0.f) {
+    for (int j = lane; j < nkt; j += 32) {
+      const float p = Pr[j] * inv;
+      const float dp = dSr[j] * drop_factor(d, (uint64_t)w * nkt + j);
+      Pr[j] = p; dSr[j] = dp; dot += p * dp;
+    }
+    dot = warp_sum(dot);
+    for (int j = lane; j < nkt; j += 32) {
+      const float m = drop_factor(d, (uint64_t)w * nkt + j);
+      dSr[j] = Pr[j] * (dSr[j] - dot);
+      Pr[j] = m != 0.f ? Pr[j] * m : 0.f;
+    }
+    return;
+  }
   for (int j = lane; j < nkt; j += 32) { const float p = Pr[j] * inv; Pr[j] = p; dot += p * dSr[j]; }
   dot = warp_sum(dot);
   for (int j = lane; j < nkt; j += 32) dSr[j] = Pr[j] * (dSr[j] - dot);
@@ -687,7 +767,7 @@ int64_t attn_bwd_scratch_floats(int b, int H, int n, int nkt, int dh) {
 // q [b*n, I], kv [b*m, 2I], dO [b*n, I] -> dq [b*n, I], dkv [b*m, 2I]; parameter gradients accumulate
 int attention_backward(const float* q, const float* kv, const phk_attn_t& A, const phk_attn_t& G, const float* bias,
                        const uint8_t* key_mask, const float* dO, float* dq, float* dkv, float* dbias,
-                       const AttnBwdGeom& g, float* scratch, cudaStream_t st, bool bf16_products = false) {
+                       const AttnBwdGeom& g, float* scratch, cudaStream_t st, bool bf16_products, const DropSite& drop) {
   PHK_REQUIRE(g.dh <= 32 * kDPL, PHK_E_UNSUPPORTED, "train: dim_head > 128");
   PHK_REQUIRE(g.nnull == 0 || (A.null_kv && G.null_kv), PHK_E_ARG, "train: null_kv (gradient) missing");
   const int nkt = g.nnull + g.m;
@@ -710,7 +790,7 @@ int attention_backward(const float* q, const float* kv, const phk_attn_t& A, con
   const GemmBatch bd{(int)bh, g.H, (int64_t)g.n * I, (int64_t)g.dh, (int64_t)g.H * nkt * g.dh, (int64_t)nkt * g.dh,
                      (int64_t)g.H * g.n * nkt, (int64_t)g.n * nkt};
   PHK_TRY(sgemm_batched(dO, I, 1, B.vv, 1, g.dh, B.dS, nkt, g.n, nkt, g.dh, 0, bd, st, bf16_products));
-  PHK_KERNEL_LAUNCH(attn_bwd_softmax_kernel, dim3((unsigned)((bh * g.n + 7) / 8)), dim3(256), (size_t)(0), st, bias, key_mask, B.P, B.dS, g);
+  PHK_KERNEL_LAUNCH(attn_bwd_softmax_kernel, dim3((unsigned)((bh * g.n + 7) / 8)), dim3(256), (size_t)(0), st, bias, key_mask, B.P, B.dS, g, drop);
   PHK_LAUNCH_CHECK();
   // dq / dk / dv contractions: batched register-tiled products for long sequences (the warp-per-row loops of the two
   // kernels walk a column of dS / P with a stride of nkt floats: 1.5 ms per layer at n = 576), loops for short ones
@@ -739,6 +819,34 @@ int attention_backward(const float* q, const float* kv, const phk_attn_t& A, con
     PHK_LAUNCH_CHECK();
   }
   return 0;
+}
+
+// Attention forward with dropout on the probabilities (attention.py:177): the explicit path of the backward's
+// recomputation -- prep, S = qh.kh^T, softmax + dropout, then O = P_drop.vv written token-major into o [b*n, I].
+// fp32 products in both precision modes (the attention core is fp32).  Uses the backward's scratch (qh, kh, vv, P).
+int attention_forward_dropout(const float* q, const float* kv, const phk_attn_t& A, const float* bias,
+                              const uint8_t* key_mask, float* o, const AttnBwdGeom& g, float* scratch, cudaStream_t st,
+                              const DropSite& drop) {
+  PHK_REQUIRE(g.dh <= 32 * kDPL, PHK_E_UNSUPPORTED, "train: dim_head > 128");
+  PHK_REQUIRE(g.nnull == 0 || A.null_kv, PHK_E_ARG, "train: null_kv missing");
+  const int nkt = g.nnull + g.m;
+  const int64_t bh = (int64_t)g.b * g.H;
+  float* qh = scratch;
+  float* kh = qh + bh * g.n * g.dh;
+  float* vv = kh + bh * nkt * g.dh;
+  float* P = vv + bh * nkt * g.dh;
+  const int64_t prep_warps = bh * (g.n + nkt);
+  PHK_KERNEL_LAUNCH(attn_bwd_prep_kernel, dim3((unsigned)((prep_warps + 7) / 8)), dim3(256), (size_t)(0), st, q, kv, A.null_kv, A.q_scale, A.k_scale, qh, kh, vv, g);
+  PHK_LAUNCH_CHECK();
+  const GemmBatch bs{(int)bh, 1, (int64_t)g.n * g.dh, 0, (int64_t)nkt * g.dh, 0, (int64_t)g.n * nkt, 0};
+  PHK_TRY(sgemm_batched(qh, g.dh, 1, kh, 1, g.dh, P, nkt, g.n, nkt, g.dh, 0, bs, st));
+  PHK_KERNEL_LAUNCH(attn_fwd_softmax_dropout_kernel, dim3((unsigned)((bh * g.n + 7) / 8)), dim3(256), (size_t)(0), st, bias, key_mask, P, g, drop);
+  PHK_LAUNCH_CHECK();
+  // o[(bi, i), h * dh + d] = sum_j P[bi, h, i, j] vv[bi, h, j, d]
+  const int I = g.H * g.dh;
+  const GemmBatch bo{(int)bh, g.H, (int64_t)g.H * g.n * nkt, (int64_t)g.n * nkt, (int64_t)g.H * nkt * g.dh,
+                     (int64_t)nkt * g.dh, (int64_t)g.n * I, (int64_t)g.dh};
+  return sgemm_batched(P, nkt, 1, vv, g.dh, 1, o, I, g.n, g.dh, nkt, 0, bo, st);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1059,6 +1167,26 @@ int64_t tc_scratch_elems(const phk_maskgit_t* m, int64_t R, int64_t CR, bool bce
   return (tokens > feat + 8 ? tokens : feat + 8) * (width + 8);
 }
 
+// Counter layout of one step's dropout masks (include/phk.h, phk_dropout_t): per layer, in order, the self-attention
+// probabilities [b, H, n, n], the cross-attention probabilities [b, H, n, nnull + L] when the layer runs cross-attention
+// (L > 0), the FF hidden [b*n, inner]; each site takes ceil(count / 4) counters right after the previous one.
+// bases (optional, [depth][3]): the first counter of each site, relative to the step's offset.  Returns the total.
+uint64_t dropout_layout(const phk_maskgit_t* m, int b, int n, int L, uint64_t (*bases)[3]) {
+  const phk_transformer_t* T = &m->transformer;
+  const uint64_t bh = (uint64_t)b * T->heads;
+  uint64_t c = 0;
+  for (int l = 0; l < T->depth; ++l) {
+    const phk_layer_t& Ly = T->layers[l];
+    const uint64_t cross = Ly.has_cross && L > 0 ? bh * n * (uint64_t)(Ly.cross_attn.num_null_kv + L) : 0;
+    const uint64_t count[3] = {bh * n * n, cross, (uint64_t)b * n * Ly.ff.inner};
+    for (int s = 0; s < 3; ++s) {
+      if (bases) bases[l][s] = c;
+      c += (count[s] + 3) / 4;
+    }
+  }
+  return c;
+}
+
 }  // namespace
 }  // namespace phk
 
@@ -1108,6 +1236,11 @@ extern "C" int64_t phk_maskgit_train_workspace_bytes(const phk_maskgit_t* m, int
   return bytes;
 }
 
+extern "C" int64_t phk_maskgit_train_dropout_counters(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L) {
+  if (!m || b <= 0 || n <= 0 || L < 0 || !m->transformer.layers) return -1;
+  return (int64_t)dropout_layout(m, b, n, L, nullptr);
+}
+
 // See include/phk.h.  grads: a table of the SAME layout as `m` whose float pointers address zero-filled gradient
 // buffers (bf16 members unused); every parameter gradient is accumulated into it.
 extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_t* grads, const int64_t* ids_in,
@@ -1115,7 +1248,7 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
                                       int32_t n, int32_t pt, int32_t ph, int32_t pw, const float* context, int32_t L,
                                       const uint8_t* text_mask, const uint8_t* video_mask, float loss_scale,
                                       float* loss_out, float* logits_out, void* workspace, int64_t workspace_bytes,
-                                      int32_t prec, phk_stream_t s) {
+                                      int32_t prec, phk_stream_t s, const phk_dropout_t* dropout) {
   PHK_REQUIRE(m && grads && ids_in && loss_out && workspace, PHK_E_ARG, "maskgit_train_step: null pointer");
   PHK_REQUIRE(b > 0 && n > 0 && (int64_t)pt * ph * pw == n, PHK_E_SHAPE, "video patch shape must cover the token sequence");
   PHK_REQUIRE(n <= m->max_seq_len, PHK_E_SHAPE,
@@ -1136,6 +1269,9 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   PHK_REQUIRE(T->layers && GT->layers && T->depth > 0 && GT->depth == T->depth && !T->causal, PHK_E_ARG,
               "maskgit_train_step: transformer table / gradient table mismatch");
   PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "maskgit_train_step: dim must be a multiple of 4");
+  PHK_REQUIRE(!dropout || (dropout->attn_p >= 0.f && dropout->attn_p <= 1.f && dropout->ff_p >= 0.f && dropout->ff_p <= 1.f),
+              PHK_E_ARG, "maskgit_train_step: dropout probabilities must lie in [0, 1]");
+  const bool drop_on = dropout && (dropout->attn_p > 0.f || dropout->ff_p > 0.f);
   cudaStream_t st = to_stream(s);
   void** prog = g_progress_events;  // one-shot: consumed by this call
   const int nprog = g_progress_count;
@@ -1170,6 +1306,26 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   LayerSave* sv = new (std::nothrow) LayerSave[T->depth];
   PHK_REQUIRE(sv, PHK_E_ARG, "maskgit_train_step: out of host memory");
   struct Free { LayerSave* p; ~Free() { delete[] p; } } free_sv{sv};
+  // dropout: site s of layer l (0 self-attention, 1 cross-attention, 2 FF) draws from counters offset + bases[l][s]
+  uint64_t (*bases)[3] = drop_on ? new (std::nothrow) uint64_t[T->depth][3] : nullptr;
+  PHK_REQUIRE(!drop_on || bases, PHK_E_ARG, "maskgit_train_step: out of host memory");
+  struct FreeBases { uint64_t (*p)[3]; ~FreeBases() { delete[] p; } } free_bases{bases};
+  if (drop_on) dropout_layout(m, b, n, context ? L : 0, bases);
+  auto site = [&](float p, int l, int k) {  // p == 0: the site is off
+    DropSite d{0.f, 0.f, 0u, 0u, 0u};
+    if (drop_on && p > 0.f) {
+      d.p = p; d.scale = 1.0f / (1.0f - p);
+      d.k0 = (uint32_t)dropout->seed; d.k1 = (uint32_t)(dropout->seed >> 32);
+      d.base = dropout->offset + bases[l][k];
+    }
+    return d;
+  };
+  const float attn_p = dropout ? dropout->attn_p : 0.f, ff_p = dropout ? dropout->ff_p : 0.f;
+  // the attention backward's scratch; the forward's explicit attention path (dropout) uses it too
+  const int nk_cross = L + 8;
+  const int64_t as1 = attn_bwd_scratch_floats(b, H, n, n, DH), as2 = attn_bwd_scratch_floats(b, H, n, nk_cross, DH);
+  float* asc = ar.f(as1 > as2 ? as1 : as2);
+  PHK_REQUIRE(asc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (attention scratch)");
   phk_attn_geom_t ag;
   const float* xin = x;
   for (int l = 0; l < T->depth; ++l) {
@@ -1196,7 +1352,13 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
     ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)n * 2 * I; ag.k_tok = 2 * I;
     ag.o_outer = ag.q_outer; ag.o_tok = I; ag.mask_off_from = -1; ag.scale = 8.f;
     PHK_REQUIRE(A.num_null_kv == 0, PHK_E_UNSUPPORTED, "maskgit_train_step: self-attention null-kv is not supported");
-    PHK_TRY(phk_attention(S.q1, S.kv1, A.null_kv, A.q_scale, A.k_scale, bias, video_mask, nullptr, S.o1, &ag, s));
+    const DropSite d_self = site(attn_p, l, 0);
+    if (d_self.p > 0.f) {
+      const AttnBwdGeom g1{b, H, n, n, 0, DH};
+      PHK_TRY(attention_forward_dropout(S.q1, S.kv1, A, bias, video_mask, S.o1, g1, asc, st, d_self));
+    } else {
+      PHK_TRY(phk_attention(S.q1, S.kv1, A.null_kv, A.q_scale, A.k_scale, bias, video_mask, nullptr, S.o1, &ag, s));
+    }
     PHK_TRY(linear_fwd(prec, tc, S.o1, A.wo, S.x2, R, D, I, nullptr, S.x1, s));  // x2 = x1 + o Wo^T
     const bool cross = Ly.has_cross && context;
     if (cross) {
@@ -1212,7 +1374,14 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
       ag.n_outer = b; ag.n_inner = 1; ag.n_q = n; ag.n_k = L; ag.heads = H; ag.dim_head = DH; ag.num_null_kv = Cx.num_null_kv;
       ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)L * 2 * I; ag.k_tok = 2 * I;
       ag.o_outer = ag.q_outer; ag.o_tok = I; ag.kv_outer_mod = b; ag.mask_outer_mod = b; ag.mask_off_from = -1; ag.scale = 8.f;
-      PHK_TRY(phk_attention(S.q2, S.ckv, Cx.null_kv, Cx.q_scale, Cx.k_scale, nullptr, text_mask, nullptr, S.o2, &ag, s));
+      const DropSite d_cross = site(attn_p, l, 1);
+      if (d_cross.p > 0.f) {
+        PHK_REQUIRE(Cx.num_null_kv <= 8, PHK_E_UNSUPPORTED, "maskgit_train_step: more than 8 null key/values");
+        const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
+        PHK_TRY(attention_forward_dropout(S.q2, S.ckv, Cx, nullptr, text_mask, S.o2, g2, asc, st, d_cross));
+      } else {
+        PHK_TRY(phk_attention(S.q2, S.ckv, Cx.null_kv, Cx.q_scale, Cx.k_scale, nullptr, text_mask, nullptr, S.o2, &ag, s));
+      }
       PHK_TRY(linear_fwd(prec, tc, S.o2, Cx.wo, S.x3, R, D, I, nullptr, S.x2, s));  // x3 = x2 + o2 Wo^T
     } else {
       PHK_CUDA(cudaMemcpyAsync(S.x3, S.x2, R * D * 4, cudaMemcpyDeviceToDevice, st));
@@ -1220,7 +1389,13 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
     // feed forward (attention.py:45-53)
     PHK_TRY(phk_layernorm(S.x3, Ly.ff.ln_g, Ly.ff.ln_b, S.xn3, nullptr, R, D, 0, 0, 0, 0, s));
     PHK_TRY(linear_fwd(prec, tc, S.xn3, Ly.ff.w1, S.h, R, 2 * inner, D, nullptr, nullptr, s));
-    PHK_TRY(phk_geglu(S.h, S.g, R, inner, s));
+    const DropSite d_ff = site(ff_p, l, 2);
+    if (d_ff.p > 0.f) {
+      PHK_KERNEL_LAUNCH(geglu_dropout_kernel, dim3(ew_grid_fwd(R * inner)), dim3(256), (size_t)(0), st, S.h, S.g, R, inner, d_ff);
+      PHK_LAUNCH_CHECK();
+    } else {
+      PHK_TRY(phk_geglu(S.h, S.g, R, inner, s));
+    }
     PHK_TRY(linear_fwd(prec, tc, S.g, Ly.ff.w2, xout, R, D, inner, nullptr, S.x3, s));  // x4 = x3 + g W2^T
     xin = xout;
   }
@@ -1278,10 +1453,7 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   float* dg = ar.f(R * inner_max);
   float* dckv = context ? ar.f(CR * 2 * I) : nullptr;
   float* dctxn = context ? ar.f(CR * (dc_max > 0 ? dc_max : 1)) : nullptr;
-  const int nk_cross = L + 8;
-  const int64_t as1 = attn_bwd_scratch_floats(b, H, n, n, DH), as2 = attn_bwd_scratch_floats(b, H, n, nk_cross, DH);
-  float* asc = ar.f(as1 > as2 ? as1 : as2);
-  PHK_REQUIRE(dq && dkv && dob && dh && dg && asc && (!context || (dckv && dctxn)), PHK_E_WORKSPACE,
+  PHK_REQUIRE(dq && dkv && dob && dh && dg && (!context || (dckv && dctxn)), PHK_E_WORKSPACE,
               "maskgit_train_step: workspace too small (gradients)");
   float* dx = dxa;      // d loss / d (current residual stream)
   float* dx_alt = dxb;
@@ -1295,7 +1467,7 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
     // feed forward: x4 = x3 + geglu(LN(x3) W1^T) W2^T
     PHK_TRY(dgrad_p(prec, tc, dx, Ly.ff.w2, dg, R, D, inner, 0, s));
     PHK_TRY(wgrad_p(prec, tc, dx, S.g, (float*)Gy.ff.w2, R, D, inner, s));
-    PHK_KERNEL_LAUNCH(geglu_bwd_kernel, dim3(ew_grid(R * inner)), dim3(256), (size_t)(0), st, S.h, dg, dh, R, inner);
+    PHK_KERNEL_LAUNCH(geglu_bwd_kernel, dim3(ew_grid(R * inner)), dim3(256), (size_t)(0), st, S.h, dg, dh, R, inner, site(ff_p, l, 2));
     PHK_LAUNCH_CHECK();
     PHK_TRY(wgrad_p(prec, tc, dh, S.xn3, (float*)Gy.ff.w1, R, 2 * inner, D, s));
     PHK_TRY(dgrad_p(prec, tc, dh, Ly.ff.w1, dtmp, R, 2 * inner, D, 0, s));
@@ -1309,7 +1481,8 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
       PHK_TRY(dgrad_p(prec, tc, dx, Cx.wo, dob, R, D, I, 0, s));
       PHK_TRY(wgrad_p(prec, tc, dx, S.o2, (float*)Gx.wo, R, D, I, s));
       const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
-      PHK_TRY(attention_backward(S.q2, S.ckv, Cx, Gx, nullptr, text_mask, dob, dq, dckv, nullptr, g2, asc, st, prec == PHK_PREC_BF16));
+      PHK_TRY(attention_backward(S.q2, S.ckv, Cx, Gx, nullptr, text_mask, dob, dq, dckv, nullptr, g2, asc, st, prec == PHK_PREC_BF16,
+                                 site(attn_p, l, 1)));
       PHK_TRY(wgrad_p(prec, tc, dq, S.xn2, (float*)Gx.wq, R, I, D, s));
       PHK_TRY(dgrad_p(prec, tc, dq, Cx.wq, dtmp, R, I, D, 0, s));
       PHK_TRY(ln_backward(S.x2, Cx.norm_g, dtmp, dx, 1, (float*)Gx.norm_g, nullptr, stats, R, D, st));
@@ -1324,7 +1497,8 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
       PHK_TRY(dgrad_p(prec, tc, dx, A.wo, dob, R, D, I, 0, s));
       PHK_TRY(wgrad_p(prec, tc, dx, S.o1, (float*)GA.wo, R, D, I, s));
       const AttnBwdGeom g1{b, H, n, n, 0, DH};
-      PHK_TRY(attention_backward(S.q1, S.kv1, A, GA, bias, video_mask, dob, dq, dkv, dbias, g1, asc, st, prec == PHK_PREC_BF16));
+      PHK_TRY(attention_backward(S.q1, S.kv1, A, GA, bias, video_mask, dob, dq, dkv, dbias, g1, asc, st, prec == PHK_PREC_BF16,
+                                 site(attn_p, l, 0)));
       PHK_TRY(wgrad_p(prec, tc, dq, S.xn1, (float*)GA.wq, R, I, D, s));
       PHK_TRY(wgrad_p(prec, tc, dkv, S.x1, (float*)GA.wkv, R, 2 * I, D, s));
       PHK_TRY(dgrad_p(prec, tc, dq, A.wq, dtmp, R, I, D, 0, s));

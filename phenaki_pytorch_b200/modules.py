@@ -101,7 +101,8 @@ class Transformer(nn.Module):
                  ff_dropout=0.0):
         super().__init__()
         self.dim, self.depth, self.causal, self.dim_head, self.heads = dim, depth, causal, dim_head, heads
-        self.attn_dropout, self.ff_dropout = attn_dropout, ff_dropout  # inference ignores them; the training step refuses > 0
+        # applied by the training step in training mode (phk_dropout_t); the inference entry points ignore them
+        self.attn_dropout, self.ff_dropout = attn_dropout, ff_dropout
         self.layers = nn.ModuleList([])
         for _ in range(depth):
             self.layers.append(nn.ModuleList([

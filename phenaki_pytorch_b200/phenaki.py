@@ -241,13 +241,18 @@ class _TokenTransformer(nn.Module):
         wgmma bf16 products, everything else is fp32 in both modes): returns (loss 0-d tensor,
         GradKeep with d(loss_scale * loss)/d(parameter), logits or None).  ``labels`` given: Linear(dim, 1) head + BCE
         with logits (TokenCritic; or ``head`` = SelfCritic.to_pred on this MaskGit, gradients laid out for
-        ``owner.parameters()``); otherwise masked cross entropy against ``targets`` at ``token_mask``."""
+        ``owner.parameters()``); otherwise masked cross entropy against ``targets`` at ``token_mask``.
+        In training mode (``self.training``) the transformer's ``attn_dropout`` / ``ff_dropout`` apply as the
+        reference's nn.Dropout does; the masks come from fresh counters of the device's noise generator (include/phk.h,
+        phk_dropout_t), so every call draws new masks and ``torch.manual_seed`` repeats them."""
         lib = L.lib()
         bce = labels is not None
         assert bce or not self.is_critic, "a TokenCritic trains against labels"
-        if self.transformer.attn_dropout > 0 or self.transformer.ff_dropout > 0:
-            raise NotImplementedError("the training step has no dropout kernels: construct with attn_dropout = "
-                                      "ff_dropout = 0 (the reference's defaults)")
+        attn_p, ff_p = float(self.transformer.attn_dropout), float(self.transformer.ff_dropout)
+        for name, p in (("attn_dropout", attn_p), ("ff_dropout", ff_p)):
+            if not 0.0 <= p <= 1.0:
+                raise ValueError(f"{name} has to be between 0 and 1, but got {p}")
+        dropout_on = self.training and (attn_p > 0 or ff_p > 0)
         ids_in = L.require_cuda(ids_in, "token ids", torch.int64)
         b, n = ids_in.shape
         assert _prod(patch_shape) == n, "video patch shape must cover the token sequence"
@@ -289,6 +294,13 @@ class _TokenTransformer(nn.Module):
             nbytes = lib.phk_maskgit_train_workspace_bytes(C.byref(table), b, n, ctx_len, int(bce), prec)
             ws = self._ws.get(nbytes, dev)
             pt, ph, pw = (int(v) for v in patch_shape)
+            dropout = None
+            if dropout_on:  # reserve exactly the counters the step's masks use (the C side owns the layout)
+                counters = int(lib.phk_maskgit_train_dropout_counters(C.byref(table), b, n, ctx_len))
+                assert counters >= 0, "phk_maskgit_train_dropout_counters: bad arguments"
+                seed = _noise_seed(dev)
+                offset = _rng_take(dev, seed, counters)
+                dropout = C.byref(L.DropoutT(attn_p, ff_p, seed & (2 ** 64 - 1), offset))
             plan = self._overlap_plan(gk, owner if owner is not None else self, dev) if overlap_all_reduce else None
             if plan is not None:  # the C call records these events as gradient groups become final
                 L.check(lib.phk_train_set_progress_events(plan["handles"], len(plan["events"])), "phk_train_set_progress_events")
@@ -296,7 +308,7 @@ class _TokenTransformer(nn.Module):
                                                L.ptr(token_mask), L.ptr(labels), b, n, pt, ph, pw, L.ptr(context),
                                                ctx_len, L.ptr(text_mask), L.ptr(video_mask), float(loss_scale),
                                                L.ptr(loss), L.ptr(logits), L.ptr(ws), ws.numel(), prec,
-                                               L.stream_ptr()),
+                                               L.stream_ptr(), dropout),
                     "phk_maskgit_train_step")
             if plan is not None:
                 self._launch_overlapped_all_reduce(gk, plan)
@@ -855,9 +867,9 @@ class Phenaki(nn.Module):
                noise_fn=None):
         """phenaki_pytorch.py:418-560.  Extra keywords: ``text_embeds`` (precomputed T5 output, SURVEY 8f-4),
         ``return_token_ids`` (skip the final C-ViViT decode), ``noise_fn`` (inject the uniform draws)."""
-        # eval_decorator (phenaki_pytorch.py:31-38).  The mode flags only matter to dropout, which the kernels do not have
-        # (construction rejects attn_dropout / ff_dropout > 0 for training); the walk over ~600 submodules cost ~2 ms of
-        # host time per call, twice per sample, so it is skipped when the model is already in eval mode.
+        # eval_decorator (phenaki_pytorch.py:31-38).  The mode flags only matter to dropout, which only the training step
+        # applies (the sampling kernels have none); the walk over ~600 submodules cost ~2 ms of host time per call,
+        # twice per sample, so it is skipped when the model is already in eval mode.
         was_training = self.training
         if was_training:
             self.eval()
