@@ -205,43 +205,11 @@ int phk_gemm_bf16_qkv(const void* xn, const void* xraw, int64_t lda, const void*
                       void* Qn, void* KVn, int64_t M, int32_t I, int32_t K, const float* q_scale, const float* k_scale,
                       float sim_scale, phk_stream_t s);
 
-/* x = A W^T (+bias) + x IN PLACE (C is the fp32 residual stream, nn.Linear + residual of attention.py:322-330) and, from
- * the same epilogue, the LayerNorm the NEXT sub-block applies to x: ln_out[M, ln_ld] = bf16(LayerNorm(x) * ln_g + ln_b)
- * (ln_b may be NULL), raw_out (optional) = bf16(x).  N = row width in {128, 256, 512, 1024}: the N / 128 CTAs of a
- * 128-row tile form a cluster and sum their row statistics through distributed shared memory. */
-int phk_gemm_bf16_ln(const void* A, int64_t lda, const void* W, int64_t ldw, float* C, int64_t ldc, int64_t M, int32_t N,
-                     int32_t K, const float* bias, const float* ln_g, const float* ln_b, float ln_eps, void* ln_out,
-                     void* raw_out, int64_t ln_ld, phk_stream_t s);
-
-/* The same product with the row statistics exchanged through global memory instead of a cluster (the N / 128 CTAs of a
- * 128-row tile are ordinary CTAs of a grid of at most one CTA per SM, all resident; no GPC-local cluster placement).
- *   stat_ws : PHK_LN_STAT_BYTES bytes of device scratch, 16-byte aligned, any content;
- *   counters: PHK_LN_COUNTERS zero-initialised 32-bit device words, consumed by the call (left non-zero) -- give every
- *             call of a stream-ordered sequence its own words and clear them together once per sequence. */
-#define PHK_LN_STAT_BYTES (2 * 132 * 128 * 8)
-#define PHK_LN_COUNTERS 160
-int phk_gemm_bf16_ln_ws(const void* A, int64_t lda, const void* W, int64_t ldw, float* C, int64_t ldc, int64_t M,
-                        int32_t N, int32_t K, const float* bias, const float* ln_g, const float* ln_b, float ln_eps,
-                        void* ln_out, void* raw_out, int64_t ln_ld, void* stat_ws, uint32_t* counters, phk_stream_t s);
-
 /* PHK_PREC_BF16X3 operand split: x fp32 [rows, ld] (K valid columns) -> bf16 [rows, 3 * Kp], Kp = K rounded up to 8:
  * [hi | hi | lo] (weights == 0: the activation side) or [hi | lo | hi] (weights != 0), hi = bf16(x), lo = bf16(x - hi),
  * zero in the padding columns.  With both sides split this way a plain bf16 GEMM over K' = 3 Kp computes
  * A_hi W_hi + A_hi W_lo + A_lo W_hi. */
 int phk_split3(const float* x, int64_t ld, void* out, int64_t rows, int32_t K, int32_t weights, phk_stream_t s);
-
-/* debug aid: per-CTA clock64 phase stamps of phk_gemm_bf16 (16 x int64 per CTA); NULL disables */
-int phk_debug_gemm_trace(long long* device_buffer);
-/* tests: GEMM variant selector, kept for ABI compatibility: modes <= 3 are accepted and every mode runs the one
- * 128x128-tile wgmma kernel (the CTA-pair variants of modes 2 and 3 need an MMA Hopper does not have). */
-int phk_debug_gemm_mode(int32_t mode);
-/* tests / A-B measurements: declare (1) or withdraw (0), for the calling thread, that the W operands of the following
- * phk_gemm_bf16* calls are not written by earlier kernels of the stream -- the kernel then requests their first tiles before
- * its programmatic-dependent-launch wait.  The forward drivers (phk_cvivit_*, phk_maskgit_*) set this themselves. */
-int phk_debug_static_weights(int32_t on);
-/* tests: phk_attention_tc* variant selector, kept for ABI compatibility: values <= 1 are accepted and one kernel serves
- * all of them (probabilities stay in registers as the A operand of P.V). */
-int phk_debug_attention_tc_variant(int32_t variant);
 
 /* GEGLU (attention.py:40-43): out[r, j] = gelu_erf(h[r, inner + j]) * h[r, j] */
 int phk_geglu(const float* h, float* out, int64_t rows, int32_t inner, phk_stream_t s);
@@ -410,8 +378,8 @@ int phk_cfg_combine(const float* cond, const float* null_out, float cond_scale, 
  * tap_proj [rows, bits] = LFQ pre-sign projection.
  * Launch cost: the ~75 launches of one call are a pure function of (table contents, buffers, shape, prec).  With
  * spatial_bias given and no taps, the second call with an identical key is captured into a CUDA graph on a
- * library-owned stream and later calls replay it on `s` (one cudaGraphLaunch; env PHK_GRAPH=0 keeps every call
- * eager).  The graph only bakes in addresses: new data in the same buffers (video, weights updated in place) is
+ * library-owned stream and later calls replay it on `s` (one cudaGraphLaunch; calls stay eager while the per-family
+ * profiler is on).  The graph only bakes in addresses: new data in the same buffers (video, weights updated in place) is
  * honoured; a table with different pointers or dims is a different key. */
 int64_t phk_cvivit_workspace_bytes(const phk_cvivit_t* m, int32_t B, int32_t F, int32_t prec);
 int phk_cvivit_encode(const phk_cvivit_t* m, const float* video, int32_t B, int32_t F,
@@ -562,7 +530,7 @@ int phk_rng_advance(uint64_t* rng_state, uint64_t stride, phk_stream_t s);
  * Prime prefix: token_in [b, prime_len + n] int64 holds the prime ids in the first prime_len columns (written once by the
  * caller); with prime_len == 0 pass token_in == ids.  pt*ph*pw == prime_len + n.
  * k_remask == 0 is the first iteration (every token masked: mask must be all ones).  rng_state: device uint64[2]
- * {seed, offset}.  With PHK_STEP_GRAPH=1 the launch sequence is captured into a CUDA graph the second time the same
+ * {seed, offset}.  With pos_bias given, the launch sequence is captured into a CUDA graph the second time the same
  * arguments are seen (same table contents, pointers, shape, scalars) and later calls are ONE cudaGraphLaunch -- the
  * noise key and the token state live in device memory, so nothing that changes between calls is baked in.  Buffers
  * must therefore be stable across calls.  bf16 weights, cond_scale != 1 (as phk_maskgit_sample_step). */
@@ -577,7 +545,7 @@ int phk_maskgit_demask_iteration(const phk_maskgit_t* m, const phk_maskgit_t* cr
                                  float noise_mult, int32_t skip_critic, void* workspace, int64_t workspace_bytes,
                                  phk_stream_t s);
 
-/* tests / A-B runs: 1 = phk_maskgit_demask_iteration replays a CUDA graph, 0 = eager, < 0 = the PHK_STEP_GRAPH default */
+/* tests: 1 = phk_maskgit_demask_iteration replays a CUDA graph, 0 = eager, < 0 = the default (on) */
 int phk_debug_step_graph(int32_t on);
 
 /* ------------------------------------------------------------------------------------------ */

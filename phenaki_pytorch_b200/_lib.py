@@ -9,7 +9,6 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PHK_LIB") or os.path.join(_HERE, "libphk.so")  # PHK_LIB: an A/B build of the same ABI (tools/ only)
 
 PREC_F32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
-LN_STAT_BYTES, LN_COUNTERS = 2 * 132 * 128 * 8, 160   # phk_gemm_bf16_ln_ws scratch (include/phk.h)
 
 
 def default_precision():
@@ -118,10 +117,6 @@ PROTOTYPES = {
     "phk_gemm_f32": [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp, i64, i64, i64, vp],
     "phk_gemm_bf16": [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp, i64, i64, i64, i32, vp],
     "phk_gemm_bf16_x2": [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp],
-    "phk_debug_gemm_trace": [vp],
-    "phk_debug_gemm_mode": [i32],
-    "phk_debug_static_weights": [i32],
-    "phk_debug_attention_tc_variant": [i32],
     "phk_geglu": [vp, vp, i64, i32, vp],
     "phk_attention": [vp, vp, vp, vp, vp, vp, vp, vp, vp, C.POINTER(AttnGeomT), vp],
     "phk_attention_tc_scratch_bytes": [i32, i32, i32],
@@ -129,8 +124,6 @@ PROTOTYPES = {
     "phk_attention_tc_bf16": [vp, i64, vp, i64, vp, vp, i32, i32, i32, vp],
     "phk_attention_small_bf16": [vp, vp, vp, vp, C.POINTER(AttnGeomT), vp],
     "phk_attention_mid_bf16": [vp, i64, vp, i64, vp, vp, i32, i32, i32, vp],
-    "phk_gemm_bf16_ln": [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp, vp, f32, vp, vp, i64, vp],
-    "phk_gemm_bf16_ln_ws": [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp, vp, f32, vp, vp, i64, vp, vp, vp],
     "phk_train_set_progress_events": [vp, i32],
     "phk_split3": [vp, i64, vp, i64, i32, i32, vp],
     "phk_cross_kv_pack": [vp, vp, vp, i32, vp, i32, i32, i32, i32, vp, vp, vp],

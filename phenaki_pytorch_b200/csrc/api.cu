@@ -4,7 +4,6 @@
 // No host synchronisation, no allocation: scratch is carved from the caller's workspace.
 #include "phk_common.cuh"
 #include <atomic>
-#include <cstdlib>
 #include <cstring>
 #include <cstdio>
 #include <mutex>
@@ -84,18 +83,13 @@ struct TfCall {
   int dup_halves;
 };
 
-constexpr int kFuseLnDefault = 0;     // PHK_FUSE_LN default: 0 separate LayerNorm kernels, 1 cluster epilogue, 2 global exchange
-constexpr int kLnFusedLaunches = 64;  // LayerNorm-in-epilogue GEMMs per transformer call that get their own arrival counters
-
 static int64_t tf_scratch_bytes(const phk_transformer_t* T, int64_t R) {
   const int64_t I = (int64_t)T->heads * T->dim_head;
   int64_t inner = 0;
   for (int l = 0; l < T->depth; ++l) inner = inner > T->layers[l].ff.inner ? inner : T->layers[l].ff.inner;
   // xn, q, kv, o, h(2*inner), g(inner)  -- all fp32 in parity mode
   // + head-major bf16 q/k/v^T operands of the tensor-core attention (bf16 mode): 3 * R * I * 2 bytes + padding
-  // + the statistics exchange and arrival counters of the LayerNorm-in-epilogue GEMMs (phk_gemm_bf16_ln_ws)
-  return 256 * 14 + R * 4 * (T->dim + I + 2 * I + I + 2 * inner + inner) + R * I * 6 + 64 * 64 * 2 * (R / 64 + 64) +
-         PHK_LN_STAT_BYTES + kLnFusedLaunches * PHK_LN_COUNTERS * 4;
+  return 256 * 14 + R * 4 * (T->dim + I + 2 * I + I + 2 * inner + inner) + R * I * 6 + 64 * 64 * 2 * (R / 64 + 64);
 }
 
 static int64_t tf_kmax(const phk_transformer_t* T) {  // largest K of a transformer's nn.Linear products
@@ -133,9 +127,6 @@ static int linear(const Lin& ln, const void* act, int64_t lda, const float* w32,
 static int transformer_forward(const TfCall& c, Arena scratch, float* out, void* out_h, cudaStream_t st) {
   const phk_transformer_t* T = c.T;
   const bool h16 = c.prec == PHK_PREC_BF16;
-  // (StaticWeightsScope -- requesting the first weight tiles BEFORE the programmatic-dependent-launch wait -- is not used
-  //  here: griddepcontrol.wait appears to drain the thread's outstanding bulk copies first, so the activation tiles would
-  //  be requested a full TMA latency later.  The hint stays available through phk_debug_static_weights.)
   PHK_REQUIRE(c.prec == PHK_PREC_F32 || c.prec == PHK_PREC_BF16X3 || h16, PHK_E_ARG, "transformer: unknown precision mode");
   PHK_REQUIRE(c.lin.prec == c.prec, PHK_E_ARG, "transformer: contraction descriptor not initialised");
   const int D = T->dim, H = T->heads, DH = T->dim_head, I = H * DH;
@@ -156,32 +147,6 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
   float* x = c.x;
   float* x_alt = c.x_alt;
 
-  // bf16 mode, opt-in (PHK_FUSE_LN=1): the LayerNorm that follows a residual GEMM (out-projection -> cross-attention /
-  // feed-forward norm, feed-forward -> the next layer's attention norm when no PEG sits in between) computed by that
-  // GEMM's epilogue (phk_gemm_bf16_ln: row statistics summed over a cluster of N / 128 CTAs through distributed shared
-  // memory).  Correct (tests/test_gpu_fused_qkv.py); off by default because a cluster of 4 full-SM CTAs needs 4 free SMs
-  // of one GPC, so few clusters are resident at once and the row tiles of 4608 tokens take two waves.
-  // PHK_FUSE_LN=2: the same fusion without clusters -- the CTAs of a row tile exchange the statistics through global
-  // memory (phk_gemm_bf16_ln_ws; one set of arrival counters per fused launch, cleared together by one memset here).
-  static const int fuse_ln_env = [] { const char* e = std::getenv("PHK_FUSE_LN"); return e && e[0] >= '0' && e[0] <= '2' ? e[0] - '0' : kFuseLnDefault; }();
-  const bool fuse_ln = fuse_ln_env != 0 && h16 && (D == 128 || D == 256 || D == 512 || D == 1024);
-  void* ln_stat = nullptr;
-  uint32_t* ln_counters = nullptr;
-  int ln_launch = 0;
-  if (fuse_ln && fuse_ln_env == 2) {
-    ln_stat = scratch.take(PHK_LN_STAT_BYTES);
-    ln_counters = (uint32_t*)scratch.take((int64_t)kLnFusedLaunches * PHK_LN_COUNTERS * 4);
-    PHK_REQUIRE(ln_stat && ln_counters, PHK_E_WORKSPACE, "transformer: workspace too small (LayerNorm statistics exchange)");
-    PHK_CUDA(cudaMemsetAsync(ln_counters, 0, (size_t)kLnFusedLaunches * PHK_LN_COUNTERS * 4, st));
-  }
-  // residual GEMM + the following LayerNorm in one launch (cluster or global-exchange variant)
-  auto gemm_ln = [&](const void* a, int64_t lda, const void* w, int64_t ldw, float* xio, int64_t rows, int K, const float* g,
-                     const float* b, void* ln_o, void* raw_o) -> int {
-    if (ln_stat && ln_launch < kLnFusedLaunches)
-      return phk_gemm_bf16_ln_ws(a, lda, w, ldw, xio, D, rows, D, K, nullptr, g, b, 1e-5f, ln_o, raw_o, D, ln_stat,
-                                 ln_counters + (int64_t)(ln_launch++) * PHK_LN_COUNTERS, s);
-    return phk_gemm_bf16_ln(a, lda, w, ldw, xio, D, rows, D, K, nullptr, g, b, 1e-5f, ln_o, raw_o, D, s);
-  };
   // bf16 mode: cross-attention on packed operands -- the text keys / values of all layers are l2-normalised, scaled and
   // converted ONCE per call (phk_cross_kv_pack) instead of once per attention CTA, and the q projection's epilogue writes the
   // normalised bf16 queries (phk_gemm_bf16_qnorm): the attention kernel is 32 MMAs behind an 8 KB copy.
@@ -190,8 +155,7 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
   int cross_nnull = 0;
 #ifndef PHK_CUDA_EMU
   {
-    static const bool pack_env = [] { const char* e = std::getenv("PHK_CROSS_PACK"); return !(e && e[0] == '0'); }();
-    bool ok = pack_env && h16 && c.ctx_kv && DH == 64 && I % 128 == 0 && T->depth <= 16 && c.seq.n_inner == 1 && c.seq.tok == 1 &&
+    bool ok = h16 && c.ctx_kv && DH == 64 && I % 128 == 0 && T->depth <= 16 && c.seq.n_inner == 1 && c.seq.tok == 1 &&
               c.seq.outer == c.seq.n_tok && c.ctx_b > 0;
     for (int l = 0; ok && l < T->depth; ++l) {
       const phk_layer_t& Ly = T->layers[l];
@@ -218,7 +182,6 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
     }
   }
 #endif
-  bool ln_ready = false;  // xn (+ xraw) already hold this layer's self-attention LayerNorm (written by the previous FF2)
   for (int l = 0; l < T->depth; ++l) {
     const phk_layer_t& L = T->layers[l];
     // first layer of a CFG pair with identical halves: PEG + self-attention on the first half only
@@ -226,7 +189,6 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
     const int64_t Rl = dup ? R / 2 : R;
     const int n_outer = dup ? c.seq.n_outer / 2 : c.seq.n_outer;
     const int pegB = dup ? c.pegB / 2 : c.pegB;
-    bool norm_done = false;  // xn already holds the LayerNorm the next sub-block needs (written by a GEMM epilogue)
     if (L.has_peg) {  // x = peg(x) + x
       PHK_REQUIRE((int64_t)pegB * c.pegT * c.pegH * c.pegW == Rl, PHK_E_SHAPE, "PEG: video shape does not cover the tokens");
       PHK_TRY(phk_peg3d(x, L.peg.w, L.peg.b, x_alt, pegB, c.pegT, c.pegH, c.pegW, D, L.peg.causal, c.peg_layout, s));
@@ -234,8 +196,7 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
     }
     {  // x = self_attn(x) + x ; q from LN(x), k/v from RAW x (attention.py:140-144)
       const phk_attn_t& A = L.self_attn;
-      if (!ln_ready) PHK_TRY(phk_layernorm(x, A.norm_g, A.norm_b, xn, xraw, Rl, D, h16, 0, 0, 0, s));
-      ln_ready = false;
+      PHK_TRY(phk_layernorm(x, A.norm_g, A.norm_b, xn, xraw, Rl, D, h16, 0, 0, 0, s));
       phk_attn_geom_t g;
       std::memset(&g, 0, sizeof(g));
       g.n_outer = n_outer; g.n_inner = c.seq.n_inner; g.n_q = c.seq.n_tok; g.n_k = c.seq.n_tok;
@@ -251,15 +212,11 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
       // 16 < n <= 64 (the spatial transformer's 8 x 8 frames): warp-level MMAs, all (sequence, head) CTAs resident at once
       bool mid_ok = false;
 #ifndef PHK_CUDA_EMU
-      // (at exactly 64 tokens the wgmma kernel is used, so the MMA kernel takes 17..63 tokens, which used to fall back to
-      //  the fp32 kernel;
-      //  PHK_MID_ATTN_MMA=1 forces it for 64 as well, =0 disables it)
-      static const int mid_env = [] { const char* e = std::getenv("PHK_MID_ATTN_MMA"); return e ? (e[0] == '0' ? 0 : 2) : 1; }();
-      mid_ok = mid_env != 0 && plain && !T->causal && c.seq.n_inner == 1 && c.seq.tok == 1 && c.seq.outer == c.seq.n_tok &&
-               c.seq.n_tok > 16 && c.seq.n_tok <= (mid_env == 2 ? 64 : 63);
+      // (at exactly 64 tokens the wgmma kernel is used, so the MMA kernel takes 17..63 tokens)
+      mid_ok = plain && !T->causal && c.seq.n_inner == 1 && c.seq.tok == 1 && c.seq.outer == c.seq.n_tok &&
+               c.seq.n_tok > 16 && c.seq.n_tok < 64;
 #endif
-      static const bool fuse_qkv = [] { const char* e = std::getenv("PHK_FUSE_QKV"); return !(e && e[0] == '0'); }();
-      if ((tc_ok || small_ok || mid_ok) && fuse_qkv && I % 128 == 0 && A.wq_h && A.wkv_h) {
+      if ((tc_ok || small_ok || mid_ok) && I % 128 == 0 && A.wq_h && A.wkv_h) {
         // q / k,v projections in ONE launch whose epilogue writes the attention core's bf16 operands directly
         // (l2-normalised q, k times their learned scales, the similarity scale 8 folded into q, v converted): no fp32
         // q / kv round trip and no separate normalisation pass (attention.py:146-157)
@@ -279,7 +236,7 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
           PHK_TRY(linear(c.lin, xn, D, A.wq, A.wq_h, D, q, I, Rl, I, D, nullptr, nullptr, s));
           PHK_TRY(linear(c.lin, h16 ? xraw : (const void*)x, D, A.wkv, A.wkv_h, D, kv, 2 * I, Rl, 2 * I, D, nullptr, nullptr, s));
         }
-        if (tc_ok) {  // wgmma path from fp32 projections (PHK_FUSE_QKV=0): operands prepared by attention_prep_kernel
+        if (tc_ok) {  // wgmma path from fp32 projections (heads * 64 not a multiple of 128): operands prepared by attention_prep_kernel
           const int64_t ab = phk_attention_tc_scratch_bytes(n_outer, c.seq.n_tok, H);
           Arena tmp = scratch;
           void* asc = tmp.take(ab);
@@ -289,25 +246,14 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
           PHK_TRY(phk_attention(q, kv, A.null_kv, A.q_scale, A.k_scale, c.attn_bias, c.self_mask, T->alibi_slopes, o, &g, s));
         }
       }
-      if (fuse_ln && A.wo_h) {  // x += o Wo^T and the next sub-block's LayerNorm of the new x in one kernel
-        const bool to_cross = L.has_cross && c.ctx_kv;
-        const float* ng = to_cross ? L.cross_attn.norm_g : L.ff.ln_g;
-        const float* nb = to_cross ? L.cross_attn.norm_b : L.ff.ln_b;
-        PHK_TRY(gemm_ln(o, I, A.wo_h, I, x, Rl, I, ng, nb, xn, nullptr));
-        norm_done = true;
-      } else {
-        PHK_TRY(linear(c.lin, o, I, A.wo, A.wo_h, I, x, D, Rl, D, I, nullptr, x, s));
-      }
+      PHK_TRY(linear(c.lin, o, I, A.wo, A.wo_h, I, x, D, Rl, D, I, nullptr, x, s));
     }
-    if (dup) {  // the null half continues from the same rows
+    if (dup)  // the null half continues from the same rows
       PHK_CUDA(cudaMemcpyAsync(x + Rl * D, x, Rl * D * 4, cudaMemcpyDeviceToDevice, st));
-      if (norm_done) PHK_CUDA(cudaMemcpyAsync((char*)xn + Rl * D * 2, xn, Rl * D * 2, cudaMemcpyDeviceToDevice, st));
-    }
     if (L.has_cross && c.ctx_kv) {  // x = cross_attn(x, context) + x   (attention.py:327-328)
       const phk_attn_t& A = L.cross_attn;
       PHK_REQUIRE(c.seq.n_inner == 1, PHK_E_UNSUPPORTED, "cross attention needs (b, n) sequences");
-      if (!norm_done) PHK_TRY(phk_layernorm(x, A.norm_g, A.norm_b, xn, nullptr, R, D, h16, 0, 0, 0, s));
-      norm_done = false;
+      PHK_TRY(phk_layernorm(x, A.norm_g, A.norm_b, xn, nullptr, R, D, h16, 0, 0, 0, s));
 #ifndef PHK_CUDA_EMU
       if (cross_pack) {
         PHK_TRY(phk_gemm_bf16_qnorm(xn, D, A.wq_h, D, q, R, I, D, A.q_scale, 8.f, s));  // bf16 [R, I] in the fp32-sized q buffer
@@ -330,30 +276,17 @@ static int transformer_forward(const TfCall& c, Arena scratch, float* out, void*
       const float* kvl = c.ctx_kv + (int64_t)l * c.ctx_b * c.ctx_L * 2 * I;
       PHK_TRY(phk_attention(q, kvl, A.null_kv, A.q_scale, A.k_scale, nullptr, c.ctx_mask, nullptr, o, &g, s));
       }
-      if (fuse_ln && A.wo_h) {
-        PHK_TRY(gemm_ln(o, I, A.wo_h, I, x, R, I, L.ff.ln_g, L.ff.ln_b, xn, nullptr));
-        norm_done = true;
-      } else {
-        PHK_TRY(linear(c.lin, o, I, A.wo, A.wo_h, I, x, D, R, D, I, nullptr, x, s));
-      }
+      PHK_TRY(linear(c.lin, o, I, A.wo, A.wo_h, I, x, D, R, D, I, nullptr, x, s));
     }
     {  // x = ff(x) + x  (attention.py:45-53, 330)
       const phk_ff_t& Fw = L.ff;
-      if (!norm_done) PHK_TRY(phk_layernorm(x, Fw.ln_g, Fw.ln_b, xn, nullptr, R, D, h16, 0, 0, 0, s));
-      norm_done = false;
+      PHK_TRY(phk_layernorm(x, Fw.ln_g, Fw.ln_b, xn, nullptr, R, D, h16, 0, 0, 0, s));
       if (h16) {
         PHK_REQUIRE(Fw.w1_h && Fw.w2_h && Fw.inner_pad % 64 == 0 && Fw.inner_pad >= Fw.inner, PHK_E_ARG,
                     "bf16 mode needs the packed feed-forward weights");
         // first linear + GEGLU in one kernel (value/gate rows interleaved per 64), bf16 [R, inner_pad] out
         PHK_TRY(phk_gemm_bf16(xn, D, Fw.w1_h, D, gbuf, Fw.inner_pad, R, 2 * Fw.inner_pad, D, nullptr, nullptr, 0, 0, 0, 2, s));
-        const bool next_plain = l + 1 < T->depth && !T->layers[l + 1].has_peg;
-        if (fuse_ln && next_plain) {  // ... + the next layer's attention LayerNorm and its raw bf16 rows
-          const phk_attn_t& NA = T->layers[l + 1].self_attn;
-          PHK_TRY(gemm_ln(gbuf, Fw.inner_pad, Fw.w2_h, Fw.inner_pad, x, R, Fw.inner_pad, NA.norm_g, NA.norm_b, xn, xraw));
-          ln_ready = true;
-        } else {
-          PHK_TRY(phk_gemm_bf16(gbuf, Fw.inner_pad, Fw.w2_h, Fw.inner_pad, x, D, R, D, Fw.inner_pad, nullptr, x, 0, 0, 0, 0, s));
-        }
+        PHK_TRY(phk_gemm_bf16(gbuf, Fw.inner_pad, Fw.w2_h, Fw.inner_pad, x, D, R, D, Fw.inner_pad, nullptr, x, 0, 0, 0, 0, s));
       } else {
         PHK_TRY(linear(c.lin, xn, D, Fw.w1, Fw.w1_h, D, hbuf, 2 * Fw.inner, R, 2 * Fw.inner, D, nullptr, nullptr, s));
         PHK_TRY(phk_geglu(hbuf, (float*)gbuf, R, Fw.inner, s));
@@ -392,7 +325,7 @@ static int check_transformer(const phk_transformer_t* T) {
 
 using namespace phk;
 
-extern "C" int phk_version(void) { return 102; }
+extern "C" int phk_version(void) { return 103; }
 extern "C" const char* phk_last_error(void) { return g_err; }
 extern "C" int64_t phk_launch_count(void) { return g_launches.load(); }
 
@@ -563,8 +496,8 @@ static int cvivit_encode_impl(const phk_cvivit_t* m, const float* video, int32_t
 // as long as the GPU work (0.85 ms in bf16 mode).  The launch sequence is a pure function of (weight table contents,
 // buffers, shape, precision), so the second call with the same key captures it on a library-owned stream and later
 // calls replay the instantiated graph on the caller's stream (one cudaGraphLaunch).  The first call always runs
-// eagerly (one-time cudaFuncSetAttribute / tensor-map creation happen outside capture).  Disabled by PHK_GRAPH=0,
-// while the per-family profiler is on, and when a parity test taps intermediates.
+// eagerly (one-time cudaFuncSetAttribute / tensor-map creation happen outside capture).  Disabled while the per-family
+// profiler is on, when a parity test taps intermediates, and for good after a failed capture.
 struct EncodeGraphKey {
   uint64_t table_hash;
   const void *video, *ids, *ws, *bias;
@@ -598,18 +531,12 @@ static uint64_t hash_transformer(const phk_transformer_t& T, uint64_t h) {
   return h;
 }
 
-static int graphs_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = std::getenv("PHK_GRAPH"); on = (e && e[0] == '0') ? 0 : 1; }
-  return on;
-}
-
 extern "C" int phk_cvivit_encode(const phk_cvivit_t* m, const float* video, int32_t B, int32_t F, int64_t* ids,
                                  void* workspace, int64_t workspace_bytes, int32_t prec, const float* spatial_bias,
                                  float* tap_patch, float* tap_spatial, float* tap_temporal, float* tap_proj,
                                  phk_stream_t s) {
   const bool taps = tap_patch || tap_spatial || tap_temporal || tap_proj;
-  if (!m || taps || !spatial_bias || !graphs_enabled() || g_prof_on.load(std::memory_order_relaxed))
+  if (!m || taps || !spatial_bias || g_prof_on.load(std::memory_order_relaxed))
     return cvivit_encode_impl(m, video, B, F, ids, workspace, workspace_bytes, prec, spatial_bias, tap_patch, tap_spatial,
                               tap_temporal, tap_proj, s);
   static std::unordered_map<EncodeGraphKey, EncodeGraphEntry, EncodeGraphKeyHash> cache;
@@ -1016,8 +943,7 @@ static int sample_step_impl(const phk_maskgit_t* m, const int64_t* ids_in, int32
   float* x = (float*)ar.take(R * D * 4);
   float* x_alt = (float*)ar.take(R * D * 4);
   // masked rows only (phk_sample_tail) when the caller vouches for the per-sequence count and it saves work
-  static const bool compact_ok = [] { const char* e = std::getenv("PHK_HEAD_COMPACT"); return !(e && e[0] == '0'); }();
-  const bool compact = (compact_ok || prime_len > 0) && mask && ids && masked_per_seq > 0 && masked_per_seq < n;
+  const bool compact = mask && ids && masked_per_seq > 0 && masked_per_seq < n;
   const int64_t hb = compact ? phk_sample_tail_scratch_bytes(b, masked_per_seq, D) : phk_head_sample_scratch_bytes((int32_t)tokens);
   void* emb_h = compact ? nullptr : ar.take(tokens * D * 2);
   void* hsc = ar.take(hb);
@@ -1075,16 +1001,9 @@ static uint64_t noise_stride(int32_t b, int32_t n, int32_t V) {
   return ((uint64_t)b * (uint64_t)n * (uint64_t)((V + 3) / 4) + 1 + 3) / 4 * 4;
 }
 
-static std::atomic<int> g_step_graph{-1};  // -1: PHK_STEP_GRAPH from the environment; 0 / 1: phk_debug_step_graph
-static int step_graphs_enabled() {
-  const int v = g_step_graph.load(std::memory_order_relaxed);
-  if (v >= 0) return v;
-  static int env = -1;
-  if (env < 0) { const char* e = std::getenv("PHK_STEP_GRAPH"); env = (e && e[0] == '0') ? 0 : 1; }  // default: on
-  return env;
-}
-// tests / A-B runs: 1 replays phk_maskgit_demask_iteration as a CUDA graph, 0 keeps it eager, < 0 back to PHK_STEP_GRAPH
-extern "C" int phk_debug_step_graph(int32_t on) { g_step_graph.store(on < 0 ? -1 : (on ? 1 : 0)); return 0; }
+static std::atomic<bool> g_step_graph{true};
+// tests: 1 replays phk_maskgit_demask_iteration as a CUDA graph, 0 keeps it eager, < 0 back to the default (on)
+extern "C" int phk_debug_step_graph(int32_t on) { g_step_graph.store(on != 0); return 0; }
 
 // Launch-sequence cache of phk_maskgit_demask_iteration: `key` identifies the call (table contents, every pointer and
 // scalar), `run(stream)` issues the launches.  First sighting of a key: eager; second: captured; later: one cudaGraphLaunch.
@@ -1213,7 +1132,7 @@ extern "C" int phk_maskgit_demask_iteration(const phk_maskgit_t* m, const phk_ma
                                  ctx_kv, critic_ctx_kv, L, text_mask, pos_bias, cond_scale, temperature, rng_state,
                                  k_remask, critic_noise, noise_K, noise_mult, skip_critic, workspace, workspace_bytes, st);
   };
-  if (!step_graphs_enabled() || !pos_bias || g_prof_on.load(std::memory_order_relaxed)) return run(s);
+  if (!g_step_graph.load(std::memory_order_relaxed) || !pos_bias || g_prof_on.load(std::memory_order_relaxed)) return run(s);
   int dev = 0;
   PHK_CUDA(cudaGetDevice(&dev));
   // key: table contents + every pointer and scalar of the call (a 64-bit FNV of them; the values behind the pointers

@@ -9,7 +9,6 @@
 // Sequences are addressed with (outer, inner, token) strides so neither the spatial
 // '(b t)(h w)' nor the temporal '(b h w) t' view is ever materialised (cvivit.py:458,468).
 #include "phk_common.cuh"
-#include <cstdlib>
 
 namespace phk {
 
@@ -1431,8 +1430,7 @@ extern "C" int phk_attention(const float* q, const float* kv, const float* null_
   }
 #ifndef PHK_CUDA_EMU
   {  // bf16-mode cross-attention over <= 32 key slots on warp-level MMAs
-    static const bool cross_mma = [] { const char* e = std::getenv("PHK_CROSS_ATTN_MMA"); return !(e && e[0] == '0'); }();
-    if (cross_mma && !g->causal && !bias && g->out_bf16 && g->dim_head == 64 && g->num_null_kv > 0 &&
+    if (!g->causal && !bias && g->out_bf16 && g->dim_head == 64 && g->num_null_kv > 0 &&
         g->n_k + g->num_null_kv <= XK && g->q_tok % 2 == 0 && g->q_outer % 2 == 0 && g->q_inner % 2 == 0 && g->k_tok % 2 == 0 &&
         g->k_outer % 2 == 0 && g->k_inner % 2 == 0 && g->o_tok % 2 == 0 && g->o_outer % 2 == 0 && g->o_inner % 2 == 0 &&
         ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(kv) | reinterpret_cast<uintptr_t>(null_kv) |
@@ -1481,8 +1479,7 @@ extern "C" int phk_attention_small_bf16(const void* Qn, const void* KVn, const f
   const int n = g->n_q;
 #ifndef PHK_CUDA_EMU
   // warp-level tensor-core kernel: needs 16-byte aligned rows (token strides multiples of 8 elements)
-  static const bool use_mma = [] { const char* e = std::getenv("PHK_SMALL_ATTN_MMA"); return !(e && e[0] == '0'); }();
-  if (use_mma && g->out_bf16 && g->q_tok % 8 == 0 && g->q_outer % 8 == 0 && g->q_inner % 8 == 0 && g->k_tok % 8 == 0 &&
+  if (g->out_bf16 && g->q_tok % 8 == 0 && g->q_outer % 8 == 0 && g->q_inner % 8 == 0 && g->k_tok % 8 == 0 &&
       g->k_outer % 8 == 0 && g->k_inner % 8 == 0 && (g->heads * 64) % 8 == 0 &&
       ((reinterpret_cast<uintptr_t>(Qn) | reinterpret_cast<uintptr_t>(KVn)) & 15) == 0) {
     const int64_t npairs = (int64_t)g->n_outer * g->n_inner * g->heads;

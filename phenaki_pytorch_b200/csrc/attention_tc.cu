@@ -267,13 +267,6 @@ extern "C" int phk_attention_tc_bf16(const void* Qn, int64_t ld_q, const void* K
   return 0;
 }
 
-// tests: selected the probability path of an earlier tensor-memory design; accepted for ABI compatibility, the one
-// kernel above serves every value
-extern "C" int phk_debug_attention_tc_variant(int32_t variant) {
-  PHK_REQUIRE(variant <= 1, PHK_E_ARG, "phk_debug_attention_tc_variant: 0, 1 or < 0");
-  return 0;
-}
-
 // Self-attention core on tensor cores from fp32 projections: q fp32 [n_seq*n, heads*64], kv fp32 [n_seq*n, 2*heads*64]
 // (token-major), bias fp32 [heads, n, n] or NULL -> out bf16 [n_seq*n, heads*64].  dim_head 64, no null-kv, no key
 // mask, not causal (everything else takes phk_attention).  scratch >= phk_attention_tc_scratch_bytes.

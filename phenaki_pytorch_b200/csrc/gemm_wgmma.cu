@@ -2,7 +2,7 @@
 //   C[map(m), n] = sum_k A[m,k] * W[n,k]  (+bias) (+residual)        nn.Linear semantics
 // A, W bf16, K-major (row-major [rows, K]); fp32 accumulation in registers.
 //
-// gemm_bf16_kernel<EPI, DUAL> behind phk_gemm_bf16 / phk_gemm_bf16_x2 / _ln / _qkv / _qnorm: one CTA per 128 x 128 tile,
+// gemm_bf16_kernel<EPI, DUAL> behind phk_gemm_bf16 / phk_gemm_bf16_x2 / _qkv / _qnorm: one CTA per 128 x 128 tile,
 // DUAL = two independent problems in one persistent launch.  Persistent (one CTA per SM, static round-robin tile
 // scheduler, m-fastest so concurrent CTAs share the W tile in L2 while the A panel stays L2-resident):
 //   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor.2d (SWIZZLE_128B) stages 128x64 A and W tiles into
@@ -19,7 +19,6 @@
 //              bf16 [M, N/2]: fitted sigmoid-form GELU, swizzled bf16 staging tile, coalesced 16-byte stores.
 #include "phk_common.cuh"
 #include "phk_sm90.cuh"
-#include <cstdlib>
 #include <mutex>
 #include <unordered_map>
 
@@ -37,17 +36,12 @@ constexpr int CPAD = 132;                          // fp32 staging row stride (f
 constexpr int CSTAGE_BYTES = GM * CPAD * 4;        // 67.6 KB
 constexpr int RING_BYTES = GSTAGES * 2 * STAGE_BYTES;
 constexpr int SMEM_TOTAL = RING_BYTES + CSTAGE_BYTES + 256 /*barriers*/ + 1024 /*manual 1024-B alignment*/;
-// epilogue 4: per-part row sums [4][128] float2 + the cluster exchange [2 buffers][8 ranks][128 rows] float2
-constexpr int LN_MAX_CLUSTER = 8;
-constexpr int LN_ROWSTAT_BYTES = EPI_PARTS * GM * 8, LN_XSTAT_BYTES = 2 * LN_MAX_CLUSTER * GM * 8;
-constexpr int SMEM_TOTAL_LN = SMEM_TOTAL + LN_ROWSTAT_BYTES + LN_XSTAT_BYTES;
 
 struct EpiParams {
   void* C; int64_t ldc; int64_t M; int N; int K;
   const float* bias; const float* residual;
   int64_t seg_len, seg_stride, seg_off;
   int m_tiles, n_tiles;
-  long long* trace;  // debug: per-CTA clock64 stamps of the first tile (NULL in production)
   // fp32 epilogue through the TMA unit (identity row map, C 16-B aligned, residual == C or none): C as a tensor map
   // with [128 rows x 32 floats] SWIZZLE_128B boxes; the residual tile is bulk-LOADED into the staging boxes while the
   // main loop runs and the finished tile is bulk-STORED from them, so the epilogue warps issue no global accesses
@@ -56,19 +50,6 @@ struct EpiParams {
   // per 64-column head (F.normalize, eps 1e-12), multiplied by nscale[col % 64] (q_scale / k_scale) and by nmul (the
   // fixed similarity scale 8 folded into q); columns >= norm_cols (the value half of to_kv) are only converted
   const float* nscale; int norm_cols; float nmul;
-  // epilogue 4 (residual + the NEXT LayerNorm, attention.py:311-332): C = A W^T + C in place (fp32, bulk-stored) and, from
-  // the same registers, LayerNorm(C) * ln_g + ln_b -> bf16 ln_out [M, ln_ld] (+ optionally the un-normalised row as bf16
-  // in raw_out: the k,v projection input of attention.py:140-144).  One CTA holds 128 of the N columns of a row, so the
-  // row statistics are summed over the cluster of n_tiles CTAs that share the m-tile (distributed shared memory).
-  const float* ln_g; const float* ln_b; void* ln_out; void* raw_out; int64_t ln_ld; float ln_eps;
-  // epilogue 5: the same result without a cluster -- the n_tiles CTAs of a group (consecutive block indices, all resident:
-  // the grid is at most one CTA per SM) exchange their 128-column row statistics through global memory: xstat_g
-  // [2][gridDim][128] float2 slots (double-buffered by tile parity) and one arrival counter per group (ln_counter[group],
-  // zero when the kernel starts; release / acquire at gpu scope).
-  float2* xstat_g; unsigned int* ln_counter;
-  // the W operand is not written by the kernels that precede this one in the stream (inference weights): its first tiles
-  // are requested BEFORE griddepcontrol.wait, while the previous kernel drains
-  int w_static;
   alignas(64) CUtensorMap tmC;
 };
 
@@ -99,32 +80,19 @@ __device__ __forceinline__ void acc_to_stage(const float (&d)[32], uint8_t* stag
 }
 
 // gelu_erf(g) * v for the bf16 GEGLU epilogue (attention.py:40-43).  Phi(g) = 0.5 (1 + erf(g / sqrt2)) is evaluated
-// as sigmoid(2 g (a + b g^2 + c g^4)) = 1 / (1 + 2^(g (a' + b' g^2 + c' g^4))) with (a, b, c) fitted to the erf form
-// (max |error| of the GELU 2.5e-5 over all g -- two orders below the bf16 rounding of the result -- and, unlike
-// 0.5 (1 + tanh), no cancellation for negative g).  10 issue slots per output (two of them MUFU) instead of ~19 for
-// the erf polynomial: the epilogue was issue-bound (tools/gemm_trace.py).  g^2 is clamped to 64: beyond |g| = 8 the
-// fitted quintic would turn over, while the sigmoid is already saturated.
+// as sigmoid(2 g (a + b g^2 + c g^4)) with (a, b, c) fitted to the erf form (unlike 0.5 (1 + erf) from a polynomial, no
+// cancellation for negative g), and sigmoid(z) = 0.5 + 0.5 tanh(z / 2) on ONE MUFU op (tanh.approx.f32, relative error
+// 2^-11): a few issue slots per output instead of ~19 for the erf polynomial, because the epilogue is issue-bound.  Phi
+// is good to 2.4e-4 absolute -- below the bf16 rounding of the hidden activations.  g^2 is clamped to 64: beyond |g| = 8
+// the fitted quintic would turn over, while the sigmoid is already saturated.
 __device__ __forceinline__ float geglu_fast(float g, float v) {
   const float g2 = fminf(g * g, 64.0f);
-#ifndef PHK_GEGLU_EX2_RCP
-  // sigmoid(z) = 0.5 + 0.5 tanh(z / 2) on ONE MUFU op (tanh.approx.f32, relative error 2^-11) instead of ex2 + rcp: the same
-  // fitted quintic with its coefficients times -ln2 / 2, half the MUFU work of the epilogue's math phase.  Phi is good to
-  // 2.4e-4 absolute -- below the bf16 rounding of the hidden activations.  -DPHK_GEGLU_EX2_RCP restores the two-op form
-  // (2.5e-5, and relative accuracy in the negative tail).
   float u = fmaf(g2, -0.00035151678851506f, 0.037005646021930225f);
   u = fmaf(u, g2, 0.7975078842858219f);
   float t;
   asm("tanh.approx.f32 %0, %1;" : "=f"(t) : "f"(g * u));
   const float h = 0.5f * (g * v);
   return fmaf(h, t, h);
-#else
-  float u = fmaf(g2, 0.0010142630551597833f, -0.10677572400146226f);   // -2 log2(e) * {c, b, a}
-  u = fmaf(u, g2, -2.301121339458009f);
-  float e, r;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(e) : "f"(g * u));
-  asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(1.0f + e));
-  return (g * v) * r;
-#endif
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -167,9 +135,9 @@ __device__ __forceinline__ bool epi_residual_prefetch(const EpiParams& p, float*
 // staged as CPAD rows.  All accumulator columns this thread needs (16 value + 16 gate of ONE row) are read first; after
 // a barrier the staging memory takes the bf16 results (128 B per row), which leave as fully coalesced 16-B-per-lane
 // rows: one row per thread straight from registers made every warp store touch 32 different lines.
-template <int NCH, typename Stamp>
+template <int NCH>
 __device__ __forceinline__ void epi_geglu_tile(const EpiParams& p, void* stage, int64_t m0, int n0, int ew, int lg,
-                                               int part, int lane, Stamp&& stamp) {
+                                               int part, int lane) {
   static_assert(NCH == 1, "one 128-column chunk per tile");
   constexpr int W = 64 / EPI_PARTS;
   static_assert(W == 16, "two 16-B units per thread and chunk");
@@ -185,7 +153,6 @@ __device__ __forceinline__ void epi_geglu_tile(const EpiParams& p, void* stage, 
       gate[0][j] = b.x; gate[0][j + 1] = b.y; gate[0][j + 2] = b.z; gate[0][j + 3] = b.w;
     }
   }
-  stamp(10);  // accumulator columns in registers
   epi_bar_sync();  // every thread has read its columns: the staging memory takes the bf16 results
   const uint32_t seg_len = (uint32_t)p.seg_len;
   const bool coalesced = (p.ldc % 8 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
@@ -217,9 +184,7 @@ __device__ __forceinline__ void epi_geglu_tile(const EpiParams& p, void* stage, 
     }
   }
   if (!coalesced) return;  // uniform over the CTA
-  stamp(11);               // this thread's outputs computed and staged
   epi_bar_sync();          // tile staged
-  stamp(7);
   constexpr int RPI = 32 / U;                 // rows per warp instruction (4 or 2)
   const int rl = lane / U, u = lane % U;      // this lane's row within the instruction and its 16-B unit
   const bool chunk_ok = (n0 + (u >> 3) * 128) < p.N;
@@ -426,158 +391,6 @@ __device__ __forceinline__ void epi_chunk(const EpiParams& p, float* cstage, int
   epi_bar_sync();  // staging buffer free for the next chunk
 }
 
-__device__ __forceinline__ uint32_t cluster_rank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ uint32_t map_to_cta(uint32_t saddr, uint32_t rank) {  // shared::cta -> shared::cluster
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(saddr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity) {  // acquire at cluster scope
-  long long t0 = 0;
-  for (uint32_t spin = 0;; ++spin) {
-    uint32_t done;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-    if (done) return;
-    if ((spin & 1023u) == 1023u) {
-      if (t0 == 0) t0 = clock64();
-      else if (clock64() - t0 > 4000000000LL) __trap();
-    }
-  }
-}
-__device__ __forceinline__ uint32_t cluster_size() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void st_cluster_f2(uint32_t cluster_addr, float a, float b) {  // distributed shared memory store
-  asm volatile("st.shared::cluster.v2.f32 [%0], {%1, %2};" ::"r"(cluster_addr), "f"(a), "f"(b) : "memory");
-}
-
-// Epilogue 4, after the accumulator-ready wait: x = acc + x (bulk-stored like epi_tma_finish) and LayerNorm(x) of the
-// same registers -> bf16.  Row statistics: every thread sums its 32 columns, the four column parts meet in `rowstat`,
-// the n_tiles CTAs of the cluster (same m-tile, adjacent 128-column slices) exchange their 128-column partials through
-// distributed shared memory: thread (row r, part 0) of CTA c stores its partial into xstat[buf][c][r] of EVERY CTA of the
-// cluster and arrives on that CTA's `bar_stat` (128 * cluster_size arrivals per tile, release / acquire at cluster scope).
-// Two exchange buffers: a CTA can be at most one tile ahead of a peer (it needs the peer's arrival to get further).
-template <bool GLOBAL>
-__device__ __forceinline__ void epi_tma_finish_ln(const EpiParams& p, uint8_t* stage, uint32_t stage_s, int m0, int n0,
-                                                  int ew, int lg, int part, int lane, float2* rowstat, const float2* xstat,
-                                                  uint32_t xstat_s, uint32_t bar_stat,
-                                                  uint32_t& stat_phase, uint32_t& stat_buf, uint32_t my_rank, uint32_t csize,
-                                                  int iter, int group) {
-  const int r = lg * 32 + lane;
-  float4* box_row = reinterpret_cast<float4*>(stage + part * (GM * 128) + r * 128);
-  const int col0 = n0 + part * 32;
-  float4 o[8];
-  float s1 = 0.f, s2 = 0.f;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const int pos = j ^ (r & 7);
-    o[j] = box_row[pos];  // accumulator + residual (acc_to_stage<true>)
-    if (p.bias) {
-      const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + col0) + j);
-      o[j].x += bv.x; o[j].y += bv.y; o[j].z += bv.z; o[j].w += bv.w;
-    }
-    box_row[pos] = o[j];
-    s1 += (o[j].x + o[j].y) + (o[j].z + o[j].w);
-    s2 += (o[j].x * o[j].x + o[j].y * o[j].y) + (o[j].z * o[j].z + o[j].w * o[j].w);
-  }
-  rowstat[part * GM + r] = make_float2(s1, s2);
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA unit
-  epi_bar_sync();  // whole chunk staged, the four parts of every row are in rowstat
-  if (ew == 0 && lane == 0) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c)
-      if (n0 + 32 * c < p.N) tma_store_2d(&p.tmC, stage_s + c * (GM * 128), n0 + 32 * c, m0);
-    tma_store_commit();
-  }
-  float t1 = 0.f, t2 = 0.f;
-  if (GLOBAL) {
-    // global-memory exchange: slot [buf][block][row]; one arrival per CTA and tile on the group's counter
-    float2* mine = p.xstat_g + ((size_t)stat_buf * gridDim.x + blockIdx.x) * GM;
-    if (part == 0) {
-      float a1 = 0.f, a2 = 0.f;
-#pragma unroll
-      for (int q = 0; q < EPI_PARTS; ++q) { const float2 e = rowstat[q * GM + r]; a1 += e.x; a2 += e.y; }
-      __stcg(mine + r, make_float2(a1, a2));
-      __threadfence();
-    }
-    epi_bar_sync();  // the 128 partials of this CTA are written and fenced
-    if (ew == 0 && lane == 0) {
-      unsigned int* ctr = p.ln_counter + group;
-      const unsigned int target = (unsigned int)(iter + 1) * csize;
-      asm volatile("red.release.gpu.global.add.u32 [%0], 1;" ::"l"(ctr) : "memory");
-      long long t0 = 0;
-      for (uint32_t spin = 0;; ++spin) {
-        unsigned int seen;
-        asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(seen) : "l"(ctr) : "memory");
-        if (seen >= target) break;
-        if ((spin & 255u) == 255u) {
-          if (t0 == 0) t0 = clock64();
-          else if (clock64() - t0 > 4000000000LL) __trap();  // a peer CTA never arrived
-        }
-      }
-    }
-    epi_bar_sync();  // every peer's partials are visible
-    const float2* grp = p.xstat_g + ((size_t)stat_buf * gridDim.x + (size_t)group * csize) * GM;
-    for (uint32_t c = 0; c < csize; ++c) { const float2 e = __ldcg(grp + (size_t)c * GM + r); t1 += e.x; t2 += e.y; }
-    stat_buf ^= 1;
-  } else {
-    if (part == 0) {  // 128 threads, one per row: this CTA's 128-column partial to every CTA of the cluster
-      float a1 = 0.f, a2 = 0.f;
-#pragma unroll
-      for (int q = 0; q < EPI_PARTS; ++q) { const float2 e = rowstat[q * GM + r]; a1 += e.x; a2 += e.y; }
-      const uint32_t slot = xstat_s + ((stat_buf * LN_MAX_CLUSTER + my_rank) * GM + r) * 8;
-      for (uint32_t dst = 0; dst < csize; ++dst) {
-        st_cluster_f2(map_to_cta(slot, dst), a1, a2);
-        mbar_arrive_remote(map_to_cta(bar_stat, dst));
-      }
-    }
-    mbar_wait_cluster(bar_stat, stat_phase);
-    stat_phase ^= 1;
-    for (uint32_t c = 0; c < csize; ++c) { const float2 e = xstat[(stat_buf * LN_MAX_CLUSTER + c) * GM + r]; t1 += e.x; t2 += e.y; }
-    stat_buf ^= 1;
-  }
-  const float inv_n = 1.0f / (float)p.N;
-  const float mean = t1 * inv_n;
-  const float rstd = rsqrtf(fmaxf(t2 * inv_n - mean * mean, 0.f) + p.ln_eps);
-  if ((uint32_t)(m0 + r) < (uint32_t)p.M) {
-    __nv_bfloat16* lrow = reinterpret_cast<__nv_bfloat16*>(p.ln_out) + (int64_t)(m0 + r) * p.ln_ld + col0;
-    __nv_bfloat16* rrow = p.raw_out ? reinterpret_cast<__nv_bfloat16*>(p.raw_out) + (int64_t)(m0 + r) * p.ln_ld + col0 : nullptr;
-#pragma unroll
-    for (int j = 0; j < 8; j += 2) {
-      const float4 g0 = __ldg(reinterpret_cast<const float4*>(p.ln_g + col0) + j), g1 = __ldg(reinterpret_cast<const float4*>(p.ln_g + col0) + j + 1);
-      float4 b0 = make_float4(0.f, 0.f, 0.f, 0.f), b1 = b0;
-      if (p.ln_b) { b0 = __ldg(reinterpret_cast<const float4*>(p.ln_b + col0) + j); b1 = __ldg(reinterpret_cast<const float4*>(p.ln_b + col0) + j + 1); }
-      const float4 a = o[j], c = o[j + 1];
-      *reinterpret_cast<uint4*>(lrow + 4 * j) = make_uint4(
-          pack_bf16x2(fmaf((a.x - mean) * rstd, g0.x, b0.x), fmaf((a.y - mean) * rstd, g0.y, b0.y)),
-          pack_bf16x2(fmaf((a.z - mean) * rstd, g0.z, b0.z), fmaf((a.w - mean) * rstd, g0.w, b0.w)),
-          pack_bf16x2(fmaf((c.x - mean) * rstd, g1.x, b1.x), fmaf((c.y - mean) * rstd, g1.y, b1.y)),
-          pack_bf16x2(fmaf((c.z - mean) * rstd, g1.z, b1.z), fmaf((c.w - mean) * rstd, g1.w, b1.w)));
-      if (rrow)
-        *reinterpret_cast<uint4*>(rrow + 4 * j) = make_uint4(pack_bf16x2(a.x, a.y), pack_bf16x2(a.z, a.w),
-                                                             pack_bf16x2(c.x, c.y), pack_bf16x2(c.z, c.w));
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------
 // The kernel: 128 x 128 tiles, four MMA / epilogue warpgroups of one 64 x 64 quadrant each
 // ---------------------------------------------------------------------------------------------------
@@ -599,21 +412,14 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
   const uint32_t sA = base, sB = base + GSTAGES * STAGE_BYTES;
   float* cstage = reinterpret_cast<float*>(base_ptr + RING_BYTES);
   const uint32_t bars = base + RING_BYTES + CSTAGE_BYTES;
-  // full[s] @ +8s ; empty[s] @ +8(S+s) ; residual landed @ +16S ; cluster statistics landed @ +16S+8
-  const uint32_t bar_res = bars + 16 * GSTAGES, bar_stat = bar_res + 8;
+  // full[s] @ +8s ; empty[s] @ +8(S+s) ; residual landed @ +16S
+  const uint32_t bar_res = bars + 16 * GSTAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles1 = p.m_tiles * p.n_tiles;
   const int num_tiles = tiles1 + (DUAL ? p2.m_tiles * p2.n_tiles : 0);
-  // epilogue 4: clusters of n_tiles CTAs own one m-tile at a time (CTA rank = n-tile), round-robin over the m-tiles
-  constexpr bool LN_EPI = EPI == 4 || EPI == 5;
-  const uint32_t csize = EPI == 4 ? cluster_size() : EPI == 5 ? (uint32_t)p.n_tiles : 1u;
-  const uint32_t crank = EPI == 4 ? cluster_rank() : EPI == 5 ? blockIdx.x % csize : 0u;
-  const int cluster_id = (int)blockIdx.x / (int)csize, n_clusters = (int)gridDim.x / (int)csize;
   // tile schedule: round-robin over all tiles (problem 1 first), m-fastest; returns true for a tile of problem 2
-  const int my_tiles = LN_EPI ? (cluster_id < p.m_tiles ? (p.m_tiles - 1 - cluster_id) / n_clusters + 1 : 0)
-                                : ((int)blockIdx.x < num_tiles ? (num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0);
+  const int my_tiles = (int)blockIdx.x < num_tiles ? (num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
   auto tile_of = [&](int i, int& m0, int& n0) -> bool {
-    if (LN_EPI) { m0 = (cluster_id + i * n_clusters) * GM; n0 = (int)crank * GN; return false; }
     int tile = (int)blockIdx.x + i * (int)gridDim.x;
     const bool second = DUAL && tile >= tiles1;
     if (second) tile -= tiles1;
@@ -623,8 +429,6 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
     return second;
   };
   auto kblocks = [&](bool second) { return ((second ? p2.K : p.K) + GK - 1) / GK; };
-  const long long t_start = clock64();
-#define PHK_STAMP(slot) do { if (p.trace) p.trace[blockIdx.x * 16 + (slot)] = clock64() - t_start; } while (0)
 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
@@ -638,24 +442,10 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
       mbar_init(bars + 8 * (GSTAGES + s), EPI_WARPS);  // one arrival per MMA warp
     }
     mbar_init(bar_res, 1);                               // residual tile landed (TMA epilogue)
-    if (EPI == 4) mbar_init(bar_stat, GM * csize);       // row statistics of the whole cluster landed (epilogue 4)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  if (EPI == 4) { __syncwarp(); cluster_sync_all(); }  // every CTA of the cluster runs and has its barriers initialised
-  int pre_kb = 0;  // k-blocks of the first tile whose W half is already in flight (producer thread only)
-  if (threadIdx.x == 0 && my_tiles > 0 && p.w_static) {
-    int m0, n0;
-    const bool second = tile_of(0, m0, n0);
-    const int num_kb = kblocks(second);
-    pre_kb = num_kb < GSTAGES ? num_kb : GSTAGES;
-    for (int kb = 0; kb < pre_kb; ++kb) {
-      mbar_expect_tx(bars + 8 * kb, 2 * STAGE_BYTES);  // both halves; the A half is requested after the wait
-      tma_load_2d(second ? &tmB2 : &tmB, bars + 8 * kb, sB + kb * STAGE_BYTES, kb * GK, n0);
-    }
-  }
-  pdl_wait();  // everything above (barriers, tensor-map prefetch, W prefetch) overlapped the previous kernel
-  if (threadIdx.x == 0) PHK_STAMP(0);  // setup done
+  pdl_wait();  // everything above (barriers, tensor-map prefetch) overlapped the previous kernel
 
   if (warp < 4) {
     // ===================== TMA producer =====================
@@ -671,15 +461,9 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(bars + 8 * (GSTAGES + stage), phase ^ 1);  // slot free (passes immediately on the first lap)
           const uint32_t full = bars + 8 * stage;
-          if (it == 0 && kb < pre_kb) {  // W half requested before the wait (stage == kb on the first lap)
-            tma_load_2d(ma, full, sA + stage * STAGE_BYTES, kb * GK, m0);
-          } else {
-            mbar_expect_tx(full, 2 * STAGE_BYTES);
-            tma_load_2d(ma, full, sA + stage * STAGE_BYTES, kb * GK, m0);
-            tma_load_2d(mb, full, sB + stage * STAGE_BYTES, kb * GK, n0);
-          }
-          if (it == 0 && kb == 0) PHK_STAMP(1);            // first TMA issued
-          if (it == 0 && kb == num_kb - 1) PHK_STAMP(2);   // last TMA of the first tile issued
+          mbar_expect_tx(full, 2 * STAGE_BYTES);
+          tma_load_2d(ma, full, sA + stage * STAGE_BYTES, kb * GK, m0);
+          tma_load_2d(mb, full, sB + stage * STAGE_BYTES, kb * GK, n0);
           if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
         }
       }
@@ -691,17 +475,14 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
     const int part = ew >> 2;       // which quarter of the tile's columns this warp drains
     const int wg = ew >> 2;         // MMA warpgroup: quadrant rows 64 (wg & 1).., columns 64 (wg >> 1)..
     const int rq = (wg & 1) * 64, cq = (wg >> 1) * 64;
-    uint32_t res_phase = 0, stat_phase = 0, stat_buf = 0;
-    float2* rowstat = reinterpret_cast<float2*>(base_ptr + RING_BYTES + CSTAGE_BYTES + 256);
-    const float2* xstat = rowstat + EPI_PARTS * GM;
-    const uint32_t xstat_s = base + RING_BYTES + CSTAGE_BYTES + 256 + LN_ROWSTAT_BYTES;
+    uint32_t res_phase = 0;
     int stage = 0;
     uint32_t phase = 0;
     for (int it = 0; it < my_tiles; ++it) {
       int m0, n0;
       const bool second = tile_of(it, m0, n0);
       const EpiParams& pp = second ? p2 : p;
-      const bool tma = (EPI == 0 && pp.tma_epi) || LN_EPI;
+      const bool tma = EPI == 0 && pp.tma_epi;
       bool res_vec = false;
       if (tma) epi_tma_begin(pp, base + RING_BYTES, bar_res, m0, n0, ew, lane);
       else if (EPI == 0) res_vec = epi_residual_prefetch<EPI>(pp, cstage, m0, n0, ew, lane);
@@ -713,8 +494,6 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
       const int num_kb = kblocks(second);
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(bars + 8 * stage, phase);
-        if (it == 0 && kb == 0 && threadIdx.x == 128) PHK_STAMP(3);            // first operands landed
-        if (it == 0 && kb == num_kb - 1 && threadIdx.x == 128) PHK_STAMP(4);   // last operands landed
         const uint64_t da = gmma_desc(sA + stage * STAGE_BYTES + rq * 128);
         const uint64_t db = gmma_desc(sB + stage * STAGE_BYTES + cq * 128);
         wgmma_fence();
@@ -727,7 +506,6 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
         if (lane == 0) mbar_arrive(bars + 8 * (GSTAGES + stage));  // this warp's reads of the slot are complete
         if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
       }
-      if (it == 0 && threadIdx.x == 128) PHK_STAMP(5);   // main loop of the first tile done
       // ---- accumulator -> staging (onto the residual where one was staged) ----
       if (tma) {
         if (pp.residual) { mbar_wait(bar_res, res_phase); res_phase ^= 1; }
@@ -736,24 +514,16 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
         acc_to_stage<false>(d, reinterpret_cast<uint8_t*>(cstage), rq, cq, ew & 3, lane, res_vec);
       }
       epi_bar_sync();  // whole tile staged
-      if (it == 0 && threadIdx.x == 128) PHK_STAMP(6);
-      if (LN_EPI)
-        epi_tma_finish_ln<EPI == 5>(pp, reinterpret_cast<uint8_t*>(cstage), base + RING_BYTES, m0, n0, ew, lg, part, lane,
-                                    rowstat, xstat, xstat_s, bar_stat, stat_phase, stat_buf, crank, csize, it, cluster_id);
-      else if (tma)
+      if (tma)
         epi_tma_finish(pp, reinterpret_cast<uint8_t*>(cstage), base + RING_BYTES, m0, n0, ew, lg, part, lane);
       else if (EPI == 2)
-        epi_geglu_tile<1>(pp, cstage, m0, n0, ew, lg, part, lane,
-                          [&](int slot) { if (it == 0 && threadIdx.x == 128) PHK_STAMP(slot); });
+        epi_geglu_tile<1>(pp, cstage, m0, n0, ew, lg, part, lane);
       else
         epi_chunk<EPI>(pp, cstage, m0, n0, res_vec, ew, lane);
-      if (it == 0 && threadIdx.x == 128) PHK_STAMP(8);      // tile written out
     }
-    if ((EPI == 0 || LN_EPI) && ew == 0 && lane == 0) tma_store_wait_read();  // staging read out before the CTA exits (the writes complete with the grid)
+    if (EPI == 0 && ew == 0 && lane == 0) tma_store_wait_read();  // staging read out before the CTA exits (the writes complete with the grid)
   }
   __syncthreads();
-  if (threadIdx.x == 0) PHK_STAMP(9);  // CTA done
-  if (EPI == 4) { __syncwarp(); cluster_sync_all(); }  // no CTA exits while a peer may still write its exchange buffer
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -829,10 +599,8 @@ static int get_c_map(const void* ptr, int64_t rows, int64_t cols, int64_t ld, CU
 
 // the TMA epilogue applies to plain fp32 outputs: identity row map, 16-byte aligned rows, residual == C (or none)
 static int maybe_tma_epilogue(EpiParams& p, int epilogue) {
-  static int on = -1;
-  if (on < 0) { const char* e = std::getenv("PHK_GEMM_TMA_EPI"); on = (e && e[0] == '0') ? 0 : 1; }
   p.tma_epi = 0;
-  if (!on || epilogue != 0 || p.seg_len != 0 || p.ldc % 4 != 0 || (reinterpret_cast<uintptr_t>(p.C) & 15) != 0 ||
+  if (epilogue != 0 || p.seg_len != 0 || p.ldc % 4 != 0 || (reinterpret_cast<uintptr_t>(p.C) & 15) != 0 ||
       (p.residual && p.residual != p.C))
     return 0;
   PHK_TRY(get_c_map(p.C, p.M, p.N, p.ldc, &p.tmC));
@@ -840,16 +608,8 @@ static int maybe_tma_epilogue(EpiParams& p, int epilogue) {
   return 0;
 }
 
-static long long* g_gemm_trace = nullptr;
-
-// set by the inference drivers (api.cu) around their GEMM calls: the W operands are weights nothing in the stream rewrites
-static thread_local int t_static_weights = 0;
-void gemm_static_weights(bool on) { t_static_weights = on ? 1 : 0; }
-
 template <int EPI>
-static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const EpiParams& p_in, cudaStream_t st) {
-  EpiParams p = p_in;
-  p.w_static = t_static_weights;
+static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const EpiParams& p, cudaStream_t st) {
   static unsigned long long configured_mask = 0;
   const bool configured = device_configured(&configured_mask);
   if (!configured) {
@@ -864,10 +624,8 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const EpiPa
 }
 
 template <int EPI>
-static int launch_gemm_dual(const CUtensorMap& ta, const CUtensorMap& tb, const EpiParams& p_in, const CUtensorMap& ta2,
+static int launch_gemm_dual(const CUtensorMap& ta, const CUtensorMap& tb, const EpiParams& p, const CUtensorMap& ta2,
                             const CUtensorMap& tb2, const EpiParams& p2, cudaStream_t st) {
-  EpiParams p = p_in;
-  p.w_static = t_static_weights;  // (read from the first problem's parameters for both)
   static unsigned long long configured_mask = 0;
   const bool configured = device_configured(&configured_mask);
   if (!configured) {
@@ -904,7 +662,7 @@ extern "C" int phk_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t 
   PHK_TRY(get_tensor_map(A, M, K, lda, GM, &ta));
   cudaStream_t st = to_stream(s);
   PHK_TRY(get_tensor_map(W, N, K, ldw, GN, &tb));
-  EpiParams p{C, ldc, M, N, K, bias, residual, seg_len, seg_stride, seg_off, (int)((M + GM - 1) / GM), (N + GN - 1) / GN, g_gemm_trace};
+  EpiParams p{C, ldc, M, N, K, bias, residual, seg_len, seg_stride, seg_off, (int)((M + GM - 1) / GM), (N + GN - 1) / GN};
   PHK_REQUIRE((int64_t)p.m_tiles * p.n_tiles < (1LL << 31), PHK_E_UNSUPPORTED, "phk_gemm_bf16: too many tiles");
   PHK_TRY(maybe_tma_epilogue(p, epilogue));
   if (epilogue == 2) return launch_gemm<2>(ta, tb, p, st);
@@ -933,91 +691,12 @@ extern "C" int phk_gemm_bf16_x2(const void* A1, int64_t lda1, const void* W1, in
   PHK_TRY(get_tensor_map(A2, M2, K2, lda2, GM, &ta2));
   PHK_TRY(get_tensor_map(W1, N1, K1, ldw1, GN, &tb));
   PHK_TRY(get_tensor_map(W2, N2, K2, ldw2, GN, &tb2));
-  EpiParams p{C1, ldc1, M1, N1, K1, bias1, nullptr, 0, 0, 0, (int)((M1 + GM - 1) / GM), (N1 + GN - 1) / GN, nullptr};
-  EpiParams p2{C2, ldc2, M2, N2, K2, bias2, nullptr, 0, 0, 0, (int)((M2 + GM - 1) / GM), (N2 + GN - 1) / GN, nullptr};
+  EpiParams p{C1, ldc1, M1, N1, K1, bias1, nullptr, 0, 0, 0, (int)((M1 + GM - 1) / GM), (N1 + GN - 1) / GN};
+  EpiParams p2{C2, ldc2, M2, N2, K2, bias2, nullptr, 0, 0, 0, (int)((M2 + GM - 1) / GM), (N2 + GN - 1) / GN};
   PHK_REQUIRE((int64_t)p.m_tiles * p.n_tiles + (int64_t)p2.m_tiles * p2.n_tiles < (1LL << 31), PHK_E_UNSUPPORTED,
               "phk_gemm_bf16_x2: too many tiles");
   // (measured: the bulk-store epilogue does not pay for the two-problem launch -- 16.2 vs 15.5 us -- so it stays off)
   return launch_gemm_dual<0>(ta, tb, p, ta2, tb2, p2, to_stream(s));
-}
-
-// x = A W^T + x in place (fp32 residual stream) AND the LayerNorm the next sub-block applies to it (attention.py:311-332:
-// x = attn(x) + x is followed by ff's / the cross-attention's LayerNorm, x = ff(x) + x by the next layer's), written as
-// the bf16 operand of the next GEMM from the epilogue's registers: ln_out[M, ln_ld] = LayerNorm(x) * ln_g (+ ln_b), and
-// optionally raw_out = bf16(x) (the k,v projection reads the un-normalised rows, attention.py:140-144).  N = the model
-// width: N / 128 in {1, 2, 4, 8} CTAs form a cluster per 128-row tile and share the row statistics.
-static int gemm_bf16_ln_impl(const void* A, int64_t lda, const void* W, int64_t ldw, float* C, int64_t ldc, int64_t M,
-                             int32_t N, int32_t K, const float* bias, const float* ln_g, const float* ln_b, float ln_eps,
-                             void* ln_out, void* raw_out, int64_t ln_ld, void* stat_ws, uint32_t* counters, phk_stream_t s) {
-  Prof prof_(FAM_GEMM_BF16, s, 2.0 * (double)M * N * K);
-  PHK_REQUIRE(A && W && C && ln_g && ln_out, PHK_E_ARG, "phk_gemm_bf16_ln: null pointer");
-  PHK_REQUIRE(M > 0 && N > 0 && K > 0 && lda >= K && ldw >= K && ldc >= N && ln_ld >= N, PHK_E_ARG, "phk_gemm_bf16_ln: bad size");
-  const int nt = N / GN;
-  PHK_REQUIRE(N % GN == 0 && (nt == 1 || nt == 2 || nt == 4 || nt == 8), PHK_E_UNSUPPORTED,
-              "phk_gemm_bf16_ln: the row width must be 128, 256, 512 or 1024");
-  PHK_REQUIRE(lda % 8 == 0 && ldw % 8 == 0 && ldc % 4 == 0 && ln_ld % 8 == 0 &&
-                  ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(W) | reinterpret_cast<uintptr_t>(C) |
-                    reinterpret_cast<uintptr_t>(ln_g) | reinterpret_cast<uintptr_t>(ln_b) | reinterpret_cast<uintptr_t>(bias) |
-                    reinterpret_cast<uintptr_t>(ln_out) | reinterpret_cast<uintptr_t>(raw_out)) & 15) == 0,
-              PHK_E_ARG, "phk_gemm_bf16_ln: operands must be 16-byte aligned with leading dimensions multiple of 8 (TMA)");
-  PHK_REQUIRE(M < (1LL << 31) - GM, PHK_E_UNSUPPORTED, "phk_gemm_bf16_ln: M too large");
-  CUtensorMap ta, tb;
-  PHK_TRY(get_tensor_map(A, M, K, lda, GM, &ta));
-  PHK_TRY(get_tensor_map(W, N, K, ldw, GN, &tb));
-  EpiParams p{C, ldc, M, N, K, bias, C, 0, 0, 0, (int)((M + GM - 1) / GM), nt, nullptr};
-  PHK_TRY(get_c_map(C, M, N, ldc, &p.tmC));
-  p.tma_epi = 1;
-  p.ln_g = ln_g; p.ln_b = ln_b; p.ln_out = ln_out; p.raw_out = raw_out; p.ln_ld = ln_ld; p.ln_eps = ln_eps;
-  p.w_static = t_static_weights;
-  static unsigned long long configured_mask = 0;
-  const bool configured = device_configured(&configured_mask);
-  if (!configured) {
-    PHK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL_LN));
-    PHK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<5, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL_LN));
-    mark_configured(&configured_mask);
-  }
-  const int max_clusters = kNumSMs / nt;
-  const int clusters = p.m_tiles < max_clusters ? p.m_tiles : max_clusters;
-  if (stat_ws) {  // groups of nt CTAs without a cluster: statistics through global memory (epilogue 5)
-    p.xstat_g = reinterpret_cast<float2*>(stat_ws);
-    p.ln_counter = counters;
-    PHK_CUDA(launch_pdl(gemm_bf16_kernel<5, false>, dim3(clusters * nt), dim3(GTHREADS), (size_t)(SMEM_TOTAL_LN), to_stream(s),
-                        ta, tb, p, ta, tb, p));
-    PHK_LAUNCH_CHECK();
-    return 0;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(clusters * nt); cfg.blockDim = dim3(GTHREADS); cfg.dynamicSmemBytes = SMEM_TOTAL_LN; cfg.stream = to_stream(s);
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = nt; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = 2;
-  PHK_CUDA(cudaLaunchKernelEx(&cfg, gemm_bf16_kernel<4, false>, ta, tb, p, ta, tb, p));
-  PHK_LAUNCH_CHECK();
-  return 0;
-}
-
-extern "C" int phk_gemm_bf16_ln(const void* A, int64_t lda, const void* W, int64_t ldw, float* C, int64_t ldc, int64_t M,
-                                int32_t N, int32_t K, const float* bias, const float* ln_g, const float* ln_b, float ln_eps,
-                                void* ln_out, void* raw_out, int64_t ln_ld, phk_stream_t s) {
-  return gemm_bf16_ln_impl(A, lda, W, ldw, C, ldc, M, N, K, bias, ln_g, ln_b, ln_eps, ln_out, raw_out, ln_ld, nullptr, nullptr, s);
-}
-
-// The same product with the row statistics exchanged through global memory instead of a cluster's distributed shared
-// memory: the N / 128 CTAs of a 128-row tile are ordinary CTAs of a grid of at most one CTA per SM (all resident), so
-// the GPC-local cluster placement that limits phk_gemm_bf16_ln to ~32 resident row tiles at N = 512 does not apply.
-//   stat_ws : PHK_LN_STAT_BYTES bytes of scratch (any content);
-//   counters: PHK_LN_COUNTERS zero-initialised 32-bit words, consumed by the call (left non-zero): give every call of a
-//             stream-ordered sequence its own words and clear them together once per sequence.
-extern "C" int phk_gemm_bf16_ln_ws(const void* A, int64_t lda, const void* W, int64_t ldw, float* C, int64_t ldc, int64_t M,
-                                   int32_t N, int32_t K, const float* bias, const float* ln_g, const float* ln_b,
-                                   float ln_eps, void* ln_out, void* raw_out, int64_t ln_ld, void* stat_ws,
-                                   uint32_t* counters, phk_stream_t s) {
-  PHK_REQUIRE(stat_ws && counters && (reinterpret_cast<uintptr_t>(stat_ws) & 15) == 0, PHK_E_ARG,
-              "phk_gemm_bf16_ln_ws: statistics scratch / counters missing or misaligned");
-  return gemm_bf16_ln_impl(A, lda, W, ldw, C, ldc, M, N, K, bias, ln_g, ln_b, ln_eps, ln_out, raw_out, ln_ld, stat_ws, counters, s);
 }
 
 // The q and k,v projections of a self-attention block (attention.py:140-157) in one launch, written as the bf16 operands
@@ -1043,8 +722,8 @@ extern "C" int phk_gemm_bf16_qkv(const void* xn, const void* xraw, int64_t lda, 
   PHK_TRY(get_tensor_map(xraw, M, K, lda, GM, &ta2));
   PHK_TRY(get_tensor_map(Wq, I, K, ldw, GN, &tb));
   PHK_TRY(get_tensor_map(Wkv, 2 * I, K, ldw, GN, &tb2));
-  EpiParams p{Qn, I, M, I, K, nullptr, nullptr, 0, 0, 0, (int)((M + GM - 1) / GM), I / GN, nullptr};
-  EpiParams p2{KVn, 2 * (int64_t)I, M, 2 * I, K, nullptr, nullptr, 0, 0, 0, (int)((M + GM - 1) / GM), 2 * I / GN, nullptr};
+  EpiParams p{Qn, I, M, I, K, nullptr, nullptr, 0, 0, 0, (int)((M + GM - 1) / GM), I / GN};
+  EpiParams p2{KVn, 2 * (int64_t)I, M, 2 * I, K, nullptr, nullptr, 0, 0, 0, (int)((M + GM - 1) / GM), 2 * I / GN};
   p.tma_epi = 0; p.nscale = q_scale; p.norm_cols = I; p.nmul = sim_scale;
   p2.tma_epi = 0; p2.nscale = k_scale; p2.norm_cols = I; p2.nmul = 1.0f;
   PHK_REQUIRE((int64_t)p.m_tiles * p.n_tiles + (int64_t)p2.m_tiles * p2.n_tiles < (1LL << 31), PHK_E_UNSUPPORTED,
@@ -1068,22 +747,7 @@ extern "C" int phk_gemm_bf16_qnorm(const void* xn, int64_t lda, const void* Wq, 
   CUtensorMap ta, tb;
   PHK_TRY(get_tensor_map(xn, M, K, lda, GM, &ta));
   PHK_TRY(get_tensor_map(Wq, I, K, ldw, GN, &tb));
-  EpiParams p{Qn, I, M, I, K, nullptr, nullptr, 0, 0, 0, (int)((M + GM - 1) / GM), I / GN, nullptr};
+  EpiParams p{Qn, I, M, I, K, nullptr, nullptr, 0, 0, 0, (int)((M + GM - 1) / GM), I / GN};
   p.tma_epi = 0; p.nscale = q_scale; p.norm_cols = I; p.nmul = sim_scale;
   return launch_gemm<3>(ta, tb, p, to_stream(s));
 }
-
-// debug / tests: kernel choice.  Modes 0..3 are accepted for ABI compatibility; every mode runs the one kernel above
-// (Hopper has no CTA-pair MMA, which modes 2 and 3 selected).
-extern "C" int phk_debug_gemm_mode(int32_t mode) {
-  PHK_REQUIRE(mode <= 3, PHK_E_ARG, "phk_debug_gemm_mode: mode must be <= 3");
-  return 0;
-}
-
-extern "C" int phk_debug_static_weights(int32_t on) {
-  gemm_static_weights(on != 0);
-  return 0;
-}
-
-// debug: device buffer of 16 x int64 per CTA receiving clock64 stamps (relative to CTA start) of the first tile
-extern "C" int phk_debug_gemm_trace(long long* device_buffer) { g_gemm_trace = device_buffer; return 0; }

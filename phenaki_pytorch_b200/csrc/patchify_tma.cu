@@ -8,7 +8,6 @@
 // are staged once per CTA.  Falls back to patchify_ln_reg_kernel (rowops.cu) when the shape does not fit a box.
 #include "phk_common.cuh"
 #include "phk_sm90.cuh"
-#include <cstdlib>
 #include <mutex>
 #include <unordered_map>
 
@@ -108,11 +107,9 @@ struct VKeyHash {
 // returns 0 when launched, 1 when the shape is not eligible (caller falls back), >1 / <0 on errors
 int patchify_ln_tma_launch(const float* video, int B, int C, int F, int H, int W, int f0, int nt, int pt, int p1, int p2,
                            const float* ln_g, const float* ln_b, void* out, int out_bf16, cudaStream_t st) {
-  static int on = -1;
-  if (on < 0) { const char* e = std::getenv("PHK_PATCHIFY_TMA"); on = (e && e[0] == '0') ? 0 : 1; }
   const int K = C * pt * p1 * p2;
   const size_t smem = (size_t)4 * K * sizeof(float);  // two token buffers + gamma + beta
-  if (!on || p2 % 4 != 0 || W % 4 != 0 || (K * 4) % 128 != 0 || p1 > 256 || p2 > 256 || pt > 256 || C > 256 || smem > 100 * 1024 ||
+  if (p2 % 4 != 0 || W % 4 != 0 || (K * 4) % 128 != 0 || p1 > 256 || p2 > 256 || pt > 256 || C > 256 || smem > 100 * 1024 ||
       ((reinterpret_cast<uintptr_t>(video) | reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(ln_g) |
         reinterpret_cast<uintptr_t>(ln_b)) & 15) != 0)
     return 1;

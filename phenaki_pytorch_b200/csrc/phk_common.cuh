@@ -6,7 +6,6 @@
 #include <float.h>
 #include <utility>
 #include "../../include/phk.h"
-#include <cstdlib>
 
 #if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
 #error "libphk is written for sm_90a (H100) only"
@@ -72,11 +71,9 @@ static inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 b
                                      Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  // PHK_PDL=0 (A/B measurements): plain stream order -- the kernels' griddepcontrol instructions are then no-ops
-  static const bool pdl = [] { const char* e = std::getenv("PHK_PDL"); return !(e && e[0] == '0'); }();
   cudaLaunchAttribute attr[1];
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = pdl ? 1 : 0;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr; cfg.numAttrs = 1;
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
@@ -159,13 +156,5 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
 }
-
-// inference drivers bracket their GEMM calls with this: the W operands are weights that no kernel of the stream rewrites,
-// so the tensor-core GEMM may request their first tiles before its programmatic-dependent-launch wait (gemm_wgmma.cu)
-void gemm_static_weights(bool on);
-struct StaticWeightsScope {
-  StaticWeightsScope() { gemm_static_weights(true); }
-  ~StaticWeightsScope() { gemm_static_weights(false); }
-};
 
 }  // namespace phk

@@ -16,7 +16,6 @@
 // Checked against the reference's gradients on the CPU by tests/cuda_emu (this very source, g++-compiled) and on the GPU
 // by tests/test_gpu_train.py.
 #include "phk_common.cuh"
-#include <cstdlib>
 // the kernels of this file are ordinary stream-ordered launches (they do not use programmatic dependent launch)
 #define PHK_KERNEL_LAUNCH(kernel, grid, block, smem, st, ...) PHK_CUDA(launch_plain(kernel, grid, block, smem, st, __VA_ARGS__))
 #include <cstring>
@@ -203,8 +202,7 @@ int sgemm_batched(const float* A, int64_t sam, int64_t sak, const float* B, int6
   dim3 grid((unsigned)((N + GB - 1) / GB), (unsigned)((M + GB - 1) / GB), (unsigned)gb.count);
   PHK_REQUIRE(grid.y <= 65535, PHK_E_UNSUPPORTED, "train: GEMM M too large");
 #ifndef PHK_CUDA_EMU
-  static const bool mma_env = [] { const char* e = std::getenv("PHK_ATTN_BWD_MMA"); return !(e && e[0] == '0'); }();
-  if (bf16_products && mma_env) {
+  if (bf16_products) {
     PHK_KERNEL_LAUNCH(hgemm_strided_kernel, dim3(grid), dim3(256), (size_t)(0), st, A, sam, sak, B, sbk, sbn, C, ldc, (int)M, (int)N, (int)K, accumulate, gb);
     PHK_LAUNCH_CHECK();
     return 0;
@@ -227,9 +225,8 @@ int dgrad(const float* dY, const float* W, float* dX, int64_t M, int64_t N, int6
 int wgrad(const float* dY, const float* X, float* dW, int64_t M, int64_t N, int64_t K, cudaStream_t st) {
   // small weight, long reduction (the position-bias MLP over thousands of coordinate deltas: [64 x 64] += over 3825 rows
   // was ONE CTA for 0.3 ms): split the reduction over the batch dimension, partial sums meet in dW through atomics
-  static const int force_split = [] { const char* e = std::getenv("PHK_WGRAD_SPLITK"); return e ? (e[0] == '0' ? 0 : 1) : -1; }();
-  if (force_split != 0 && N * K <= 4 * GB * GB && (M >= 1024 || (force_split == 1 && M > 8))) {
-    const int64_t chunk = force_split == 1 && M < 1024 ? 8 : 256;
+  if (N * K <= 4 * GB * GB && M >= 1024) {
+    const int64_t chunk = 256;
     const int parts = (int)((M + chunk - 1) / chunk);
     const GemmBatch gb{parts, 1, chunk * N, 0, chunk * K, 0, 0, 0, (int)M};
     return sgemm_batched(dY, 1, N, X, K, 1, dW, K, N, K, chunk, 2, gb, st);
@@ -795,8 +792,7 @@ int attention_backward(const float* q, const float* kv, const phk_attn_t& A, con
   // dq / dk / dv contractions: batched register-tiled products for long sequences (the warp-per-row loops of the two
   // kernels walk a column of dS / P with a stride of nkt floats: 1.5 ms per layer at n = 576), loops for short ones
   float* preQ = nullptr; float* preK = nullptr; float* preV = nullptr;
-  static const int force_gemm = [] { const char* e = std::getenv("PHK_ATTN_BWD_GEMM"); return e ? (e[0] == '0' ? 0 : 1) : -1; }();
-  if (force_gemm == 1 || (force_gemm < 0 && (int64_t)g.n * nkt >= 64 * 64)) {
+  if ((int64_t)g.n * nkt >= 64 * 64) {
     preQ = B.dS + bh * g.n * nkt;
     preK = preQ + bh * g.n * g.dh;
     preV = preK + bh * nkt * g.dh;

@@ -19,7 +19,6 @@ from torch import nn
 from . import _lib as L
 from . import sharding
 from .cvivit import CViViT
-import os
 
 from .modules import (ContinuousPositionBias, GradKeep, Keep, Transformer, Workspace, _NoParams, cpb_grad_table,
                       cpb_table, transformer_grad_table, transformer_table, weights_signature)
@@ -351,8 +350,8 @@ class _TokenTransformer(nn.Module):
         phk_train_set_progress_events.  None when there is nothing to overlap (single process, non-NCCL backend)."""
         import torch.distributed as dist
         if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and gk.flat.is_cuda
-                and dist.get_backend() == "nccl") or os.environ.get("PHK_OVERLAP_ALL_REDUCE") == "0":
-            return None  # (PHK_OVERLAP_ALL_REDUCE=0: one all-reduce of the whole bucket after the step, for A/B runs)
+                and dist.get_backend() == "nccl"):
+            return None
         groups = self._gradient_groups(gk, owner)
         if groups is None:
             return None
@@ -657,8 +656,8 @@ class Phenaki(nn.Module):
         # bf16 mode: ONE C call per demasking iteration with all state in device memory
         # (phk_maskgit_demask_iteration), replayed as ONE CUDA-graph launch per iteration from the third sample() with the
         # same shapes on (BASELINE north_star: one launch per decode iteration).  Validated on the H100 against the
-        # per-step loop (identical ids: same noise counters).  PHK_STEP_GRAPH=0 restores the per-step loop.
-        self.iteration_call = os.environ.get("PHK_STEP_GRAPH", "1") != "0"
+        # per-step loop (identical ids: same noise counters).  False restores the per-step loop.
+        self.iteration_call = True
         self._iter_bufs = {}
         self.fused_head = True  # bf16 mode: logits head + CFG + gumbel argmax fused into one GEMM (no (b,n,V) logits)
 

@@ -260,47 +260,6 @@ extern "C" int phk_attention_tc_bf16(const void* Qn, int64_t ld_q, const void* K
   });
   return 0;
 }
-// phk_gemm_bf16_ln contract: C = A W^T (+bias) + C in place (fp32) and ln_out = bf16(LayerNorm(C) * ln_g + ln_b),
-// raw_out (optional) = bf16(C); two-pass statistics in fp32 (the kernel uses sum / sum of squares over the cluster)
-extern "C" int phk_gemm_bf16_ln(const void* A, int64_t lda, const void* W, int64_t ldw, float* C, int64_t ldc, int64_t M,
-                                int32_t N, int32_t K, const float* bias, const float* ln_g, const float* ln_b, float ln_eps,
-                                void* ln_out, void* raw_out, int64_t ln_ld, phk_stream_t) {
-  if (!A || !W || !C || !ln_g || !ln_out || N % 128 || lda % 8 || ldw % 8 || ln_ld % 8) return PHK_E_ARG;
-  emu::submit([=]() {
-    const __nv_bfloat16* a = (const __nv_bfloat16*)A;
-    const __nv_bfloat16* w = (const __nv_bfloat16*)W;
-    __nv_bfloat16* lo = (__nv_bfloat16*)ln_out;
-    __nv_bfloat16* ro = (__nv_bfloat16*)raw_out;
-    for (int64_t m = 0; m < M; ++m) {
-      float mean = 0.f;
-      for (int n = 0; n < N; ++n) {
-        float acc = 0.f;
-        for (int k = 0; k < K; ++k) acc += __bfloat162float(a[m * lda + k]) * __bfloat162float(w[(int64_t)n * ldw + k]);
-        if (bias) acc += bias[n];
-        C[m * ldc + n] += acc;
-        mean += C[m * ldc + n];
-      }
-      mean /= (float)N;
-      float var = 0.f;
-      for (int n = 0; n < N; ++n) { const float d = C[m * ldc + n] - mean; var += d * d; }
-      const float rstd = 1.0f / sqrtf(var / (float)N + ln_eps);
-      for (int n = 0; n < N; ++n) {
-        const float x = C[m * ldc + n];
-        lo[m * ln_ld + n] = __float2bfloat16_rn((x - mean) * rstd * ln_g[n] + (ln_b ? ln_b[n] : 0.f));
-        if (ro) ro[m * ln_ld + n] = __float2bfloat16_rn(x);
-      }
-    }
-  });
-  return 0;
-}
-// phk_gemm_bf16_ln_ws: the same contract (the statistics scratch and the arrival counters are only touched by the GPU kernel)
-extern "C" int phk_gemm_bf16_ln_ws(const void* A, int64_t lda, const void* W, int64_t ldw, float* C, int64_t ldc, int64_t M,
-                                   int32_t N, int32_t K, const float* bias, const float* ln_g, const float* ln_b,
-                                   float ln_eps, void* ln_out, void* raw_out, int64_t ln_ld, void* stat_ws,
-                                   uint32_t* counters, phk_stream_t s) {
-  if (!stat_ws || !counters) return PHK_E_ARG;
-  return phk_gemm_bf16_ln(A, lda, W, ldw, C, ldc, M, N, K, bias, ln_g, ln_b, ln_eps, ln_out, raw_out, ln_ld, s);
-}
 // phk_gemm_bf16_qkv contract: the q and k,v projections with the attention core's operands as output (bf16): per 64-column
 // head l2-normalised (eps 1e-12) * learned scale (* sim_scale for q); the value half only converted
 extern "C" int phk_gemm_bf16_qkv(const void* xn, const void* xraw, int64_t lda, const void* Wq, const void* Wkv, int64_t ldw,

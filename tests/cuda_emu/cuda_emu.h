@@ -58,7 +58,7 @@ typedef int cudaError_t;
 enum { cudaSuccess = 0, cudaMemcpyDeviceToDevice = 3, cudaFuncAttributeMaxDynamicSharedMemorySize = 8 };
 template <typename K> static inline cudaError_t cudaFuncSetAttribute(K, int, int) { return 0; }
 // ---- host-side runtime calls of the drivers (api.cu): one in-order "stream", so events and waits are no-ops, copies are
-// memcpy, and stream capture reports failure (the drivers then keep launching eagerly, as with PHK_GRAPH=0)
+// memcpy, and stream capture reports failure (the drivers then keep launching eagerly, as after any failed capture)
 typedef void* cudaEvent_t;
 typedef void* cudaGraph_t;
 typedef void* cudaGraphExec_t;
@@ -254,5 +254,4 @@ __device__ __forceinline__ float block_sum(float v, float* red) {
   t = warp_sum(t);
   return t;
 }
-struct StaticWeightsScope {};  // the GPU GEMM's weight prefetch hint (phk_common.cuh): nothing to do on the CPU executor
 }  // namespace phk

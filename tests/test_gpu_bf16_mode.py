@@ -197,7 +197,7 @@ def test_bf16_sampling_falls_back_to_the_unfused_step_for_widths_the_fused_head_
 def test_one_graph_launch_per_iteration_equals_the_per_step_loop():
     """BASELINE north_star "one kernel launch per decode iteration": phk_maskgit_demask_iteration (default; eager on the
     first sample with a shape, captured on the second, ONE cudaGraphLaunch per iteration from the third on) against the
-    per-step loop (PHK_STEP_GRAPH=0 path): same noise counters, so the ids of four consecutive samples are identical."""
+    per-step loop (iteration_call = False): same noise counters, so the ids of four consecutive samples are identical."""
     torch.manual_seed(2)
     cv = P.CViViT(**C.SAMPLE_CVIVIT)
     mg = P.MaskGit(dim=128, num_tokens=256, max_seq_len=64, heads=2, dim_head=64, depth=2, dim_context=48)

@@ -62,17 +62,11 @@ def _core_reference(qn, kvn, n_seq, n, heads, bias=None, causal_slopes=None):
     return out.permute(0, 2, 1, 3).reshape(n_seq * n, I)
 
 
-@pytest.mark.parametrize("variant", [0, 1])
 @pytest.mark.parametrize("n_seq,n,heads,with_bias", [(72, 64, 8, True), (2, 576, 8, True), (1, 200, 4, False), (3, 130, 2, True),
                                                      (8, 576, 8, True), (2, 1024, 8, True), (5, 199, 3, True)])
-def test_attention_tc_on_prenormalised_token_major_operands(n_seq, n, heads, with_bias, variant):
-    """variant 0 / 1: the values of phk_debug_attention_tc_variant (one kernel serves both).  (8, 576, 8): the MaskGit
-    shape; n = 199: odd bias rows (scalar loads) and a ragged last chunk."""
-    L.check(L.lib().phk_debug_attention_tc_variant(variant))
-    try:
-        _attention_tc_case(n_seq, n, heads, with_bias)
-    finally:
-        L.lib().phk_debug_attention_tc_variant(-1)
+def test_attention_tc_on_prenormalised_token_major_operands(n_seq, n, heads, with_bias):
+    """(8, 576, 8): the MaskGit shape; n = 199: odd bias rows (scalar loads) and a ragged last chunk."""
+    _attention_tc_case(n_seq, n, heads, with_bias)
 
 
 @pytest.mark.parametrize("n_seq,n,heads,with_bias", [(72, 64, 8, True), (5, 49, 3, True), (3, 17, 2, False), (2, 64, 4, False),
@@ -126,91 +120,6 @@ def test_small_attention_on_prenormalised_operands(n_outer, n_inner, n, heads, c
     torch.cuda.synchronize()
     err = (out.cpu().float()[idx] - ref).abs().max().item()
     assert err <= 0.02, f"max |err| {err}"
-
-
-@pytest.mark.parametrize("M,N,K,raw", [(4608, 512, 512, False), (4608, 512, 1408, True), (300, 256, 192, True), (129, 128, 64, False),
-                                       (2304, 1024, 512, True), (40000, 512, 512, False)])
-def test_residual_gemm_with_layernorm_epilogue(M, N, K, raw):
-    """phk_gemm_bf16_ln: x += A W^T in place (fp32) and bf16 LayerNorm(x) (+ raw bf16 x) from the same epilogue; row
-    statistics summed over the cluster of N / 128 CTAs.  40000 rows: more m-tiles than clusters (persistent loop, both
-    exchange buffers in use)."""
-    a = TC.seeded_randn((M, K), 430).bfloat16()
-    w = (TC.seeded_randn((N, K), 431) / K ** 0.5).bfloat16()
-    x = TC.seeded_randn((M, N), 432) * 2 + 0.5
-    g, b = TC.seeded_randn((N,), 433) * 0.2 + 1.0, TC.seeded_randn((N,), 434) * 0.1
-    ref_x = x + a.float() @ w.float().t()
-    ref_ln = F.layer_norm(ref_x, (N,), g, b)
-    ad, wd, xd, gd, bd = a.to(DEV), w.to(DEV), x.clone().to(DEV), g.to(DEV), b.to(DEV)
-    ln = torch.full((M, N), 9.0, dtype=torch.bfloat16, device=DEV)
-    rw = torch.full((M, N), 9.0, dtype=torch.bfloat16, device=DEV) if raw else None
-    L.check(L.lib().phk_gemm_bf16_ln(L.ptr(ad), K, L.ptr(wd), K, L.ptr(xd), N, M, N, K, None, L.ptr(gd), L.ptr(bd), 1e-5,
-                                     L.ptr(ln), L.ptr(rw), N, L.stream_ptr()), "phk_gemm_bf16_ln")
-    torch.cuda.synchronize()
-    torch.testing.assert_close(xd.cpu(), ref_x, rtol=1e-4, atol=1e-4)
-    torch.testing.assert_close(ln.cpu().float(), ref_ln, rtol=1e-2, atol=2e-2)
-    if raw:
-        torch.testing.assert_close(rw.cpu().float(), ref_x, rtol=1e-2, atol=2e-2)
-
-
-@pytest.mark.parametrize("M,N,K,raw", [(4608, 512, 512, False), (4608, 512, 1408, True), (300, 256, 192, True), (129, 128, 64, False),
-                                       (2304, 1024, 512, True), (40000, 512, 512, False)])
-def test_residual_gemm_with_layernorm_epilogue_global_exchange(M, N, K, raw):
-    """phk_gemm_bf16_ln_ws: the same epilogue, row statistics exchanged through global memory between the N / 128 CTAs of a
-    row tile (no cluster).  Three calls back to back, each on its own zeroed counters and all on ONE statistics scratch
-    (the way a transformer call uses it); 40000 rows: several row tiles per CTA group, both slot parities in use."""
-    a = TC.seeded_randn((M, K), 430).bfloat16()
-    w = (TC.seeded_randn((N, K), 431) / K ** 0.5).bfloat16()
-    x = TC.seeded_randn((M, N), 432) * 2 + 0.5
-    g, b = TC.seeded_randn((N,), 433) * 0.2 + 1.0, TC.seeded_randn((N,), 434) * 0.1
-    ad, wd, gd, bd = a.to(DEV), w.to(DEV), g.to(DEV), b.to(DEV)
-    stat = torch.full((L.LN_STAT_BYTES // 4,), float("nan"), dtype=torch.float32, device=DEV)
-    counters = torch.zeros((3, L.LN_COUNTERS), dtype=torch.int32, device=DEV)
-    xd = x.clone().to(DEV)
-    ref_x = x.clone()
-    for call in range(3):
-        ref_x = ref_x + a.float() @ w.float().t()
-        ln = torch.full((M, N), 9.0, dtype=torch.bfloat16, device=DEV)
-        rw = torch.full((M, N), 9.0, dtype=torch.bfloat16, device=DEV) if raw else None
-        L.check(L.lib().phk_gemm_bf16_ln_ws(L.ptr(ad), K, L.ptr(wd), K, L.ptr(xd), N, M, N, K, None, L.ptr(gd), L.ptr(bd), 1e-5,
-                                            L.ptr(ln), L.ptr(rw), N, L.ptr(stat), L.ptr(counters[call]), L.stream_ptr()),
-                "phk_gemm_bf16_ln_ws")
-    torch.cuda.synchronize()
-    ref_ln = F.layer_norm(ref_x, (N,), g, b)
-    torch.testing.assert_close(xd.cpu(), ref_x, rtol=2e-4, atol=2e-4)
-    torch.testing.assert_close(ln.cpu().float(), ref_ln, rtol=1e-2, atol=3e-2)
-    if raw:
-        torch.testing.assert_close(rw.cpu().float(), ref_x, rtol=1e-2, atol=3e-2)
-
-
-@pytest.mark.parametrize("fuse", ["1", "2"])
-def test_transformer_with_layernorm_in_gemm_epilogue_matches_separate_kernels(fuse):
-    """PHK_FUSE_LN (read once per process): the whole bf16 C-ViViT encode with the LayerNorms folded into the residual GEMMs
-    (1 cluster exchange, 2 global exchange) against the default separate-kernel path, run in child processes."""
-    import json
-    import os
-    import subprocess
-    import sys
-    code = (
-        "import json, torch\n"
-        "import phenaki_pytorch_b200 as P\n"
-        "from phenaki_pytorch_b200 import _lib as L\n"
-        "torch.manual_seed(0)\n"
-        "m = P.CViViT(dim=512, codebook_size=65536, image_size=256, patch_size=32, temporal_patch_size=2, spatial_depth=4,\n"
-        "             temporal_depth=4, dim_head=64, heads=8, use_vgg_and_gan=False).cuda().eval()\n"
-        "m.precision = L.PREC_BF16\n"
-        "v = torch.randn((2, 3, 17, 256, 256), generator=torch.Generator().manual_seed(77)).cuda()\n"
-        "ids = m(v, return_only_codebook_ids=True)\n"
-        "print(json.dumps(ids.flatten().tolist()))\n")
-    outs = {}
-    for mode in ("0", fuse):
-        env = dict(os.environ, PHK_FUSE_LN=mode)
-        r = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=300,
-                           cwd=os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-        assert r.returncode == 0, r.stderr[-2000:]
-        outs[mode] = json.loads(r.stdout.strip().splitlines()[-1])
-    a, b = torch.tensor(outs["0"]), torch.tensor(outs[fuse])
-    flipped = sum(bin(int(x)).count("1") for x in (a ^ b).tolist())
-    assert flipped <= 0.002 * a.numel() * 16, f"{flipped} of {a.numel() * 16} token-id bits differ"
 
 
 @pytest.mark.parametrize("b,n,ctx_len,heads,cfg", [(4, 576, 16, 8, True), (2, 130, 29, 4, False), (3, 64, 7, 2, True)])

@@ -108,20 +108,9 @@ def test_attention_tensor_core_matches_oracle(n_seq, n, heads, with_bias):
     assert err <= 0.02, f"max |err| {err}"
 
 
-@pytest.fixture
-def gemm_mode():
-    """Forces one wgmma GEMM variant (1 one-CTA 128x128, 2 CTA pairs 256x128, 3 CTA pairs 256x256) for a test."""
-    lib = L.lib()
-    yield lambda m: L.check(lib.phk_debug_gemm_mode(m))
-    lib.phk_debug_gemm_mode(-1)
-
-
-@pytest.mark.parametrize("mode", [1, 2, 3])
 @pytest.mark.parametrize("M,N,K", [(256, 256, 64), (600, 700, 200), (4608, 512, 512), (1300, 1000, 1408), (129, 96, 72)])
-def test_gemm_variants_fp32_out_bias_residual_rowmap(gemm_mode, mode, M, N, K):
-    """Every kernel variant (cta_group::1 and the cta_group::2 pair kernels) on ragged M / N / K, with bias, in-place
-    residual and the output row map."""
-    gemm_mode(mode)
+def test_gemm_variants_fp32_out_bias_residual_rowmap(M, N, K):
+    """Ragged M / N / K, with bias, in-place residual and the output row map."""
     Kp = (K + 7) // 8 * 8
     a, w = operands(M, N, K, lda=Kp, ldw=Kp, seed=20)
     bias, res = TC.seeded_randn((N,), 25), TC.seeded_randn((M, N), 26)
@@ -140,9 +129,7 @@ def test_gemm_variants_fp32_out_bias_residual_rowmap(gemm_mode, mode, M, N, K):
     torch.testing.assert_close(c2.cpu()[idx], ref - bias - res, rtol=1e-4, atol=2e-3 * max(1.0, (K / 512) ** 0.5))
 
 
-@pytest.mark.parametrize("mode", [1, 2, 3])
-def test_gemm_variants_bf16_out_and_geglu(gemm_mode, mode):
-    gemm_mode(mode)
+def test_gemm_variants_bf16_out_and_geglu():
     M, N, K = 700, 520, 256
     a, w = operands(M, N, K, seed=30)
     bias = TC.seeded_randn((N,), 31)
@@ -152,7 +139,7 @@ def test_gemm_variants_bf16_out_and_geglu(gemm_mode, mode):
     L.check(L.lib().phk_gemm_bf16(L.ptr(ad), K, L.ptr(wd), K, L.ptr(c), N, M, N, K, L.ptr(bd), None, 0, 0, 0, 1,
                                   L.stream_ptr()), "phk_gemm_bf16")
     torch.testing.assert_close(c.cpu().float(), ref, rtol=1e-2, atol=5e-2)
-    # GEGLU: W rows packed [64 value | 64 gate]; 5 groups -> a 256-wide pair tile with a ragged second half
+    # GEGLU: W rows packed [64 value | 64 gate]; 5 groups, the last one ragged
     inner, K2 = 300, 512
     inner_pad = (inner + 63) // 64 * 64
     a2 = TC.seeded_randn((M, K2), 32).bfloat16()
@@ -200,9 +187,8 @@ def test_geglu_epilogue_activation_error_is_below_bf16_rounding():
 
 @pytest.mark.parametrize("M,N1,N2,K1,K2", [(4608, 512, 1024, 512, 512), (300, 200, 130, 72, 136), (129, 64, 64, 64, 64)])
 def test_gemm_x2_two_problems_in_one_launch(M, N1, N2, K1, K2):
-    """phk_gemm_bf16_x2 (q and k,v projections of one attention block in a single persistent launch) equals two
-    separate phk_gemm_bf16 calls bit for bit when both use the one-CTA kernel (same tiles, same K order), and the fp32
-    product of the bf16 operands in every variant."""
+    """phk_gemm_bf16_x2 (q and k,v projections of one attention block in a single persistent launch) equals the fp32
+    product of the bf16 operands, and two separate phk_gemm_bf16 calls bit for bit (same tiles, same K order)."""
     a1, w1 = operands(M, N1, K1, seed=50)
     a2, w2 = operands(M, N2, K2, seed=52)
     d = [t.to(DEV) for t in (a1, w1, a2, w2)]
@@ -213,21 +199,10 @@ def test_gemm_x2_two_problems_in_one_launch(M, N1, N2, K1, K2):
                                  K2, L.ptr(c2), N2, M, N2, K2, None, L.stream_ptr()), "phk_gemm_bf16_x2")
     torch.testing.assert_close(c1.cpu(), a1.float() @ w1.float().t(), rtol=1e-4, atol=2e-3)
     torch.testing.assert_close(c2.cpu(), a2.float() @ w2.float().t(), rtol=1e-4, atol=2e-3)
-    L.check(lib.phk_debug_gemm_mode(1))   # one-CTA kernels on both sides: same tiles, same K order -> identical bits
-    try:
-        s1, s2, t1, t2 = torch.empty_like(c1), torch.empty_like(c2), torch.empty_like(c1), torch.empty_like(c2)
-        L.check(lib.phk_gemm_bf16(L.ptr(d[0]), K1, L.ptr(d[1]), K1, L.ptr(s1), N1, M, N1, K1, None, None, 0, 0, 0, 0, L.stream_ptr()))
-        L.check(lib.phk_gemm_bf16(L.ptr(d[2]), K2, L.ptr(d[3]), K2, L.ptr(s2), N2, M, N2, K2, None, None, 0, 0, 0, 0, L.stream_ptr()))
-        L.check(lib.phk_gemm_bf16_x2(L.ptr(d[0]), K1, L.ptr(d[1]), K1, L.ptr(t1), N1, M, N1, K1, None, L.ptr(d[2]), K2,
-                                     L.ptr(d[3]), K2, L.ptr(t2), N2, M, N2, K2, None, L.stream_ptr()), "phk_gemm_bf16_x2")
-        assert torch.equal(s1, t1) and torch.equal(s2, t2)
-        L.check(lib.phk_debug_gemm_mode(3))   # the CTA-pair variant of the two-problem launch
-        L.check(lib.phk_gemm_bf16_x2(L.ptr(d[0]), K1, L.ptr(d[1]), K1, L.ptr(t1), N1, M, N1, K1, None, L.ptr(d[2]), K2,
-                                     L.ptr(d[3]), K2, L.ptr(t2), N2, M, N2, K2, None, L.stream_ptr()), "phk_gemm_bf16_x2")
-        torch.testing.assert_close(t1.cpu(), a1.float() @ w1.float().t(), rtol=1e-4, atol=2e-3)
-        torch.testing.assert_close(t2.cpu(), a2.float() @ w2.float().t(), rtol=1e-4, atol=2e-3)
-    finally:
-        lib.phk_debug_gemm_mode(-1)
+    s1, s2 = torch.empty_like(c1), torch.empty_like(c2)
+    L.check(lib.phk_gemm_bf16(L.ptr(d[0]), K1, L.ptr(d[1]), K1, L.ptr(s1), N1, M, N1, K1, None, None, 0, 0, 0, 0, L.stream_ptr()))
+    L.check(lib.phk_gemm_bf16(L.ptr(d[2]), K2, L.ptr(d[3]), K2, L.ptr(s2), N2, M, N2, K2, None, None, 0, 0, 0, 0, L.stream_ptr()))
+    assert torch.equal(s1, c1) and torch.equal(s2, c2)
 
 
 def test_gemm_x2_different_row_counts_and_biases():

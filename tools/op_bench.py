@@ -61,38 +61,6 @@ for (M, N, K, epi, name) in [(4608, 512, 512, 0, "gemm q/out-proj (+res)"), (460
     timeit(name + f" {M}x{N}x{K}", lambda: L.check(lib.phk_gemm_bf16(L.ptr(a), K, L.ptr(w), K, L.ptr(c), c.shape[1], M, N, K, None, res, 0, 0, 0, epi, sp())),
            2.0 * M * N * K, "TFLOP/s")
 
-# the same products with the weights declared static (W tiles requested before the dependency wait), as the forward drivers run them
-L.check(lib.phk_debug_static_weights(1))
-for (M, N, K, epi, name) in [(4608, 512, 512, 0, "gemm q/out-proj (+res), static W"), (4608, 512, 1408, 0, "gemm FF2 (+res), static W"),
-                             (4608, 1024, 512, 0, "gemm kv-proj, static W")]:
-    a = torch.randn(M, K, device=dev).to(bf)
-    w = torch.randn(N, K, device=dev).to(bf)
-    c = torch.zeros(M, N, device=dev, dtype=torch.float32)
-    res = L.ptr(c) if N == 512 else None
-    timeit(name + f" {M}x{N}x{K}", lambda: L.check(lib.phk_gemm_bf16(L.ptr(a), K, L.ptr(w), K, L.ptr(c), N, M, N, K, None, res, 0, 0, 0, epi, sp())),
-           2.0 * M * N * K, "TFLOP/s")
-# residual GEMM + the following LayerNorm in one launch: cluster exchange vs global-memory exchange
-stat = torch.empty(L.LN_STAT_BYTES // 4, device=dev)
-ctr = torch.zeros(64, L.LN_COUNTERS, dtype=torch.int32, device=dev)
-ln_o = torch.empty(R, D, dtype=bf, device=dev)
-for (K, name) in [(512, "out-proj"), (1408, "FF2")]:
-    a = torch.randn(R, K, device=dev).to(bf)
-    w = (torch.randn(D, K, device=dev) / K ** 0.5).to(bf)
-    c = torch.zeros(R, D, device=dev)
-    gg, bb = torch.ones(D, device=dev), torch.zeros(D, device=dev)
-    timeit(f"gemm {name} (+res) + LayerNorm, cluster {R}x{D}x{K}", lambda: L.check(lib.phk_gemm_bf16_ln(L.ptr(a), K, L.ptr(w), K, L.ptr(c), D, R, D, K, None, L.ptr(gg), L.ptr(bb), 1e-5, L.ptr(ln_o), None, D, sp())),
-           2.0 * R * D * K, "TFLOP/s")
-    slot = [0]
-
-    def ln_ws():
-        # every launch needs its own zeroed counters: one memset per 16 launches (a transformer call clears them once)
-        if slot[0] % 16 == 0:
-            ctr[:16].zero_()
-        L.check(lib.phk_gemm_bf16_ln_ws(L.ptr(a), K, L.ptr(w), K, L.ptr(c), D, R, D, K, None, L.ptr(gg), L.ptr(bb), 1e-5, L.ptr(ln_o), None, D, L.ptr(stat), L.ptr(ctr[slot[0] % 16]), sp()))
-        slot[0] += 1
-    timeit(f"gemm {name} (+res) + LayerNorm, global exchange {R}x{D}x{K}", ln_ws, 2.0 * R * D * K, "TFLOP/s")
-L.check(lib.phk_debug_static_weights(0))
-
 a1 = torch.randn(R, D, device=dev).to(bf); a2 = torch.randn(R, D, device=dev).to(bf)
 w1 = torch.randn(I, D, device=dev).to(bf); w2 = torch.randn(2 * I, D, device=dev).to(bf)
 c1 = torch.zeros(R, I, device=dev); c2 = torch.zeros(R, 2 * I, device=dev)
@@ -112,15 +80,12 @@ gt.o_outer, gt.o_inner, gt.o_tok = gt.q_outer, gt.q_inner, gt.q_tok
 gt.mask_off_from, gt.scale, gt.out_bf16 = -1, 8.0, 1
 timeit("attention temporal (512 seq x 9, warp kernel)", lambda: L.check(lib.phk_attention(L.ptr(q), L.ptr(kv), None, L.ptr(ones), L.ptr(ones), None, None, L.ptr(slopes), L.ptr(o_h), C.byref(gt), sp())))
 
-# the attention core alone on bf16 operands (as the fused q/k,v projection writes them), both probability paths
+# the attention core alone on bf16 operands (as the fused q/k,v projection writes them)
 qn_h, kvn_h = torch.randn(R, I, device=dev).to(bf), torch.randn(R, 2 * I, device=dev).to(bf)
 for (ns, n) in [(72, 64), (8, 576)]:
     bias = torch.randn(8, n, n, device=dev)
-    for variant, label in [(0, "P via shared memory, 2 CTAs/SM"), (1, "P in tensor memory, 3 CTAs/SM")]:
-        L.check(lib.phk_debug_attention_tc_variant(variant))
-        timeit(f"attention tc core ({ns} seq x {n}) {label}", lambda: L.check(lib.phk_attention_tc_bf16(L.ptr(qn_h), I, L.ptr(kvn_h), 2 * I, L.ptr(bias), L.ptr(o_h), ns, n, 8, sp())),
-               4.0 * ns * 8 * n * n * 64, "TFLOP/s")
-L.check(lib.phk_debug_attention_tc_variant(-1))
+    timeit(f"attention tc core ({ns} seq x {n})", lambda: L.check(lib.phk_attention_tc_bf16(L.ptr(qn_h), I, L.ptr(kvn_h), 2 * I, L.ptr(bias), L.ptr(o_h), ns, n, 8, sp())),
+           4.0 * ns * 8 * n * n * 64, "TFLOP/s")
 bias64 = torch.randn(8, 64, 64, device=dev)
 timeit("attention mid mma (72 seq x 64), one CTA per (sequence, head)", lambda: L.check(lib.phk_attention_mid_bf16(L.ptr(qn_h), I, L.ptr(kvn_h), 2 * I, L.ptr(bias64), L.ptr(o_h), 72, 64, 8, sp())),
        4.0 * 72 * 8 * 64 * 64 * 64, "TFLOP/s")
