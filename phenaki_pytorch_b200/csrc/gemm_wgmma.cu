@@ -16,7 +16,8 @@
 //              bulk-stored from them; otherwise staged in a padded smem tile and written with coalesced rows
 //            1 bf16 (+bias)
 //            2 GEGLU (attention.py:40-43) on W rows packed [64 value rows | 64 gate rows] per 128-column tile ->
-//              bf16 [M, N/2]: fitted sigmoid-form GELU, swizzled bf16 staging tile, coalesced 16-byte stores.
+//              bf16 [M, N/2], fitted sigmoid-form GELU: gemm_bf16_geglu_kernel below (ping-pong, m64n128k16, the GEGLU
+//              from the accumulator registers), measured faster on these many-tile products.
 #include "phk_common.cuh"
 #include "phk_sm90.cuh"
 #include <mutex>
@@ -29,7 +30,6 @@ constexpr int GN = 128;       // BLOCK_N: two 64-column halves
 constexpr int GK = 64;        // BLOCK_K: 64 bf16 = 128 B = one SWIZZLE_128B row
 constexpr int GSTAGES = 4;
 constexpr int EPI_WARPS = 16;       // MMA + epilogue warps 4..19: four per 32-row group, each a quarter of the columns
-constexpr int EPI_PARTS = EPI_WARPS / 4;            // column parts per row group
 constexpr int GTHREADS = 128 + EPI_WARPS * 32;      // 640: the producer warpgroup + four MMA / epilogue warpgroups
 constexpr int STAGE_BYTES = GM * GK * 2;          // 16 KB per operand per stage
 constexpr int CPAD = 132;                          // fp32 staging row stride (floats): conflict-free 128-bit rows
@@ -129,77 +129,6 @@ __device__ __forceinline__ bool epi_residual_prefetch(const EpiParams& p, float*
     epi_bar_sync();  // residual chunk complete before the row-per-thread accumulate
   }
   return res_vec;
-}
-
-// GEGLU epilogue of a tile of one 128-column chunk packed [64 value | 64 gate] (attention.py:40-43), the accumulator
-// staged as CPAD rows.  All accumulator columns this thread needs (16 value + 16 gate of ONE row) are read first; after
-// a barrier the staging memory takes the bf16 results (128 B per row), which leave as fully coalesced 16-B-per-lane
-// rows: one row per thread straight from registers made every warp store touch 32 different lines.
-template <int NCH>
-__device__ __forceinline__ void epi_geglu_tile(const EpiParams& p, void* stage, int64_t m0, int n0, int ew, int lg,
-                                               int part, int lane) {
-  static_assert(NCH == 1, "one 128-column chunk per tile");
-  constexpr int W = 64 / EPI_PARTS;
-  static_assert(W == 16, "two 16-B units per thread and chunk");
-  constexpr int U = NCH * 8;  // 16-B units per staged row
-  uint32_t val[NCH][W], gate[NCH][W];
-  {
-    const uint32_t* arow = reinterpret_cast<const uint32_t*>(stage) + (lg * 32 + lane) * CPAD;
-#pragma unroll
-    for (int j = 0; j < W; j += 4) {
-      const uint4 a = *reinterpret_cast<const uint4*>(arow + part * W + j);
-      const uint4 b = *reinterpret_cast<const uint4*>(arow + 64 + part * W + j);
-      val[0][j] = a.x; val[0][j + 1] = a.y; val[0][j + 2] = a.z; val[0][j + 3] = a.w;
-      gate[0][j] = b.x; gate[0][j + 1] = b.y; gate[0][j + 2] = b.z; gate[0][j + 3] = b.w;
-    }
-  }
-  epi_bar_sync();  // every thread has read its columns: the staging memory takes the bf16 results
-  const uint32_t seg_len = (uint32_t)p.seg_len;
-  const bool coalesced = (p.ldc % 8 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
-  const int r = lg * 32 + lane;  // this thread's row of the tile
-  uint4* srow = reinterpret_cast<uint4*>(stage) + r * U;
-#pragma unroll
-  for (int h = 0; h < NCH; ++h) {
-    uint32_t pk[W / 2];
-#pragma unroll
-    for (int j = 0; j < W; j += 2)
-      pk[j / 2] = pack_bf16x2(geglu_fast(__uint_as_float(gate[h][j]), __uint_as_float(val[h][j])),
-                              geglu_fast(__uint_as_float(gate[h][j + 1]), __uint_as_float(val[h][j + 1])));
-    if (coalesced) {
-      // logical unit u of row r lives at (u & ~7) | ((u ^ r) & 7): conflict-free for the row-per-lane stores here
-      // and for the unit-per-lane loads below
-      const int u0 = h * 8 + part * 2;
-      srow[(u0 & ~7) | ((u0 ^ r) & 7)] = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-      srow[((u0 + 1) & ~7) | (((u0 + 1) ^ r) & 7)] = make_uint4(pk[4], pk[5], pk[6], pk[7]);
-    } else {  // odd leading dimension / unaligned C: 4-byte stores from registers
-      const uint32_t m = (uint32_t)m0 + r;
-      const int col = (n0 + h * 128) / 2 + part * W;
-      if (m < (uint32_t)p.M && col < p.N / 2) {
-        int64_t orow = m;
-        if (seg_len > 0) { const uint32_t q = m / seg_len; orow = q * (uint32_t)p.seg_stride + (uint32_t)p.seg_off + (m - q * seg_len); }
-        __nv_bfloat16* crow = reinterpret_cast<__nv_bfloat16*>(p.C) + orow * p.ldc + col;
-#pragma unroll
-        for (int j = 0; j < W / 2; ++j) *reinterpret_cast<uint32_t*>(crow + 2 * j) = pk[j];
-      }
-    }
-  }
-  if (!coalesced) return;  // uniform over the CTA
-  epi_bar_sync();          // tile staged
-  constexpr int RPI = 32 / U;                 // rows per warp instruction (4 or 2)
-  const int rl = lane / U, u = lane % U;      // this lane's row within the instruction and its 16-B unit
-  const bool chunk_ok = (n0 + (u >> 3) * 128) < p.N;
-#pragma unroll
-  for (int i = 0; i < GM / (EPI_WARPS * RPI); ++i) {
-    const int rr = (i * EPI_WARPS + ew) * RPI + rl;
-    const uint32_t m = (uint32_t)m0 + rr;
-    const uint4 v = reinterpret_cast<const uint4*>(stage)[rr * U + ((u & ~7) | ((u ^ rr) & 7))];
-    if (m < (uint32_t)p.M && chunk_ok) {
-      int64_t orow = m;
-      if (seg_len > 0) { const uint32_t q = m / seg_len; orow = q * (uint32_t)p.seg_stride + (uint32_t)p.seg_off + (m - q * seg_len); }
-      *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.C) + orow * p.ldc + n0 / 2 + u * 8) = v;
-    }
-  }
-  epi_bar_sync();          // staging tile free for the next accumulator
 }
 
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
@@ -516,12 +445,142 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
       epi_bar_sync();  // whole tile staged
       if (tma)
         epi_tma_finish(pp, reinterpret_cast<uint8_t*>(cstage), base + RING_BYTES, m0, n0, ew, lg, part, lane);
-      else if (EPI == 2)
-        epi_geglu_tile<1>(pp, cstage, m0, n0, ew, lg, part, lane);
       else
         epi_chunk<EPI>(pp, cstage, m0, n0, res_vec, ew, lane);
     }
     if (EPI == 0 && ew == 0 && lane == 0) tma_store_wait_read();  // staging read out before the CTA exits (the writes complete with the grid)
+  }
+  __syncthreads();
+}
+
+// ---------------------------------------------------------------------------------------------------
+// GEGLU products (epilogue 2: FF1 of every feed-forward block, 22 column tiles, several tiles per CTA): ping-pong
+// ---------------------------------------------------------------------------------------------------
+// Warpgroup 0 is the TMA producer (one thread; the warpgroup gives its registers away to the MMA warpgroups) feeding a
+// GG_STAGES-deep ring in the order the CTA's tiles are consumed.  Warpgroups 1 and 2 take the CTA's tiles in turn: each
+// multiplies a whole 128 x 128 tile as two m64n128k16 row halves that share every W slice (6 KB of operands per 64
+// tensor-core clocks instead of 4 KB per 32 for a 64 x 64 quadrant), keeps one k-block of MMAs in flight, and runs the
+// GEGLU straight from its accumulator registers while the other warpgroup runs the next tile's main loop: value column
+// c and gate column c + 64 of a row are held by the same lane, so no staging is needed.  A named-barrier handshake
+// orders the main loops, so the two warpgroups never interleave their MMAs.  Per output element the k-order (k-blocks
+// of 64 in order, k = 16 steps in order) is that of the quadrant kernel.
+constexpr int GG_STAGES = 6;
+constexpr int GG_THREADS = 384;
+constexpr int GG_PRODUCER_REGS = 40, GG_CONSUMER_REGS = 232;  // 128 x 40 + 256 x 232 <= 64 K registers
+constexpr int GG_SMEM_TOTAL = GG_STAGES * 2 * STAGE_BYTES + 128 /*barriers*/ + 1024 /*manual 1024-B alignment*/;
+constexpr int GG_BAR_TURN = 1;  // named barriers 1, 2: main-loop turn of MMA warpgroup 0, 1
+
+__global__ void __launch_bounds__(GG_THREADS, 1) gemm_bf16_geglu_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                        const __grid_constant__ CUtensorMap tmB,
+                                                                        const __grid_constant__ EpiParams p) {
+  pdl_trigger();
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B atoms need 1024-B alignment
+  const uint32_t sA = base, sB = base + GG_STAGES * STAGE_BYTES;
+  const uint32_t bars = base + GG_STAGES * 2 * STAGE_BYTES;  // full[s] @ +8s ; empty[s] @ +8(S+s)
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int num_tiles = p.m_tiles * p.n_tiles;
+  const int my_tiles = (int)blockIdx.x < num_tiles ? (num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  const int num_kb = (p.K + GK - 1) / GK;
+  auto tile_of = [&](int i, int& m0, int& n0) {  // round-robin, m-fastest
+    const int tile = (int)blockIdx.x + i * (int)gridDim.x;
+    m0 = (tile % p.m_tiles) * GM;
+    n0 = (tile / p.m_tiles) * GN;
+  };
+
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+    for (int s = 0; s < GG_STAGES; ++s) {
+      mbar_init(bars + 8 * s, 1);
+      mbar_init(bars + 8 * (GG_STAGES + s), 4);  // one arrival per warp of the consuming MMA warpgroup
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  pdl_wait();  // everything above (barriers, tensor-map prefetch) overlapped the previous kernel
+
+  if (warp < 4) {
+    // ===================== TMA producer =====================
+    setmaxnreg_dec<GG_PRODUCER_REGS>();
+    if (warp == 0 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int it = 0; it < my_tiles; ++it) {
+        int m0, n0;
+        tile_of(it, m0, n0);
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(bars + 8 * (GG_STAGES + stage), phase ^ 1);  // slot free (passes immediately on the first lap)
+          const uint32_t full = bars + 8 * stage;
+          mbar_expect_tx(full, 2 * STAGE_BYTES);
+          tma_load_2d(&tmA, full, sA + stage * STAGE_BYTES, kb * GK, m0);
+          tma_load_2d(&tmB, full, sB + stage * STAGE_BYTES, kb * GK, n0);
+          if (++stage == GG_STAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== MMA + GEGLU: warpgroup wg takes the CTA's tiles wg, wg + 2, ... =====================
+    setmaxnreg_inc<GG_CONSUMER_REGS>();
+    const int wg = (warp >> 2) - 1;
+    const int w = warp & 3;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int it = 0; it < my_tiles; ++it) {
+      if ((it & 1) != wg) {  // the other warpgroup's tile: skip its k-blocks in the ring
+        stage += num_kb;
+        while (stage >= GG_STAGES) { stage -= GG_STAGES; phase ^= 1; }
+        continue;
+      }
+      int m0, n0;
+      tile_of(it, m0, n0);
+      if (it > 0) named_bar_sync(GG_BAR_TURN + wg, 256);  // the other warpgroup has issued tile it - 1
+      // acc[h][4j + 2i + e] = (row 64h + 16w + lane/4 + 8i, column 8j + 2(lane%4) + e) of the tile
+      float acc[2][64];
+      int prev = 0;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(bars + 8 * stage, phase);
+        const uint64_t da0 = gmma_desc(sA + stage * STAGE_BYTES);
+        const uint64_t da1 = gmma_desc(sA + stage * STAGE_BYTES + 64 * 128);
+        const uint64_t db = gmma_desc(sB + stage * STAGE_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GK / 16; ++k) {  // +32 B per K = 16 inside the 128-B swizzle row => +2 in the address field
+          const uint32_t accumulate = (kb > 0 || k > 0) ? 1u : 0u;
+          wgmma_m64n128k16_ss(acc[0], da0 + 2 * k, db + 2 * k, accumulate);
+          wgmma_m64n128k16_ss(acc[1], da1 + 2 * k, db + 2 * k, accumulate);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();  // k-block kb - 1 retired: its slot can be refilled while kb runs
+        if (kb > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bars + 8 * (GG_STAGES + prev));
+        }
+        prev = stage;
+        if (++stage == GG_STAGES) { stage = 0; phase ^= 1; }
+      }
+      if (it + 1 < my_tiles) named_bar_arrive(GG_BAR_TURN + (wg ^ 1), 256);  // the other warpgroup's turn
+      wgmma_wait<0>();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bars + 8 * (GG_STAGES + prev));
+      // GEGLU of the [64 value | 64 gate] tile -> bf16 columns n0/2 + 8j + 2(lane%4) + e, j < 8 (N % 128 == 0, even ldc
+      // and 4-byte aligned C: checked on the host)
+      __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C);
+      const int oc = n0 / 2 + 2 * (lane & 3);
+#pragma unroll
+      for (int r = 0; r < 4; ++r) {
+        const uint32_t m = (uint32_t)m0 + 64 * (r >> 1) + 16 * w + (lane >> 2) + 8 * (r & 1);
+        if (m >= (uint32_t)p.M) continue;
+        int64_t orow = m;
+        const uint32_t seg_len = (uint32_t)p.seg_len;
+        if (seg_len > 0) { const uint32_t q = m / seg_len; orow = q * (uint32_t)p.seg_stride + (uint32_t)p.seg_off + (m - q * seg_len); }
+        const float* a = acc[r >> 1] + 2 * (r & 1);
+        uint32_t* crow = reinterpret_cast<uint32_t*>(C + orow * p.ldc + oc);
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          crow[4 * j] = pack_bf16x2(geglu_fast(a[4 * (j + 8)], a[4 * j]), geglu_fast(a[4 * (j + 8) + 1], a[4 * j + 1]));
+      }
+    }
   }
   __syncthreads();
 }
@@ -623,6 +682,19 @@ static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const EpiPa
   return 0;
 }
 
+static int launch_gemm_geglu(const CUtensorMap& ta, const CUtensorMap& tb, const EpiParams& p, cudaStream_t st) {
+  static unsigned long long configured_mask = 0;
+  if (!device_configured(&configured_mask)) {
+    PHK_CUDA(cudaFuncSetAttribute(gemm_bf16_geglu_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, GG_SMEM_TOTAL));
+    mark_configured(&configured_mask);
+  }
+  const int tiles = p.m_tiles * p.n_tiles;
+  const int grid = tiles < kNumSMs ? tiles : kNumSMs;
+  PHK_CUDA(launch_pdl(gemm_bf16_geglu_kernel, dim3(grid), dim3(GG_THREADS), (size_t)GG_SMEM_TOTAL, st, ta, tb, p));
+  PHK_LAUNCH_CHECK();
+  return 0;
+}
+
 template <int EPI>
 static int launch_gemm_dual(const CUtensorMap& ta, const CUtensorMap& tb, const EpiParams& p, const CUtensorMap& ta2,
                             const CUtensorMap& tb2, const EpiParams& p2, cudaStream_t st) {
@@ -665,7 +737,7 @@ extern "C" int phk_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t 
   EpiParams p{C, ldc, M, N, K, bias, residual, seg_len, seg_stride, seg_off, (int)((M + GM - 1) / GM), (N + GN - 1) / GN};
   PHK_REQUIRE((int64_t)p.m_tiles * p.n_tiles < (1LL << 31), PHK_E_UNSUPPORTED, "phk_gemm_bf16: too many tiles");
   PHK_TRY(maybe_tma_epilogue(p, epilogue));
-  if (epilogue == 2) return launch_gemm<2>(ta, tb, p, st);
+  if (epilogue == 2) return launch_gemm_geglu(ta, tb, p, st);
   if (epilogue == 1) return launch_gemm<1>(ta, tb, p, st);
   return launch_gemm<0>(ta, tb, p, st);
 }

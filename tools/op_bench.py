@@ -58,7 +58,7 @@ for (M, N, K, epi, name) in [(4608, 512, 512, 0, "gemm q/out-proj (+res)"), (460
     w = torch.randn(N, K, device=dev).to(bf)
     c = torch.zeros(M, N if epi != 2 else N // 2, device=dev, dtype=torch.float32 if epi == 0 else bf)
     res = L.ptr(c) if (epi == 0 and N == 512) else None
-    timeit(name + f" {M}x{N}x{K}", lambda: L.check(lib.phk_gemm_bf16(L.ptr(a), K, L.ptr(w), K, L.ptr(c), c.shape[1], M, N, K, None, res, 0, 0, 0, epi, sp())),
+    timeit(name + f" {M}x{N}x{K} " + ("geglu_kernel" if epi == 2 else f"<{epi}, false>"), lambda: L.check(lib.phk_gemm_bf16(L.ptr(a), K, L.ptr(w), K, L.ptr(c), c.shape[1], M, N, K, None, res, 0, 0, 0, epi, sp())),
            2.0 * M * N * K, "TFLOP/s")
 
 a1 = torch.randn(R, D, device=dev).to(bf); a2 = torch.randn(R, D, device=dev).to(bf)
@@ -66,6 +66,20 @@ w1 = torch.randn(I, D, device=dev).to(bf); w2 = torch.randn(2 * I, D, device=dev
 c1 = torch.zeros(R, I, device=dev); c2 = torch.zeros(R, 2 * I, device=dev)
 timeit("gemm q + kv in one launch (x2)", lambda: L.check(lib.phk_gemm_bf16_x2(L.ptr(a1), D, L.ptr(w1), D, L.ptr(c1), I, R, I, D, None, L.ptr(a2), D, L.ptr(w2), D, L.ptr(c2), 2 * I, R, 2 * I, D, None, sp())),
        2.0 * R * 3 * I * D, "TFLOP/s")
+# the remaining production launches of the encode and the MaskGit forward, each named with the gemm_bf16_kernel<EPI, DUAL>
+# instance it runs
+qs_ = torch.rand(64, device=dev) + 0.5
+qn_o, kvn_o = torch.empty(R, I, dtype=bf, device=dev), torch.empty(R, 2 * I, dtype=bf, device=dev)
+timeit("gemm q + kv fused (qkv) <3, true>", lambda: L.check(lib.phk_gemm_bf16_qkv(L.ptr(a1), L.ptr(a2), D, L.ptr(w1), L.ptr(w2), D, L.ptr(qn_o), L.ptr(kvn_o), R, I, D, L.ptr(qs_), L.ptr(qs_), 8.0, sp())),
+       2.0 * R * 3 * I * D, "TFLOP/s")
+timeit("gemm cross-attention q (qnorm) <3, false>", lambda: L.check(lib.phk_gemm_bf16_qnorm(L.ptr(a1), D, L.ptr(w1), D, L.ptr(qn_o), R, I, D, L.ptr(qs_), 8.0, sp())),
+       2.0 * R * I * D, "TFLOP/s")
+pa1, pw1 = torch.randn(512, 3072, device=dev).to(bf), torch.randn(D, 3072, device=dev).to(bf)
+pa2, pw2 = torch.randn(4096, 6144, device=dev).to(bf), torch.randn(D, 6144, device=dev).to(bf)
+pb1, pb2 = torch.randn(D, device=dev), torch.randn(D, device=dev)
+pc1, pc2 = torch.empty(512, D, device=dev), torch.empty(4096, D, device=dev)
+timeit("gemm patch embeddings 512x512x3072 + 4096x512x6144 (x2) <0, true>", lambda: L.check(lib.phk_gemm_bf16_x2(L.ptr(pa1), 3072, L.ptr(pw1), 3072, L.ptr(pc1), D, 512, D, 3072, L.ptr(pb1), L.ptr(pa2), 6144, L.ptr(pw2), 6144, L.ptr(pc2), D, 4096, D, 6144, L.ptr(pb2), sp())),
+       2.0 * D * (512 * 3072 + 4096 * 6144), "TFLOP/s")
 
 # temporal attention (n=9, causal) on the (b,t,h,w) layout
 q, kv = torch.randn(R, I, device=dev), torch.randn(R, 2 * I, device=dev)
