@@ -2,22 +2,28 @@
 //   C[map(m), n] = sum_k A[m,k] * W[n,k]  (+bias) (+residual)        nn.Linear semantics
 // A, W bf16, K-major (row-major [rows, K]); fp32 accumulation in registers.
 //
-// gemm_bf16_kernel<EPI, DUAL> behind phk_gemm_bf16 / phk_gemm_bf16_x2 / _qkv / _qnorm: one CTA per 128 x 128 tile,
-// DUAL = two independent problems in one persistent launch.  Persistent (one CTA per SM, static round-robin tile
-// scheduler, m-fastest so concurrent CTAs share the W tile in L2 while the A panel stays L2-resident):
+// gemm_bf16_kernel<EPI, DUAL> behind phk_gemm_bf16 / phk_gemm_bf16_x2 / _qkv / _qnorm, DUAL = two independent problems
+// in one launch.  Persistent (one CTA per SM, 128 x 128 tiles, static round-robin tile scheduler, m-fastest so
+// concurrent CTAs share the W tile in L2 while the A panel stays L2-resident).  Two bodies:
+// * quadrant (single-problem instances, 640 threads):
 //   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor.2d (SWIZZLE_128B) stages 128x64 A and W tiles into
 //                   a 4-deep shared-memory ring; out-of-bounds rows / the K tail are zero-filled by the TMA unit.
 //   warpgroups 1..4 each multiplies one 64 x 64 quadrant of the tile (wgmma.m64n64k16, both operands from shared
 //                   memory), writes it into the epilogue's staging layout, and then all sixteen warps run the epilogue
 //                   (four per 32-row group, each a quarter of the columns) while the producer fills the ring for the
 //                   next tile.
+// * ping-pong (two-problem instances and gemm_bf16_geglu_kernel, 384 threads; see gemm_pingpong below): two MMA
+//   warpgroups take whole tiles in turn as m64n128k16 row halves and run the epilogue from the accumulator registers
+//   while the other one runs its main loop.  Measured faster where a CTA gets several tiles, slower where it gets one.
 // Epilogues: 0 fp32 (+bias, +residual, row map) -- through the TMA unit when the row map is the identity: the
 //              residual tile is bulk-loaded into SWIZZLE_128B staging boxes during the main loop and the result tile
-//              bulk-stored from them; otherwise staged in a padded smem tile and written with coalesced rows
+//              bulk-stored from them; otherwise staged in a padded smem tile and written with coalesced rows.  Two
+//              problems: fp32 (+bias) from the registers.
 //            1 bf16 (+bias)
 //            2 GEGLU (attention.py:40-43) on W rows packed [64 value rows | 64 gate rows] per 128-column tile ->
-//              bf16 [M, N/2], fitted sigmoid-form GELU: gemm_bf16_geglu_kernel below (ping-pong, m64n128k16, the GEGLU
-//              from the accumulator registers), measured faster on these many-tile products.
+//              bf16 [M, N/2], fitted sigmoid-form GELU: gemm_bf16_geglu_kernel (ping-pong)
+//            3 q / k,v attention operands (per-head l2 normalisation, bf16): staged (one problem) or from the registers
+//              (two problems), rounded alike.
 #include "phk_common.cuh"
 #include "phk_sm90.cuh"
 #include <mutex>
@@ -94,6 +100,16 @@ __device__ __forceinline__ float geglu_fast(float g, float v) {
   const float h = 0.5f * (g * v);
   return fmaf(h, t, h);
 }
+
+// Per-head l2 normalisation of epilogue 3, shared by the staged and the register epilogue so that both round alike: the
+// squared norm of four consecutive columns c0..c3 of a head is fma(c3, c3, fma(c2, c2, fma(c0, c0, c1 * c1))), the
+// head's 16 such partials are summed as an xor-butterfly over 8, 4, 2, 1, and each column becomes (c * inv) * scale.
+__device__ __forceinline__ float head_sumsq_first(float c0, float c1) { return __fmaf_rn(c0, c0, __fmul_rn(c1, c1)); }
+__device__ __forceinline__ float head_sumsq_next(float c2, float c3, float s) {
+  return __fmaf_rn(c3, c3, __fmaf_rn(c2, c2, s));
+}
+__device__ __forceinline__ float head_inv_norm(float ss) { return 1.0f / fmaxf(sqrtf(ss), 1e-12f); }
+__device__ __forceinline__ float head_scale(float c, float inv, float sc) { return __fmul_rn(__fmul_rn(c, inv), sc); }
 
 // ---------------------------------------------------------------------------------------------------
 // Epilogue pieces.  A "chunk" is the tile's 128 rows x 128 accumulator columns, staged in shared memory by
@@ -279,11 +295,12 @@ __device__ __forceinline__ void epi_chunk(const EpiParams& p, float* cstage, int
       const uint32_t m = (uint32_t)m0 + r;
       float4 o = *reinterpret_cast<const float4*>(cstage + r * CPAD + lane * 4);
       if (norm) {
-        float ss = o.x * o.x + o.y * o.y + o.z * o.z + o.w * o.w;
+        float ss = head_sumsq_next(o.z, o.w, head_sumsq_first(o.x, o.y));
 #pragma unroll
         for (int d = 8; d > 0; d >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, d);
-        const float inv = 1.0f / fmaxf(sqrtf(ss), 1e-12f);
-        o.x = (o.x * inv) * sc.x; o.y = (o.y * inv) * sc.y; o.z = (o.z * inv) * sc.z; o.w = (o.w * inv) * sc.w;
+        const float inv = head_inv_norm(ss);
+        o.x = head_scale(o.x, inv, sc.x); o.y = head_scale(o.y, inv, sc.y);
+        o.z = head_scale(o.z, inv, sc.z); o.w = head_scale(o.w, inv, sc.w);
       }
       if (m < (uint32_t)p.M && col < nlim)
         *reinterpret_cast<uint2*>(reinterpret_cast<__nv_bfloat16*>(p.C) + (int64_t)m * p.ldc + col) =
@@ -321,19 +338,10 @@ __device__ __forceinline__ void epi_chunk(const EpiParams& p, float* cstage, int
 }
 
 // ---------------------------------------------------------------------------------------------------
-// The kernel: 128 x 128 tiles, four MMA / epilogue warpgroups of one 64 x 64 quadrant each
+// Quadrant body (single-problem instances): 128 x 128 tiles, four MMA / epilogue warpgroups of one 64 x 64 quadrant each
 // ---------------------------------------------------------------------------------------------------
-// DUAL: two independent problems (own operands, output, N and K) in ONE launch -- the q and k,v projections of a
-// self-attention block, which read different inputs (LayerNorm(x) vs raw x, attention.py:140-144) and are each a
-// single wave of tiles: together they make ~3 tiles per CTA, so prologue, epilogue and main loop overlap across tiles
-// instead of being paid twice.
-template <int EPI, bool DUAL>
-__global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                const __grid_constant__ CUtensorMap tmB,
-                                                                const __grid_constant__ EpiParams p,
-                                                                const __grid_constant__ CUtensorMap tmA2,
-                                                                const __grid_constant__ CUtensorMap tmB2,
-                                                                const __grid_constant__ EpiParams p2) {
+template <int EPI>
+__device__ __forceinline__ void gemm_quadrant(const CUtensorMap& tmA, const CUtensorMap& tmB, const EpiParams& p) {
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B atoms need 1024-B alignment
@@ -344,10 +352,138 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
   // full[s] @ +8s ; empty[s] @ +8(S+s) ; residual landed @ +16S
   const uint32_t bar_res = bars + 16 * GSTAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int num_tiles = p.m_tiles * p.n_tiles;
+  // tile schedule: round-robin, m-fastest
+  const int my_tiles = (int)blockIdx.x < num_tiles ? (num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  auto tile_of = [&](int i, int& m0, int& n0) {
+    const int tile = (int)blockIdx.x + i * (int)gridDim.x;
+    m0 = (tile % p.m_tiles) * GM;
+    n0 = (tile / p.m_tiles) * GN;
+  };
+  const int num_kb = (p.K + GK - 1) / GK;
+
+  if (threadIdx.x == 0) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
+    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+    for (int s = 0; s < GSTAGES; ++s) {
+      mbar_init(bars + 8 * s, 1);
+      mbar_init(bars + 8 * (GSTAGES + s), EPI_WARPS);  // one arrival per MMA warp
+    }
+    mbar_init(bar_res, 1);                               // residual tile landed (TMA epilogue)
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  pdl_wait();  // everything above (barriers, tensor-map prefetch) overlapped the previous kernel
+
+  if (warp < 4) {
+    // ===================== TMA producer =====================
+    if (warp == 0 && lane == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int it = 0; it < my_tiles; ++it) {
+        int m0, n0;
+        tile_of(it, m0, n0);
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(bars + 8 * (GSTAGES + stage), phase ^ 1);  // slot free (passes immediately on the first lap)
+          const uint32_t full = bars + 8 * stage;
+          mbar_expect_tx(full, 2 * STAGE_BYTES);
+          tma_load_2d(&tmA, full, sA + stage * STAGE_BYTES, kb * GK, m0);
+          tma_load_2d(&tmB, full, sB + stage * STAGE_BYTES, kb * GK, n0);
+          if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
+        }
+      }
+    }
+  } else {
+    // ===================== MMA + epilogue: warps 4..19 =====================
+    const int ew = warp - 4;        // 0..15: rows ew, ew+16, ... in the coalesced write-out
+    const int lg = warp & 3;        // 32-row group whose rows this warp drains (one row per lane)
+    const int part = ew >> 2;       // which quarter of the tile's columns this warp drains
+    const int wg = ew >> 2;         // MMA warpgroup: quadrant rows 64 (wg & 1).., columns 64 (wg >> 1)..
+    const int rq = (wg & 1) * 64, cq = (wg >> 1) * 64;
+    uint32_t res_phase = 0;
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int it = 0; it < my_tiles; ++it) {
+      int m0, n0;
+      tile_of(it, m0, n0);
+      const bool tma = EPI == 0 && p.tma_epi;
+      bool res_vec = false;
+      if (tma) epi_tma_begin(p, base + RING_BYTES, bar_res, m0, n0, ew, lane);
+      else if (EPI == 0) res_vec = epi_residual_prefetch<EPI>(p, cstage, m0, n0, ew, lane);
+      else epi_bar_sync();  // the previous tile's epilogue has left the staging memory
+      // ---- main loop: this warpgroup's 64 x 64 quadrant ----
+      float d[32];
+#pragma unroll
+      for (int i = 0; i < 32; ++i) d[i] = 0.f;
+      for (int kb = 0; kb < num_kb; ++kb) {
+        mbar_wait(bars + 8 * stage, phase);
+        const uint64_t da = gmma_desc(sA + stage * STAGE_BYTES + rq * 128);
+        const uint64_t db = gmma_desc(sB + stage * STAGE_BYTES + cq * 128);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < GK / 16; ++k)  // +32 B per K = 16 inside the 128-B swizzle row => +2 in the address field
+          wgmma_m64n64k16_ss<0>(d, da + 2 * k, db + 2 * k, 1u);
+        wgmma_commit();
+        wgmma_wait<0>();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bars + 8 * (GSTAGES + stage));  // this warp's reads of the slot are complete
+        if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
+      }
+      // ---- accumulator -> staging (onto the residual where one was staged) ----
+      if (tma) {
+        if (p.residual) { mbar_wait(bar_res, res_phase); res_phase ^= 1; }
+        acc_to_stage<true>(d, reinterpret_cast<uint8_t*>(cstage), rq, cq, ew & 3, lane, p.residual != nullptr);
+      } else {
+        acc_to_stage<false>(d, reinterpret_cast<uint8_t*>(cstage), rq, cq, ew & 3, lane, res_vec);
+      }
+      epi_bar_sync();  // whole tile staged
+      if (tma)
+        epi_tma_finish(p, reinterpret_cast<uint8_t*>(cstage), base + RING_BYTES, m0, n0, ew, lg, part, lane);
+      else
+        epi_chunk<EPI>(p, cstage, m0, n0, res_vec, ew, lane);
+    }
+    if (EPI == 0 && ew == 0 && lane == 0) tma_store_wait_read();  // staging read out before the CTA exits (the writes complete with the grid)
+  }
+  __syncthreads();
+}
+
+// ---------------------------------------------------------------------------------------------------
+// Ping-pong body: the GEGLU products (FF1 of every feed-forward block, 22 column tiles) and the two-problem launches
+// (q + k,v projections, patch embeddings) -- the products where a CTA gets several tiles
+// ---------------------------------------------------------------------------------------------------
+// Warpgroup 0 is the TMA producer (one thread; the warpgroup gives its registers away to the MMA warpgroups) feeding a
+// GG_STAGES-deep ring in the order the CTA's tiles are consumed.  Warpgroups 1 and 2 take the CTA's tiles in turn: each
+// multiplies a whole 128 x 128 tile as two m64n128k16 row halves that share every W slice (6 KB of operands per 64
+// tensor-core clocks instead of 4 KB per 32 for a 64 x 64 quadrant), keeps one k-block of MMAs in flight, and runs the
+// epilogue straight from its accumulator registers while the other warpgroup runs the next tile's main loop.  A
+// named-barrier handshake orders the main loops, so the two warpgroups never interleave their MMAs.  Per output element
+// the k-order (k-blocks of 64 in order, k = 16 steps in order) is that of the quadrant body.
+// DUAL: two independent problems (own operands, output, N and K) in ONE launch, tiles of problem 1 first.  The q and
+// k,v projections of a self-attention block read different inputs (LayerNorm(x) vs raw x, attention.py:140-144) and
+// are each a single wave of tiles; together they make 3-4 tiles per CTA.
+constexpr int GG_STAGES = 6;
+constexpr int GG_THREADS = 384;
+constexpr int GG_PRODUCER_REGS = 40, GG_CONSUMER_REGS = 232;  // 128 x 40 + 256 x 232 <= 64 K registers
+constexpr int GG_SMEM_TOTAL = GG_STAGES * 2 * STAGE_BYTES + 128 /*barriers*/ + 1024 /*manual 1024-B alignment*/;
+constexpr int GG_BAR_TURN = 1;  // named barriers 1, 2: main-loop turn of MMA warpgroup 0, 1
+
+// The accumulator of a ping-pong tile: acc[h][4j + 2i + e] = (row 64h + 16w + lane/4 + 8i, column 8j + 2(lane%4) + e).
+typedef float PingPongAcc[2][64];
+
+template <bool DUAL, class Epilogue>
+__device__ __forceinline__ void gemm_pingpong(const CUtensorMap& tmA, const CUtensorMap& tmB, const EpiParams& p,
+                                              const CUtensorMap& tmA2, const CUtensorMap& tmB2, const EpiParams& p2,
+                                              const Epilogue& epilogue) {
+  pdl_trigger();
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B atoms need 1024-B alignment
+  const uint32_t sA = base, sB = base + GG_STAGES * STAGE_BYTES;
+  const uint32_t bars = base + GG_STAGES * 2 * STAGE_BYTES;  // full[s] @ +8s ; empty[s] @ +8(S+s)
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles1 = p.m_tiles * p.n_tiles;
   const int num_tiles = tiles1 + (DUAL ? p2.m_tiles * p2.n_tiles : 0);
-  // tile schedule: round-robin over all tiles (problem 1 first), m-fastest; returns true for a tile of problem 2
   const int my_tiles = (int)blockIdx.x < num_tiles ? (num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+  // round-robin over all tiles (problem 1 first), m-fastest; returns true for a tile of problem 2
   auto tile_of = [&](int i, int& m0, int& n0) -> bool {
     int tile = (int)blockIdx.x + i * (int)gridDim.x;
     const bool second = DUAL && tile >= tiles1;
@@ -366,131 +502,6 @@ __global__ void __launch_bounds__(GTHREADS, 1) gemm_bf16_kernel(const __grid_con
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA2) : "memory");
       asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB2) : "memory");
     }
-    for (int s = 0; s < GSTAGES; ++s) {
-      mbar_init(bars + 8 * s, 1);
-      mbar_init(bars + 8 * (GSTAGES + s), EPI_WARPS);  // one arrival per MMA warp
-    }
-    mbar_init(bar_res, 1);                               // residual tile landed (TMA epilogue)
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  __syncthreads();
-  pdl_wait();  // everything above (barriers, tensor-map prefetch) overlapped the previous kernel
-
-  if (warp < 4) {
-    // ===================== TMA producer =====================
-    if (warp == 0 && lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int it = 0; it < my_tiles; ++it) {
-        int m0, n0;
-        const bool second = tile_of(it, m0, n0);
-        const int num_kb = kblocks(second);
-        const CUtensorMap* ma = second ? &tmA2 : &tmA;
-        const CUtensorMap* mb = second ? &tmB2 : &tmB;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(bars + 8 * (GSTAGES + stage), phase ^ 1);  // slot free (passes immediately on the first lap)
-          const uint32_t full = bars + 8 * stage;
-          mbar_expect_tx(full, 2 * STAGE_BYTES);
-          tma_load_2d(ma, full, sA + stage * STAGE_BYTES, kb * GK, m0);
-          tma_load_2d(mb, full, sB + stage * STAGE_BYTES, kb * GK, n0);
-          if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else {
-    // ===================== MMA + epilogue: warps 4..19 =====================
-    const int ew = warp - 4;        // 0..15: rows ew, ew+16, ... in the coalesced write-out
-    const int lg = warp & 3;        // 32-row group whose rows this warp drains (one row per lane)
-    const int part = ew >> 2;       // which quarter of the tile's columns this warp drains
-    const int wg = ew >> 2;         // MMA warpgroup: quadrant rows 64 (wg & 1).., columns 64 (wg >> 1)..
-    const int rq = (wg & 1) * 64, cq = (wg >> 1) * 64;
-    uint32_t res_phase = 0;
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int it = 0; it < my_tiles; ++it) {
-      int m0, n0;
-      const bool second = tile_of(it, m0, n0);
-      const EpiParams& pp = second ? p2 : p;
-      const bool tma = EPI == 0 && pp.tma_epi;
-      bool res_vec = false;
-      if (tma) epi_tma_begin(pp, base + RING_BYTES, bar_res, m0, n0, ew, lane);
-      else if (EPI == 0) res_vec = epi_residual_prefetch<EPI>(pp, cstage, m0, n0, ew, lane);
-      else epi_bar_sync();  // the previous tile's epilogue has left the staging memory
-      // ---- main loop: this warpgroup's 64 x 64 quadrant ----
-      float d[32];
-#pragma unroll
-      for (int i = 0; i < 32; ++i) d[i] = 0.f;
-      const int num_kb = kblocks(second);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(bars + 8 * stage, phase);
-        const uint64_t da = gmma_desc(sA + stage * STAGE_BYTES + rq * 128);
-        const uint64_t db = gmma_desc(sB + stage * STAGE_BYTES + cq * 128);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < GK / 16; ++k)  // +32 B per K = 16 inside the 128-B swizzle row => +2 in the address field
-          wgmma_m64n64k16_ss<0>(d, da + 2 * k, db + 2 * k, 1u);
-        wgmma_commit();
-        wgmma_wait<0>();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bars + 8 * (GSTAGES + stage));  // this warp's reads of the slot are complete
-        if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
-      }
-      // ---- accumulator -> staging (onto the residual where one was staged) ----
-      if (tma) {
-        if (pp.residual) { mbar_wait(bar_res, res_phase); res_phase ^= 1; }
-        acc_to_stage<true>(d, reinterpret_cast<uint8_t*>(cstage), rq, cq, ew & 3, lane, pp.residual != nullptr);
-      } else {
-        acc_to_stage<false>(d, reinterpret_cast<uint8_t*>(cstage), rq, cq, ew & 3, lane, res_vec);
-      }
-      epi_bar_sync();  // whole tile staged
-      if (tma)
-        epi_tma_finish(pp, reinterpret_cast<uint8_t*>(cstage), base + RING_BYTES, m0, n0, ew, lg, part, lane);
-      else
-        epi_chunk<EPI>(pp, cstage, m0, n0, res_vec, ew, lane);
-    }
-    if (EPI == 0 && ew == 0 && lane == 0) tma_store_wait_read();  // staging read out before the CTA exits (the writes complete with the grid)
-  }
-  __syncthreads();
-}
-
-// ---------------------------------------------------------------------------------------------------
-// GEGLU products (epilogue 2: FF1 of every feed-forward block, 22 column tiles, several tiles per CTA): ping-pong
-// ---------------------------------------------------------------------------------------------------
-// Warpgroup 0 is the TMA producer (one thread; the warpgroup gives its registers away to the MMA warpgroups) feeding a
-// GG_STAGES-deep ring in the order the CTA's tiles are consumed.  Warpgroups 1 and 2 take the CTA's tiles in turn: each
-// multiplies a whole 128 x 128 tile as two m64n128k16 row halves that share every W slice (6 KB of operands per 64
-// tensor-core clocks instead of 4 KB per 32 for a 64 x 64 quadrant), keeps one k-block of MMAs in flight, and runs the
-// GEGLU straight from its accumulator registers while the other warpgroup runs the next tile's main loop: value column
-// c and gate column c + 64 of a row are held by the same lane, so no staging is needed.  A named-barrier handshake
-// orders the main loops, so the two warpgroups never interleave their MMAs.  Per output element the k-order (k-blocks
-// of 64 in order, k = 16 steps in order) is that of the quadrant kernel.
-constexpr int GG_STAGES = 6;
-constexpr int GG_THREADS = 384;
-constexpr int GG_PRODUCER_REGS = 40, GG_CONSUMER_REGS = 232;  // 128 x 40 + 256 x 232 <= 64 K registers
-constexpr int GG_SMEM_TOTAL = GG_STAGES * 2 * STAGE_BYTES + 128 /*barriers*/ + 1024 /*manual 1024-B alignment*/;
-constexpr int GG_BAR_TURN = 1;  // named barriers 1, 2: main-loop turn of MMA warpgroup 0, 1
-
-__global__ void __launch_bounds__(GG_THREADS, 1) gemm_bf16_geglu_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                                        const __grid_constant__ CUtensorMap tmB,
-                                                                        const __grid_constant__ EpiParams p) {
-  pdl_trigger();
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B atoms need 1024-B alignment
-  const uint32_t sA = base, sB = base + GG_STAGES * STAGE_BYTES;
-  const uint32_t bars = base + GG_STAGES * 2 * STAGE_BYTES;  // full[s] @ +8s ; empty[s] @ +8(S+s)
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int num_tiles = p.m_tiles * p.n_tiles;
-  const int my_tiles = (int)blockIdx.x < num_tiles ? (num_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
-  const int num_kb = (p.K + GK - 1) / GK;
-  auto tile_of = [&](int i, int& m0, int& n0) {  // round-robin, m-fastest
-    const int tile = (int)blockIdx.x + i * (int)gridDim.x;
-    m0 = (tile % p.m_tiles) * GM;
-    n0 = (tile / p.m_tiles) * GN;
-  };
-
-  if (threadIdx.x == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     for (int s = 0; s < GG_STAGES; ++s) {
       mbar_init(bars + 8 * s, 1);
       mbar_init(bars + 8 * (GG_STAGES + s), 4);  // one arrival per warp of the consuming MMA warpgroup
@@ -508,35 +519,38 @@ __global__ void __launch_bounds__(GG_THREADS, 1) gemm_bf16_geglu_kernel(const __
       uint32_t phase = 0;
       for (int it = 0; it < my_tiles; ++it) {
         int m0, n0;
-        tile_of(it, m0, n0);
+        const bool second = tile_of(it, m0, n0);
+        const int num_kb = kblocks(second);
+        const CUtensorMap* ma = second ? &tmA2 : &tmA;
+        const CUtensorMap* mb = second ? &tmB2 : &tmB;
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(bars + 8 * (GG_STAGES + stage), phase ^ 1);  // slot free (passes immediately on the first lap)
           const uint32_t full = bars + 8 * stage;
           mbar_expect_tx(full, 2 * STAGE_BYTES);
-          tma_load_2d(&tmA, full, sA + stage * STAGE_BYTES, kb * GK, m0);
-          tma_load_2d(&tmB, full, sB + stage * STAGE_BYTES, kb * GK, n0);
+          tma_load_2d(ma, full, sA + stage * STAGE_BYTES, kb * GK, m0);
+          tma_load_2d(mb, full, sB + stage * STAGE_BYTES, kb * GK, n0);
           if (++stage == GG_STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
   } else {
-    // ===================== MMA + GEGLU: warpgroup wg takes the CTA's tiles wg, wg + 2, ... =====================
+    // ===================== MMA + epilogue: warpgroup wg takes the CTA's tiles wg, wg + 2, ... =====================
     setmaxnreg_inc<GG_CONSUMER_REGS>();
     const int wg = (warp >> 2) - 1;
     const int w = warp & 3;
     int stage = 0;
     uint32_t phase = 0;
     for (int it = 0; it < my_tiles; ++it) {
+      int m0, n0;
+      const bool second = tile_of(it, m0, n0);
+      const int num_kb = kblocks(second);
       if ((it & 1) != wg) {  // the other warpgroup's tile: skip its k-blocks in the ring
         stage += num_kb;
         while (stage >= GG_STAGES) { stage -= GG_STAGES; phase ^= 1; }
         continue;
       }
-      int m0, n0;
-      tile_of(it, m0, n0);
       if (it > 0) named_bar_sync(GG_BAR_TURN + wg, 256);  // the other warpgroup has issued tile it - 1
-      // acc[h][4j + 2i + e] = (row 64h + 16w + lane/4 + 8i, column 8j + 2(lane%4) + e) of the tile
-      float acc[2][64];
+      PingPongAcc acc;
       int prev = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(bars + 8 * stage, phase);
@@ -563,26 +577,149 @@ __global__ void __launch_bounds__(GG_THREADS, 1) gemm_bf16_geglu_kernel(const __
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(bars + 8 * (GG_STAGES + prev));
-      // GEGLU of the [64 value | 64 gate] tile -> bf16 columns n0/2 + 8j + 2(lane%4) + e, j < 8 (N % 128 == 0, even ldc
-      // and 4-byte aligned C: checked on the host)
-      __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C);
-      const int oc = n0 / 2 + 2 * (lane & 3);
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        const uint32_t m = (uint32_t)m0 + 64 * (r >> 1) + 16 * w + (lane >> 2) + 8 * (r & 1);
-        if (m >= (uint32_t)p.M) continue;
-        int64_t orow = m;
-        const uint32_t seg_len = (uint32_t)p.seg_len;
-        if (seg_len > 0) { const uint32_t q = m / seg_len; orow = q * (uint32_t)p.seg_stride + (uint32_t)p.seg_off + (m - q * seg_len); }
-        const float* a = acc[r >> 1] + 2 * (r & 1);
-        uint32_t* crow = reinterpret_cast<uint32_t*>(C + orow * p.ldc + oc);
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          crow[4 * j] = pack_bf16x2(geglu_fast(a[4 * (j + 8)], a[4 * j]), geglu_fast(a[4 * (j + 8) + 1], a[4 * j + 1]));
-      }
+      epilogue(second ? p2 : p, acc, m0, n0, w, lane);
     }
   }
   __syncthreads();
+}
+
+// GEGLU of the [64 value | 64 gate] tile -> bf16 columns n0/2 + 8j + 2(lane%4) + e, j < 8: value column c and gate
+// column c + 64 of a row are held by the same lane (N % 128 == 0, even ldc and 4-byte aligned C: checked on the host)
+struct GegluEpilogue {
+  __device__ __forceinline__ void operator()(const EpiParams& p, const PingPongAcc& acc, int m0, int n0, int w,
+                                             int lane) const {
+    __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C);
+    const int oc = n0 / 2 + 2 * (lane & 3);
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const uint32_t m = (uint32_t)m0 + 64 * (r >> 1) + 16 * w + (lane >> 2) + 8 * (r & 1);
+      if (m >= (uint32_t)p.M) continue;
+      int64_t orow = m;
+      const uint32_t seg_len = (uint32_t)p.seg_len;
+      if (seg_len > 0) { const uint32_t q = m / seg_len; orow = q * (uint32_t)p.seg_stride + (uint32_t)p.seg_off + (m - q * seg_len); }
+      const float* a = acc[r >> 1] + 2 * (r & 1);
+      uint32_t* crow = reinterpret_cast<uint32_t*>(C + orow * p.ldc + oc);
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+        crow[4 * j] = pack_bf16x2(geglu_fast(a[4 * (j + 8)], a[4 * j]), geglu_fast(a[4 * (j + 8) + 1], a[4 * j + 1]));
+    }
+  }
+};
+
+// Epilogue 3 from the accumulator: bit-identical to epi_chunk<3>.  There lane L of a half-warp owns head-local columns
+// 4L..4L+3; here lane quad position t holds columns 8jj + 2t + {0, 1} of a head (jj < 8), so the four columns of L sit
+// in quad lanes t = 2(L & 1) (first two) and t + 1 (last two) at jj = L >> 1.  The first lane's partial goes to the
+// second, which adds its two squares: the odd quad lanes then hold the staged path's 4-column partials.  Its xor-butterfly
+// over L ^ 8, L ^ 4, L ^ 2 pairs registers jj ^ 4, jj ^ 2, jj ^ 1 of one lane, and L ^ 1 pairs quad lanes 1 and 3; float
+// addition is commutative, so every level rounds as there.  Columns >= norm_cols (the value half of k,v) are only
+// converted.  bf16 output, no bias, identity row map, N % 128 == 0 and 8-byte aligned C (checked on the host).
+struct QkNormEpilogue {
+  __device__ __forceinline__ void operator()(const EpiParams& p, const PingPongAcc& acc, int m0, int n0, int w,
+                                             int lane) const {
+    const int t = lane & 3;
+    const bool norm = n0 < p.norm_cols;  // tiles are 128-aligned and norm_cols % 128 == 0
+    float2 sc[8];
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) sc[jj] = make_float2(1.f, 1.f);
+    if (norm) {
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        const float2 s = __ldg(reinterpret_cast<const float2*>(p.nscale + 8 * jj + 2 * t));
+        sc[jj] = make_float2(s.x * p.nmul, s.y * p.nmul);
+      }
+    }
+    __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C);
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const uint32_t m = (uint32_t)m0 + 64 * (r >> 1) + 16 * w + (lane >> 2) + 8 * (r & 1);
+      const float* a = acc[r >> 1] + 2 * (r & 1);
+      uint32_t* crow = reinterpret_cast<uint32_t*>(C + (int64_t)m * p.ldc + n0 + 2 * t);
+#pragma unroll
+      for (int hd = 0; hd < 2; ++hd) {
+        float inv = 1.f;
+        if (norm) {  // tile-uniform: every lane of the warp takes part in the shuffles, whatever its row
+          float s[8];
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            const float c0 = a[4 * (8 * hd + jj)], c1 = a[4 * (8 * hd + jj) + 1];
+            const float first = __shfl_xor_sync(0xffffffffu, head_sumsq_first(c0, c1), 1);
+            s[jj] = head_sumsq_next(c0, c1, first);
+          }
+          float ss = ((s[0] + s[4]) + (s[2] + s[6])) + ((s[1] + s[5]) + (s[3] + s[7]));
+          ss += __shfl_xor_sync(0xffffffffu, ss, 2);
+          ss = __shfl_sync(0xffffffffu, ss, lane | 1);
+          inv = head_inv_norm(ss);
+        }
+        if (m < (uint32_t)p.M) {
+#pragma unroll
+          for (int jj = 0; jj < 8; ++jj) {
+            float x = a[4 * (8 * hd + jj)], y = a[4 * (8 * hd + jj) + 1];
+            if (norm) { x = head_scale(x, inv, sc[jj].x); y = head_scale(y, inv, sc[jj].y); }
+            crow[4 * (8 * hd + jj)] = pack_bf16x2(x, y);
+          }
+        }
+      }
+    }
+  }
+};
+
+// Epilogue 0 of the two-problem launch from the accumulator: fp32 acc + bias (one add, as epi_chunk<0>), no residual,
+// identity row map; float2 stores, scalar ones for ragged N or a C that is not 8-byte aligned.
+struct Fp32BiasEpilogue {
+  __device__ __forceinline__ void operator()(const EpiParams& p, const PingPongAcc& acc, int m0, int n0, int w,
+                                             int lane) const {
+    const int c0 = n0 + 2 * (lane & 3);
+    float2 bv[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int c = c0 + 8 * j;
+      bv[j].x = (p.bias && c < p.N) ? __ldg(p.bias + c) : 0.f;
+      bv[j].y = (p.bias && c + 1 < p.N) ? __ldg(p.bias + c + 1) : 0.f;
+    }
+    const bool vec = (p.ldc % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+#pragma unroll
+    for (int r = 0; r < 4; ++r) {
+      const uint32_t m = (uint32_t)m0 + 64 * (r >> 1) + 16 * w + (lane >> 2) + 8 * (r & 1);
+      if (m >= (uint32_t)p.M) continue;
+      const float* a = acc[r >> 1] + 2 * (r & 1);
+      float* crow = reinterpret_cast<float*>(p.C) + (int64_t)m * p.ldc + c0;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const float2 o = make_float2(a[4 * j] + bv[j].x, a[4 * j + 1] + bv[j].y);
+        const int c = c0 + 8 * j;
+        if (vec && c + 1 < p.N) {
+          *reinterpret_cast<float2*>(crow + 8 * j) = o;
+        } else {
+          if (c < p.N) crow[8 * j] = o.x;
+          if (c + 1 < p.N) crow[8 * j + 1] = o.y;
+        }
+      }
+    }
+  }
+};
+
+__global__ void __launch_bounds__(GG_THREADS, 1) gemm_bf16_geglu_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                        const __grid_constant__ CUtensorMap tmB,
+                                                                        const __grid_constant__ EpiParams p) {
+  gemm_pingpong<false>(tmA, tmB, p, tmA, tmB, p, GegluEpilogue{});
+}
+
+// ---------------------------------------------------------------------------------------------------
+// gemm_bf16_kernel<EPI, DUAL>: single-problem instances run the quadrant body, two-problem ones (epilogues 0 and 3) the
+// ping-pong body
+// ---------------------------------------------------------------------------------------------------
+template <int EPI, bool DUAL>
+__global__ void __launch_bounds__(DUAL ? GG_THREADS : GTHREADS, 1) gemm_bf16_kernel(
+    const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ EpiParams p,
+    const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
+    const __grid_constant__ EpiParams p2) {
+  if constexpr (DUAL) {
+    static_assert(EPI == 0 || EPI == 3, "two-problem launches have the fp32 (+bias) or the q/k,v epilogue");
+    if constexpr (EPI == 3) gemm_pingpong<true>(tmA, tmB, p, tmA2, tmB2, p2, QkNormEpilogue{});
+    else gemm_pingpong<true>(tmA, tmB, p, tmA2, tmB2, p2, Fp32BiasEpilogue{});
+  } else {
+    gemm_quadrant<EPI>(tmA, tmB, p);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -701,12 +838,12 @@ static int launch_gemm_dual(const CUtensorMap& ta, const CUtensorMap& tb, const 
   static unsigned long long configured_mask = 0;
   const bool configured = device_configured(&configured_mask);
   if (!configured) {
-    PHK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<EPI, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
+    PHK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<EPI, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, GG_SMEM_TOTAL));
     mark_configured(&configured_mask);
   }
   const int tiles = p.m_tiles * p.n_tiles + p2.m_tiles * p2.n_tiles;
   const int grid = tiles < kNumSMs ? tiles : kNumSMs;
-  PHK_CUDA(launch_pdl(gemm_bf16_kernel<EPI, true>, dim3(grid), dim3(GTHREADS), (size_t)(SMEM_TOTAL), st, ta, tb, p, ta2, tb2, p2));
+  PHK_CUDA(launch_pdl(gemm_bf16_kernel<EPI, true>, dim3(grid), dim3(GG_THREADS), (size_t)GG_SMEM_TOTAL, st, ta, tb, p, ta2, tb2, p2));
   PHK_LAUNCH_CHECK();
   return 0;
 }
@@ -767,7 +904,7 @@ extern "C" int phk_gemm_bf16_x2(const void* A1, int64_t lda1, const void* W1, in
   EpiParams p2{C2, ldc2, M2, N2, K2, bias2, nullptr, 0, 0, 0, (int)((M2 + GM - 1) / GM), (N2 + GN - 1) / GN};
   PHK_REQUIRE((int64_t)p.m_tiles * p.n_tiles + (int64_t)p2.m_tiles * p2.n_tiles < (1LL << 31), PHK_E_UNSUPPORTED,
               "phk_gemm_bf16_x2: too many tiles");
-  // (measured: the bulk-store epilogue does not pay for the two-problem launch -- 16.2 vs 15.5 us -- so it stays off)
+  // (the two-problem launch stores from the accumulator registers: no TMA epilogue)
   return launch_gemm_dual<0>(ta, tb, p, ta2, tb2, p2, to_stream(s));
 }
 

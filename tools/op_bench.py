@@ -72,6 +72,11 @@ qs_ = torch.rand(64, device=dev) + 0.5
 qn_o, kvn_o = torch.empty(R, I, dtype=bf, device=dev), torch.empty(R, 2 * I, dtype=bf, device=dev)
 timeit("gemm q + kv fused (qkv) <3, true>", lambda: L.check(lib.phk_gemm_bf16_qkv(L.ptr(a1), L.ptr(a2), D, L.ptr(w1), L.ptr(w2), D, L.ptr(qn_o), L.ptr(kvn_o), R, I, D, L.ptr(qs_), L.ptr(qs_), 8.0, sp())),
        2.0 * R * 3 * I * D, "TFLOP/s")
+# the same launch at the other row counts the benchmarks run: 2304 (first MaskGit layer of a CFG pair), 1152 and 384
+# (the decode and prime-frame encodes of make_video, one tile per CTA)
+for rows in (2304, 1152, 384):
+    timeit(f"gemm q + kv fused (qkv) <3, true>, {rows} rows", lambda: L.check(lib.phk_gemm_bf16_qkv(L.ptr(a1), L.ptr(a2), D, L.ptr(w1), L.ptr(w2), D, L.ptr(qn_o), L.ptr(kvn_o), rows, I, D, L.ptr(qs_), L.ptr(qs_), 8.0, sp())),
+           2.0 * rows * 3 * I * D, "TFLOP/s")
 timeit("gemm cross-attention q (qnorm) <3, false>", lambda: L.check(lib.phk_gemm_bf16_qnorm(L.ptr(a1), D, L.ptr(w1), D, L.ptr(qn_o), R, I, D, L.ptr(qs_), 8.0, sp())),
        2.0 * R * I * D, "TFLOP/s")
 pa1, pw1 = torch.randn(512, 3072, device=dev).to(bf), torch.randn(D, 3072, device=dev).to(bf)
