@@ -605,6 +605,38 @@ int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_t* grads, c
  * transformer layer depth-1-k, events[depth + 1] embeddings + position-bias MLP (= all).  One-shot; NULL clears. */
 int phk_train_set_progress_events(void** events, int32_t count);
 
+/* Backward of a MaskGit / TokenCritic / SelfCritic forward from a gradient the caller supplies: what
+ * `out = module(ids, ...); out.backward(upstream)` computes for the parameters (and the text embeddings) under torch
+ * autograd, where `out` is MaskGit.forward (:163-213; logits, or the embeddings with return_embeds), TokenCritic.forward
+ * (:265-302), SelfCritic.forward (:320-336) or their forward_with_cond_scale (:149-161, 251-263).  The forward is
+ * recomputed with saved activations (activation checkpointing): one call costs a training forward plus the backward
+ * of phk_maskgit_train_step, with the same precision semantics (prec as there; PHK_PREC_BF16X3 is not accepted).
+ *   head_kind PHK_HEAD_LOGITS  upstream = d out / d logits, fp32 [b*n, num_tokens]; head_w / head_b = to_logits
+ *             PHK_HEAD_EMBEDS  upstream = d out / d embeddings (after norm_out), fp32 [b*n, dim]; no head gradient
+ *             PHK_HEAD_SCORE   upstream = d out / d score, fp32 [b*n]; head_w [1, dim] / head_b [1] = the TokenCritic's
+ *                              to_logits, or SelfCritic.to_pred swapped into a MaskGit table
+ *   ids (b,n) int64, patch shape, context (b,L,dim_context) fp32 raw text embeddings or NULL, text_mask (b,L) uint8 (after
+ *   any cond_drop_prob draw), video_mask (b,n) uint8 or NULL: the arguments of the forward being differentiated.
+ *   cfg_pair != 0: the forward was the classifier-free-guidance pair of phk_maskgit_forward(cfg_pair = 1) combined as
+ *   null + cond_scale * (cond - null) (the second half sees an all-false text mask, attention.py:137-144 with the
+ *   context mask of :188-190).  Without a context both halves are the same function and the pair is differentiated as
+ *   one pass.
+ *   grads    a table of the SAME layout as `m` addressing ZERO-FILLED gradient buffers, as for phk_maskgit_train_step;
+ *            every parameter gradient is ACCUMULATED into it (the head members only for LOGITS / SCORE).
+ *   d_context NULL, or fp32 [b, L, dim_context] (zero-filled by the caller): d out / d context is accumulated into it,
+ *            over every cross-attention layer and both halves of a pair.
+ * No dropout is applied: the module forwards this differentiates apply none.  The gradient-shrink trick (:199) scales
+ * the embedding gradients as in the training step.  Configurations the training step does not support return
+ * PHK_E_UNSUPPORTED. */
+enum { PHK_HEAD_LOGITS = 0, PHK_HEAD_EMBEDS = 1, PHK_HEAD_SCORE = 2 };
+int64_t phk_maskgit_backward_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L, int32_t cfg_pair,
+                                             int32_t head_kind, int32_t prec);
+int phk_maskgit_backward(const phk_maskgit_t* m, const phk_maskgit_t* grads, const int64_t* ids, int32_t b, int32_t n,
+                         int32_t pt, int32_t ph, int32_t pw, const float* context, int32_t L, const uint8_t* text_mask,
+                         const uint8_t* video_mask, int32_t cfg_pair, float cond_scale, int32_t head_kind,
+                         const float* upstream, float* d_context, void* workspace, int64_t workspace_bytes, int32_t prec,
+                         phk_stream_t s);
+
 #ifdef __cplusplus
 }
 #endif

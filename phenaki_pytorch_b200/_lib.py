@@ -9,6 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PHK_LIB") or os.path.join(_HERE, "libphk.so")  # PHK_LIB: an A/B build of the same ABI (tools/ only)
 
 PREC_F32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
+HEAD_LOGITS, HEAD_EMBEDS, HEAD_SCORE = 0, 1, 2  # phk_maskgit_backward head kinds
 
 
 def default_precision():
@@ -178,9 +179,12 @@ PROTOTYPES = {
     "phk_maskgit_train_dropout_counters": [C.POINTER(MaskgitT), i32, i32, i32],
     "phk_maskgit_train_step": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, i32,
                                vp, vp, f32, vp, vp, vp, i64, i32, vp, C.POINTER(DropoutT)],
+    "phk_maskgit_backward_workspace_bytes": [C.POINTER(MaskgitT), i32, i32, i32, i32, i32, i32],
+    "phk_maskgit_backward": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, i32,
+                             f32, i32, vp, vp, vp, i64, i32, vp],
 }
 _RESTYPES = {"phk_attention_tc_scratch_bytes": i64, "phk_head_sample_scratch_bytes": i64,
-             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_maskgit_train_dropout_counters": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
+             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_maskgit_train_dropout_counters": i64, "phk_maskgit_backward_workspace_bytes": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
              "phk_cvivit_workspace_bytes": i64, "phk_cvivit_decode_workspace_bytes": i64, "phk_maskgit_workspace_bytes": i64}
 
 FAMILIES = ["patchify_ln", "layernorm", "gemm_f32", "gemm_bf16", "attention", "peg", "geglu", "lfq", "embed",

@@ -1204,9 +1204,327 @@ static inline int progress_mark(void** ev, int n, int idx, cudaStream_t st) {
   return 0;
 }
 
-extern "C" int64_t phk_maskgit_train_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L,
-                                                     int32_t bce_head, int32_t prec) {
-  if (!m || b <= 0 || n <= 0 || L < 0 || !m->transformer.layers) return -1;
+// ------------------------------------------------------------------------------------------------------------------
+// The three stages of one differentiation of the MaskGit / TokenCritic body, shared by phk_maskgit_train_step (a loss
+// head) and phk_maskgit_backward (a gradient the caller supplies):
+//   1. step_forward   embed -> [PEG, self-attn, cross-attn, FF] x depth -> norm_out, keeping every layer's activations;
+//                     S.emb = the final embeddings [R, D]
+//   2. the head       (in each entry point) accumulates the head's parameter gradients and writes d/d(emb) to S.dtmp
+//   3. step_backward  norm_out, transformer, embedding and position-bias backward from S.dtmp
+// ------------------------------------------------------------------------------------------------------------------
+namespace phk {
+namespace {
+
+struct Step {
+  const phk_maskgit_t* m = nullptr;
+  const phk_maskgit_t* grads = nullptr;
+  const phk_transformer_t* T = nullptr;
+  const phk_transformer_t* GT = nullptr;
+  const int64_t* ids = nullptr;
+  int b = 0, n = 0, pt = 0, ph = 0, pw = 0, L = 0;
+  const float* context = nullptr;
+  const uint8_t* text_mask = nullptr;
+  const uint8_t* video_mask = nullptr;
+  int prec = PHK_PREC_F32;
+  phk_stream_t s = nullptr;
+  cudaStream_t st = nullptr;
+  const phk_dropout_t* dropout = nullptr;
+  bool drop_on = false;
+  float attn_p = 0.f, ff_p = 0.f;
+  int D = 0, H = 0, DH = 0, I = 0;
+  int64_t R = 0, CR = 0;
+  Arena ar{nullptr, 0, 0};
+  TcScratch tc{nullptr, nullptr, 0};
+  float* emb = nullptr;
+  float* bias = nullptr;
+  float* dbias = nullptr;
+  float* asc = nullptr;
+  const float* xf = nullptr;
+  float* dxa = nullptr;
+  float* dxb = nullptr;
+  float* dtmp = nullptr;
+  float2* stats = nullptr;
+  LayerSave* sv = nullptr;
+  uint64_t (*bases)[3] = nullptr;
+  ~Step() { delete[] sv; delete[] bases; }
+
+  // dropout: site k of layer l (0 self-attention, 1 cross-attention, 2 FF) draws from counters offset + bases[l][k];
+  // p == 0: the site is off
+  DropSite site(float p, int l, int k) const {
+    DropSite d{0.f, 0.f, 0u, 0u, 0u};
+    if (drop_on && p > 0.f) {
+      d.p = p; d.scale = 1.0f / (1.0f - p);
+      d.k0 = (uint32_t)dropout->seed; d.k1 = (uint32_t)(dropout->seed >> 32);
+      d.base = dropout->offset + bases[l][k];
+    }
+    return d;
+  }
+};
+
+// Fills the derived members of S from its inputs (m, grads, b, n, L, context, prec, s, dropout, workspace arena).
+void step_init(Step& S) {
+  S.T = &S.m->transformer;
+  S.GT = &S.grads->transformer;
+  S.st = to_stream(S.s);
+  S.drop_on = S.dropout && (S.dropout->attn_p > 0.f || S.dropout->ff_p > 0.f);
+  S.attn_p = S.dropout ? S.dropout->attn_p : 0.f;
+  S.ff_p = S.dropout ? S.dropout->ff_p : 0.f;
+  S.D = S.m->dim; S.H = S.T->heads; S.DH = S.T->dim_head; S.I = S.H * S.DH;
+  S.R = (int64_t)S.b * S.n; S.CR = (int64_t)S.b * S.L;
+}
+
+// Stage 1.  wide_head: the bf16 operand buffers must hold the V-wide operands of the logits head.
+int step_forward(Step& S, bool wide_head) {
+  const phk_maskgit_t* m = S.m;
+  const phk_transformer_t* T = S.T;
+  const int b = S.b, n = S.n, pt = S.pt, ph = S.ph, pw = S.pw, L = S.L;
+  const int D = S.D, H = S.H, DH = S.DH, I = S.I;
+  const int64_t R = S.R, CR = S.CR;
+  const int prec = S.prec;
+  const phk_stream_t s = S.s;
+  const cudaStream_t st = S.st;
+  const float* context = S.context;
+  const uint8_t* text_mask = S.text_mask;
+  const uint8_t* video_mask = S.video_mask;
+  Arena& ar = S.ar;
+  TcScratch& tc = S.tc;
+  if (prec == PHK_PREC_BF16) {  // operand buffers of the wgmma products (activations stay fp32 everywhere else)
+    tc.elems = tc_scratch_elems(m, R, CR, !wide_head);
+    tc.a = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
+    tc.b = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
+    PHK_REQUIRE(tc.a && tc.b, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (tensor-core operands)");
+  }
+
+  float* x = ar.f(R * D);
+  S.emb = ar.f(R * D);
+  if (m->has_bias) {
+    S.bias = ar.f((int64_t)H * n * n);
+    S.dbias = ar.f((int64_t)H * n * n);
+    float* sc = ar.f(phk_cpb_scratch_floats(&m->pos_bias, pt, ph, pw));
+    PHK_REQUIRE(S.bias && S.dbias && sc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (bias)");
+    PHK_TRY(phk_cpb_bias(&m->pos_bias, pt, ph, pw, sc, S.bias, s));
+    PHK_CUDA(cudaMemsetAsync(S.dbias, 0, (int64_t)H * n * n * 4, st));
+  }
+  PHK_REQUIRE(x && S.emb, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small");
+  PHK_TRY(phk_token_embed(S.ids, m->token_emb, m->pos_emb, x, b, n, D, m->num_tokens + 1,
+                          m->is_critic ? -1.f : m->shrink_alpha, 1, s));
+  S.sv = new (std::nothrow) LayerSave[T->depth];
+  PHK_REQUIRE(S.sv, PHK_E_ARG, "maskgit_train_step: out of host memory");
+  if (S.drop_on) {
+    S.bases = new (std::nothrow) uint64_t[T->depth][3];
+    PHK_REQUIRE(S.bases, PHK_E_ARG, "maskgit_train_step: out of host memory");
+    dropout_layout(m, b, n, context ? L : 0, S.bases);
+  }
+  // the attention backward's scratch; the forward's explicit attention path (dropout) uses it too
+  const int nk_cross = L + 8;
+  const int64_t as1 = attn_bwd_scratch_floats(b, H, n, n, DH), as2 = attn_bwd_scratch_floats(b, H, n, nk_cross, DH);
+  S.asc = ar.f(as1 > as2 ? as1 : as2);
+  PHK_REQUIRE(S.asc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (attention scratch)");
+  float* asc = S.asc;
+  const float* bias = S.bias;
+  phk_attn_geom_t ag;
+  const float* xin = x;
+  for (int l = 0; l < T->depth; ++l) {
+    const phk_layer_t& Ly = T->layers[l];
+    LayerSave& Sv = S.sv[l];
+    std::memset(&Sv, 0, sizeof(Sv));
+    const int inner = Ly.ff.inner;
+    PHK_REQUIRE(Ly.has_peg, PHK_E_UNSUPPORTED, "maskgit_train_step: layers without PEG are not supported");
+    Sv.x0 = const_cast<float*>(xin);
+    Sv.x1 = ar.f(R * D); Sv.xn1 = ar.f(R * D); Sv.q1 = ar.f(R * I); Sv.kv1 = ar.f(R * 2 * I); Sv.o1 = ar.f(R * I);
+    Sv.x2 = ar.f(R * D); Sv.x3 = ar.f(R * D); Sv.xn3 = ar.f(R * D); Sv.h = ar.f(R * 2 * (int64_t)inner); Sv.g = ar.f(R * (int64_t)inner);
+    float* xout = ar.f(R * D);
+    PHK_REQUIRE(Sv.x1 && Sv.xn1 && Sv.q1 && Sv.kv1 && Sv.o1 && Sv.x2 && Sv.x3 && Sv.xn3 && Sv.h && Sv.g && xout, PHK_E_WORKSPACE,
+                "maskgit_train_step: workspace too small (activations)");
+    // x1 = peg(x0) + x0
+    PHK_TRY(phk_peg3d(Sv.x0, Ly.peg.w, Ly.peg.b, Sv.x1, b, pt, ph, pw, D, Ly.peg.causal, 0, s));
+    // self attention: q from LN(x1), k/v from RAW x1 (attention.py:140-144)
+    const phk_attn_t& A = Ly.self_attn;
+    PHK_TRY(phk_layernorm(Sv.x1, A.norm_g, A.norm_b, Sv.xn1, nullptr, R, D, 0, 0, 0, 0, s));
+    PHK_TRY(linear_fwd(prec, tc, Sv.xn1, A.wq, Sv.q1, R, I, D, nullptr, nullptr, s));
+    PHK_TRY(linear_fwd(prec, tc, Sv.x1, A.wkv, Sv.kv1, R, 2 * I, D, nullptr, nullptr, s));
+    std::memset(&ag, 0, sizeof(ag));
+    ag.n_outer = b; ag.n_inner = 1; ag.n_q = n; ag.n_k = n; ag.heads = H; ag.dim_head = DH; ag.num_null_kv = A.num_null_kv;
+    ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)n * 2 * I; ag.k_tok = 2 * I;
+    ag.o_outer = ag.q_outer; ag.o_tok = I; ag.mask_off_from = -1; ag.scale = 8.f;
+    PHK_REQUIRE(A.num_null_kv == 0, PHK_E_UNSUPPORTED, "maskgit_train_step: self-attention null-kv is not supported");
+    const DropSite d_self = S.site(S.attn_p, l, 0);
+    if (d_self.p > 0.f) {
+      const AttnBwdGeom g1{b, H, n, n, 0, DH};
+      PHK_TRY(attention_forward_dropout(Sv.q1, Sv.kv1, A, bias, video_mask, Sv.o1, g1, asc, st, d_self));
+    } else {
+      PHK_TRY(phk_attention(Sv.q1, Sv.kv1, A.null_kv, A.q_scale, A.k_scale, bias, video_mask, nullptr, Sv.o1, &ag, s));
+    }
+    PHK_TRY(linear_fwd(prec, tc, Sv.o1, A.wo, Sv.x2, R, D, I, nullptr, Sv.x1, s));  // x2 = x1 + o Wo^T
+    const bool cross = Ly.has_cross && context;
+    if (cross) {
+      const phk_attn_t& Cx = Ly.cross_attn;
+      const int dc = Cx.dim_context;
+      Sv.ctxn = ar.f(CR * dc); Sv.ckv = ar.f(CR * 2 * I); Sv.xn2 = ar.f(R * D); Sv.q2 = ar.f(R * I); Sv.o2 = ar.f(R * I);
+      PHK_REQUIRE(Sv.ctxn && Sv.ckv && Sv.xn2 && Sv.q2 && Sv.o2, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (cross)");
+      PHK_TRY(phk_layernorm(context, Cx.ctx_g, Cx.ctx_b, Sv.ctxn, nullptr, CR, dc, 0, 0, 0, 0, s));
+      PHK_TRY(linear_fwd(prec, tc, Sv.ctxn, Cx.wkv, Sv.ckv, CR, 2 * I, dc, nullptr, nullptr, s));
+      PHK_TRY(phk_layernorm(Sv.x2, Cx.norm_g, Cx.norm_b, Sv.xn2, nullptr, R, D, 0, 0, 0, 0, s));
+      PHK_TRY(linear_fwd(prec, tc, Sv.xn2, Cx.wq, Sv.q2, R, I, D, nullptr, nullptr, s));
+      std::memset(&ag, 0, sizeof(ag));
+      ag.n_outer = b; ag.n_inner = 1; ag.n_q = n; ag.n_k = L; ag.heads = H; ag.dim_head = DH; ag.num_null_kv = Cx.num_null_kv;
+      ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)L * 2 * I; ag.k_tok = 2 * I;
+      ag.o_outer = ag.q_outer; ag.o_tok = I; ag.kv_outer_mod = b; ag.mask_outer_mod = b; ag.mask_off_from = -1; ag.scale = 8.f;
+      const DropSite d_cross = S.site(S.attn_p, l, 1);
+      if (d_cross.p > 0.f) {
+        PHK_REQUIRE(Cx.num_null_kv <= 8, PHK_E_UNSUPPORTED, "maskgit_train_step: more than 8 null key/values");
+        const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
+        PHK_TRY(attention_forward_dropout(Sv.q2, Sv.ckv, Cx, nullptr, text_mask, Sv.o2, g2, asc, st, d_cross));
+      } else {
+        PHK_TRY(phk_attention(Sv.q2, Sv.ckv, Cx.null_kv, Cx.q_scale, Cx.k_scale, nullptr, text_mask, nullptr, Sv.o2, &ag, s));
+      }
+      PHK_TRY(linear_fwd(prec, tc, Sv.o2, Cx.wo, Sv.x3, R, D, I, nullptr, Sv.x2, s));  // x3 = x2 + o2 Wo^T
+    } else {
+      PHK_CUDA(cudaMemcpyAsync(Sv.x3, Sv.x2, R * D * 4, cudaMemcpyDeviceToDevice, st));
+    }
+    // feed forward (attention.py:45-53)
+    PHK_TRY(phk_layernorm(Sv.x3, Ly.ff.ln_g, Ly.ff.ln_b, Sv.xn3, nullptr, R, D, 0, 0, 0, 0, s));
+    PHK_TRY(linear_fwd(prec, tc, Sv.xn3, Ly.ff.w1, Sv.h, R, 2 * inner, D, nullptr, nullptr, s));
+    const DropSite d_ff = S.site(S.ff_p, l, 2);
+    if (d_ff.p > 0.f) {
+      PHK_KERNEL_LAUNCH(geglu_dropout_kernel, dim3(ew_grid_fwd(R * inner)), dim3(256), (size_t)(0), st, Sv.h, Sv.g, R, inner, d_ff);
+      PHK_LAUNCH_CHECK();
+    } else {
+      PHK_TRY(phk_geglu(Sv.h, Sv.g, R, inner, s));
+    }
+    PHK_TRY(linear_fwd(prec, tc, Sv.g, Ly.ff.w2, xout, R, D, inner, nullptr, Sv.x3, s));  // x4 = x3 + g W2^T
+    xin = xout;
+  }
+  S.xf = xin;
+  PHK_TRY(phk_layernorm(S.xf, T->out_g, T->out_b, S.emb, nullptr, R, D, 0, 0, 0, 0, s));
+  return 0;
+}
+
+// The gradient buffers of stage 2 and 3: dxa / dxb (d/d residual stream), dtmp (d/d emb on entry to stage 3), stats.
+int step_gradient_buffers(Step& S) {
+  S.dxa = S.ar.f(S.R * S.D);
+  S.dxb = S.ar.f(S.R * S.D);
+  S.dtmp = S.ar.f(S.R * S.D);
+  return S.dxa && S.dxb && S.dtmp ? 0 : -1;
+}
+int step_stats_buffer(Step& S) {
+  S.stats = reinterpret_cast<float2*>(S.ar.f(2 * (S.R > S.CR ? S.R : S.CR)));
+  return S.stats ? 0 : -1;
+}
+
+// Stage 3.  d_context (optional, [R_ctx, dim_context]): d/d(context) is ACCUMULATED into it over the cross-attention
+// layers.  prog / nprog: the data-parallel progress events (phk_train_set_progress_events).
+int step_backward(Step& S, float* d_context, void** prog, int nprog) {
+  const phk_maskgit_t* m = S.m;
+  const phk_maskgit_t* grads = S.grads;
+  const phk_transformer_t* T = S.T;
+  const phk_transformer_t* GT = S.GT;
+  const int b = S.b, n = S.n, pt = S.pt, ph = S.ph, pw = S.pw, L = S.L;
+  const int D = S.D, H = S.H, DH = S.DH, I = S.I;
+  const int64_t R = S.R, CR = S.CR;
+  const int prec = S.prec;
+  const phk_stream_t s = S.s;
+  const cudaStream_t st = S.st;
+  const float* context = S.context;
+  const uint8_t* text_mask = S.text_mask;
+  const uint8_t* video_mask = S.video_mask;
+  Arena& ar = S.ar;
+  const TcScratch& tc = S.tc;
+  float2* stats = S.stats;
+  int64_t inner_max = 0, dc_max = 0;
+  for (int l = 0; l < T->depth; ++l) {
+    if (T->layers[l].ff.inner > inner_max) inner_max = T->layers[l].ff.inner;
+    if (T->layers[l].has_cross && T->layers[l].cross_attn.dim_context > dc_max) dc_max = T->layers[l].cross_attn.dim_context;
+  }
+  float* dq = ar.f(R * I);
+  float* dkv = ar.f(R * 2 * I);
+  float* dob = ar.f(R * I);
+  float* dh = ar.f(R * 2 * inner_max);
+  float* dg = ar.f(R * inner_max);
+  float* dckv = context ? ar.f(CR * 2 * I) : nullptr;
+  float* dctxn = context ? ar.f(CR * (dc_max > 0 ? dc_max : 1)) : nullptr;
+  PHK_REQUIRE(dq && dkv && dob && dh && dg && (!context || (dckv && dctxn)), PHK_E_WORKSPACE,
+              "maskgit_train_step: workspace too small (gradients)");
+  float* dx = S.dxa;      // d loss / d (current residual stream)
+  float* dx_alt = S.dxb;
+  PHK_TRY(ln_backward(S.xf, T->out_g, S.dtmp, dx, 0, (float*)GT->out_g, nullptr, stats, R, D, st));
+  PHK_TRY(progress_mark(prog, nprog, 0, st));  // head + norm_out gradients final
+  for (int l = T->depth - 1; l >= 0; --l) {
+    const phk_layer_t& Ly = T->layers[l];
+    const phk_layer_t& Gy = GT->layers[l];
+    const LayerSave& Sv = S.sv[l];
+    const int inner = Ly.ff.inner;
+    // feed forward: x4 = x3 + geglu(LN(x3) W1^T) W2^T
+    PHK_TRY(dgrad_p(prec, tc, dx, Ly.ff.w2, dg, R, D, inner, 0, s));
+    PHK_TRY(wgrad_p(prec, tc, dx, Sv.g, (float*)Gy.ff.w2, R, D, inner, s));
+    PHK_KERNEL_LAUNCH(geglu_bwd_kernel, dim3(ew_grid(R * inner)), dim3(256), (size_t)(0), st, Sv.h, dg, dh, R, inner, S.site(S.ff_p, l, 2));
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(wgrad_p(prec, tc, dh, Sv.xn3, (float*)Gy.ff.w1, R, 2 * inner, D, s));
+    PHK_TRY(dgrad_p(prec, tc, dh, Ly.ff.w1, S.dtmp, R, 2 * inner, D, 0, s));
+    PHK_TRY(ln_backward(Sv.x3, Ly.ff.ln_g, S.dtmp, dx, 1, (float*)Gy.ff.ln_g, (float*)Gy.ff.ln_b, stats, R, D, st));
+    // cross attention: x3 = x2 + attn(LN(x2) Wq^T, LN_ctx(context) Wkv^T) Wo^T
+    if (Sv.o2) {
+      const phk_attn_t& Cx = Ly.cross_attn;
+      const phk_attn_t& Gx = Gy.cross_attn;
+      const int dc = Cx.dim_context;
+      PHK_REQUIRE(Cx.num_null_kv <= 8, PHK_E_UNSUPPORTED, "maskgit_train_step: more than 8 null key/values");
+      PHK_TRY(dgrad_p(prec, tc, dx, Cx.wo, dob, R, D, I, 0, s));
+      PHK_TRY(wgrad_p(prec, tc, dx, Sv.o2, (float*)Gx.wo, R, D, I, s));
+      const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
+      PHK_TRY(attention_backward(Sv.q2, Sv.ckv, Cx, Gx, nullptr, text_mask, dob, dq, dckv, nullptr, g2, S.asc, st, prec == PHK_PREC_BF16,
+                                 S.site(S.attn_p, l, 1)));
+      PHK_TRY(wgrad_p(prec, tc, dq, Sv.xn2, (float*)Gx.wq, R, I, D, s));
+      PHK_TRY(dgrad_p(prec, tc, dq, Cx.wq, S.dtmp, R, I, D, 0, s));
+      PHK_TRY(ln_backward(Sv.x2, Cx.norm_g, S.dtmp, dx, 1, (float*)Gx.norm_g, nullptr, stats, R, D, st));
+      PHK_TRY(wgrad_p(prec, tc, dckv, Sv.ctxn, (float*)Gx.wkv, CR, 2 * I, dc, s));
+      PHK_TRY(dgrad_p(prec, tc, dckv, Cx.wkv, dctxn, CR, 2 * I, dc, 0, s));
+      // context_norm backward: d/d(context) accumulates over the layers when the caller asks for it
+      PHK_TRY(ln_backward(context, Cx.ctx_g, dctxn, d_context, d_context ? 1 : 0, (float*)Gx.ctx_g, nullptr, stats, CR, dc, st));
+    }
+    // self attention: x2 = x1 + attn(LN(x1) Wq^T, x1 Wkv^T) Wo^T
+    {
+      const phk_attn_t& A = Ly.self_attn;
+      const phk_attn_t& GA = Gy.self_attn;
+      PHK_TRY(dgrad_p(prec, tc, dx, A.wo, dob, R, D, I, 0, s));
+      PHK_TRY(wgrad_p(prec, tc, dx, Sv.o1, (float*)GA.wo, R, D, I, s));
+      const AttnBwdGeom g1{b, H, n, n, 0, DH};
+      PHK_TRY(attention_backward(Sv.q1, Sv.kv1, A, GA, S.bias, video_mask, dob, dq, dkv, S.dbias, g1, S.asc, st, prec == PHK_PREC_BF16,
+                                 S.site(S.attn_p, l, 0)));
+      PHK_TRY(wgrad_p(prec, tc, dq, Sv.xn1, (float*)GA.wq, R, I, D, s));
+      PHK_TRY(wgrad_p(prec, tc, dkv, Sv.x1, (float*)GA.wkv, R, 2 * I, D, s));
+      PHK_TRY(dgrad_p(prec, tc, dq, A.wq, S.dtmp, R, I, D, 0, s));
+      PHK_TRY(ln_backward(Sv.x1, A.norm_g, S.dtmp, dx, 1, (float*)GA.norm_g, nullptr, stats, R, D, st));
+      PHK_TRY(dgrad_p(prec, tc, dkv, A.wkv, dx, R, 2 * I, D, 1, s));  // the raw-x path of k, v
+    }
+    // PEG: x1 = x0 + conv(x0) + b
+    PHK_TRY(colsum(dx, R, D, D, (float*)Gy.peg.b, st));
+    PHK_REQUIRE(D <= 128 * PEG_DW_MAXJ, PHK_E_UNSUPPORTED, "maskgit_train_step: dim > 1024");
+    PHK_KERNEL_LAUNCH(peg_bwd_dw_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, Sv.x0, dx, (float*)Gy.peg.w, R, pt, ph, pw, D, Ly.peg.causal ? 2 : 1);
+    PHK_LAUNCH_CHECK();
+    PHK_KERNEL_LAUNCH(peg_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, Sv.x0, Ly.peg.w, dx, dx_alt, pt, ph, pw, D, Ly.peg.causal ? 2 : 1);
+    PHK_LAUNCH_CHECK();
+    float* t = dx; dx = dx_alt; dx_alt = t;
+    // this layer's parameter gradients are final -- except, with a context, the cross-attention's context_norm / to_kv
+    // share nothing with other layers either; the position-bias gradient (dbias, all layers) is finished below
+    PHK_TRY(progress_mark(prog, nprog, 1 + (T->depth - 1 - l), st));
+  }
+  // ---------------------------------------------------------------- embeddings, position-bias MLP
+  PHK_KERNEL_LAUNCH(embed_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, S.ids, dx, (float*)grads->token_emb, (float*)grads->pos_emb, n, D,
+                                               m->is_critic ? 1.0f : m->shrink_alpha, m->num_tokens + 1);
+  PHK_LAUNCH_CHECK();
+  if (m->has_bias) {
+    float* csc = ar.f(cpb_bwd_scratch_floats(m->pos_bias, pt, ph, pw));
+    PHK_REQUIRE(csc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (position-bias backward)");
+    PHK_TRY(cpb_backward(m->pos_bias, grads->pos_bias, S.dbias, pt, ph, pw, csc, st));
+  }
+  PHK_TRY(progress_mark(prog, nprog, T->depth + 1, st));
+  return 0;
+}
+
+// Workspace of one differentiation of b sequences: stage 1 and 3 (activations, gradient buffers, attention and
+// position-bias scratch) + head_floats for stage 2; wide_head: the bf16 operand buffers hold the V-wide head operands.
+int64_t step_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L, int64_t head_floats, bool wide_head,
+                             int32_t prec) {
   const phk_transformer_t* T = &m->transformer;
   const int64_t R = (int64_t)b * n, CR = (int64_t)b * L, D = m->dim, I = (int64_t)T->heads * T->dim_head;
   int64_t inner = 0, dc = 0, f = 0;
@@ -1216,7 +1534,7 @@ extern "C" int64_t phk_maskgit_train_workspace_bytes(const phk_maskgit_t* m, int
     if (T->layers[l].has_cross && T->layers[l].cross_attn.dim_context > dc) dc = T->layers[l].cross_attn.dim_context;
   }
   f += R * D * 2;                                            // x (embedding output), final embeddings
-  f += bce_head ? 3 * R : R * (int64_t)m->num_tokens + 2 * R;  // (d)logits in place or the differentiated copy; row losses
+  f += head_floats;
   f += R * (D * 3 + I * 4 + 3 * inner) + CR * (2 * I + dc);  // dxa dxb dtmp | dq dkv(2) do | dh(2) dg | dckv dctxn
   f += 2 * (R > CR ? R : CR);                                // LayerNorm statistics
   const int64_t a1 = attn_bwd_scratch_floats(b, T->heads, n, n, T->dim_head);
@@ -1228,8 +1546,20 @@ extern "C" int64_t phk_maskgit_train_workspace_bytes(const phk_maskgit_t* m, int
     f += 2 * (int64_t)T->heads * n * n + U * m->pos_bias.heads + U * (3 + 4 * (int64_t)m->pos_bias.hidden + m->pos_bias.heads) + 128;
   }
   int64_t bytes = f * 4 + 256 * 64;
-  if (prec == PHK_PREC_BF16) bytes += 2 * (tc_scratch_elems(m, R, CR, bce_head != 0) * 2 + 256);
+  if (prec == PHK_PREC_BF16) bytes += 2 * (tc_scratch_elems(m, R, CR, !wide_head) * 2 + 256);
   return bytes;
+}
+
+}  // namespace
+}  // namespace phk
+
+extern "C" int64_t phk_maskgit_train_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L,
+                                                     int32_t bce_head, int32_t prec) {
+  if (!m || b <= 0 || n <= 0 || L < 0 || !m->transformer.layers) return -1;
+  const int64_t R = (int64_t)b * n;
+  // (d)logits in place or the differentiated copy; row losses
+  const int64_t head = bce_head ? 3 * R : R * (int64_t)m->num_tokens + 2 * R;
+  return step_workspace_bytes(m, b, n, L, head, !bce_head, prec);
 }
 
 extern "C" int64_t phk_maskgit_train_dropout_counters(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L) {
@@ -1267,158 +1597,41 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "maskgit_train_step: dim must be a multiple of 4");
   PHK_REQUIRE(!dropout || (dropout->attn_p >= 0.f && dropout->attn_p <= 1.f && dropout->ff_p >= 0.f && dropout->ff_p <= 1.f),
               PHK_E_ARG, "maskgit_train_step: dropout probabilities must lie in [0, 1]");
-  const bool drop_on = dropout && (dropout->attn_p > 0.f || dropout->ff_p > 0.f);
-  cudaStream_t st = to_stream(s);
   void** prog = g_progress_events;  // one-shot: consumed by this call
   const int nprog = g_progress_count;
   g_progress_events = nullptr; g_progress_count = 0;
-  const int D = m->dim, H = T->heads, DH = T->dim_head, I = H * DH, V = m->num_tokens;
-  const int64_t R = (int64_t)b * n, CR = (int64_t)b * L;
-  Arena ar{(char*)workspace, workspace_bytes, 0};
-  TcScratch tc{nullptr, nullptr, 0};
-  if (prec == PHK_PREC_BF16) {  // operand buffers of the wgmma products (activations stay fp32 everywhere else)
-    tc.elems = tc_scratch_elems(m, R, CR, bce);
-    tc.a = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
-    tc.b = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
-    PHK_REQUIRE(tc.a && tc.b, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (tensor-core operands)");
-  }
+  Step S;
+  S.m = m; S.grads = grads; S.ids = ids_in; S.b = b; S.n = n; S.pt = pt; S.ph = ph; S.pw = pw; S.L = L;
+  S.context = context; S.text_mask = text_mask; S.video_mask = video_mask; S.prec = prec; S.s = s; S.dropout = dropout;
+  S.ar = Arena{(char*)workspace, workspace_bytes, 0};
+  step_init(S);
+  const cudaStream_t st = S.st;
+  const int D = S.D, V = m->num_tokens;
+  const int64_t R = S.R;
 
   // ---------------------------------------------------------------- forward (saving activations)
-  float* x = ar.f(R * D);
-  float* emb = ar.f(R * D);
-  float* bias = nullptr;
-  float* dbias = nullptr;
-  if (m->has_bias) {
-    bias = ar.f((int64_t)H * n * n);
-    dbias = ar.f((int64_t)H * n * n);
-    float* sc = ar.f(phk_cpb_scratch_floats(&m->pos_bias, pt, ph, pw));
-    PHK_REQUIRE(bias && dbias && sc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (bias)");
-    PHK_TRY(phk_cpb_bias(&m->pos_bias, pt, ph, pw, sc, bias, s));
-    PHK_CUDA(cudaMemsetAsync(dbias, 0, (int64_t)H * n * n * 4, st));
-  }
-  PHK_REQUIRE(x && emb, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small");
-  PHK_TRY(phk_token_embed(ids_in, m->token_emb, m->pos_emb, x, b, n, D, m->num_tokens + 1,
-                          m->is_critic ? -1.f : m->shrink_alpha, 1, s));
-  LayerSave* sv = new (std::nothrow) LayerSave[T->depth];
-  PHK_REQUIRE(sv, PHK_E_ARG, "maskgit_train_step: out of host memory");
-  struct Free { LayerSave* p; ~Free() { delete[] p; } } free_sv{sv};
-  // dropout: site s of layer l (0 self-attention, 1 cross-attention, 2 FF) draws from counters offset + bases[l][s]
-  uint64_t (*bases)[3] = drop_on ? new (std::nothrow) uint64_t[T->depth][3] : nullptr;
-  PHK_REQUIRE(!drop_on || bases, PHK_E_ARG, "maskgit_train_step: out of host memory");
-  struct FreeBases { uint64_t (*p)[3]; ~FreeBases() { delete[] p; } } free_bases{bases};
-  if (drop_on) dropout_layout(m, b, n, context ? L : 0, bases);
-  auto site = [&](float p, int l, int k) {  // p == 0: the site is off
-    DropSite d{0.f, 0.f, 0u, 0u, 0u};
-    if (drop_on && p > 0.f) {
-      d.p = p; d.scale = 1.0f / (1.0f - p);
-      d.k0 = (uint32_t)dropout->seed; d.k1 = (uint32_t)(dropout->seed >> 32);
-      d.base = dropout->offset + bases[l][k];
-    }
-    return d;
-  };
-  const float attn_p = dropout ? dropout->attn_p : 0.f, ff_p = dropout ? dropout->ff_p : 0.f;
-  // the attention backward's scratch; the forward's explicit attention path (dropout) uses it too
-  const int nk_cross = L + 8;
-  const int64_t as1 = attn_bwd_scratch_floats(b, H, n, n, DH), as2 = attn_bwd_scratch_floats(b, H, n, nk_cross, DH);
-  float* asc = ar.f(as1 > as2 ? as1 : as2);
-  PHK_REQUIRE(asc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (attention scratch)");
-  phk_attn_geom_t ag;
-  const float* xin = x;
-  for (int l = 0; l < T->depth; ++l) {
-    const phk_layer_t& Ly = T->layers[l];
-    LayerSave& S = sv[l];
-    std::memset(&S, 0, sizeof(S));
-    const int inner = Ly.ff.inner;
-    PHK_REQUIRE(Ly.has_peg, PHK_E_UNSUPPORTED, "maskgit_train_step: layers without PEG are not supported");
-    S.x0 = const_cast<float*>(xin);
-    S.x1 = ar.f(R * D); S.xn1 = ar.f(R * D); S.q1 = ar.f(R * I); S.kv1 = ar.f(R * 2 * I); S.o1 = ar.f(R * I);
-    S.x2 = ar.f(R * D); S.x3 = ar.f(R * D); S.xn3 = ar.f(R * D); S.h = ar.f(R * 2 * (int64_t)inner); S.g = ar.f(R * (int64_t)inner);
-    float* xout = ar.f(R * D);
-    PHK_REQUIRE(S.x1 && S.xn1 && S.q1 && S.kv1 && S.o1 && S.x2 && S.x3 && S.xn3 && S.h && S.g && xout, PHK_E_WORKSPACE,
-                "maskgit_train_step: workspace too small (activations)");
-    // x1 = peg(x0) + x0
-    PHK_TRY(phk_peg3d(S.x0, Ly.peg.w, Ly.peg.b, S.x1, b, pt, ph, pw, D, Ly.peg.causal, 0, s));
-    // self attention: q from LN(x1), k/v from RAW x1 (attention.py:140-144)
-    const phk_attn_t& A = Ly.self_attn;
-    PHK_TRY(phk_layernorm(S.x1, A.norm_g, A.norm_b, S.xn1, nullptr, R, D, 0, 0, 0, 0, s));
-    PHK_TRY(linear_fwd(prec, tc, S.xn1, A.wq, S.q1, R, I, D, nullptr, nullptr, s));
-    PHK_TRY(linear_fwd(prec, tc, S.x1, A.wkv, S.kv1, R, 2 * I, D, nullptr, nullptr, s));
-    std::memset(&ag, 0, sizeof(ag));
-    ag.n_outer = b; ag.n_inner = 1; ag.n_q = n; ag.n_k = n; ag.heads = H; ag.dim_head = DH; ag.num_null_kv = A.num_null_kv;
-    ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)n * 2 * I; ag.k_tok = 2 * I;
-    ag.o_outer = ag.q_outer; ag.o_tok = I; ag.mask_off_from = -1; ag.scale = 8.f;
-    PHK_REQUIRE(A.num_null_kv == 0, PHK_E_UNSUPPORTED, "maskgit_train_step: self-attention null-kv is not supported");
-    const DropSite d_self = site(attn_p, l, 0);
-    if (d_self.p > 0.f) {
-      const AttnBwdGeom g1{b, H, n, n, 0, DH};
-      PHK_TRY(attention_forward_dropout(S.q1, S.kv1, A, bias, video_mask, S.o1, g1, asc, st, d_self));
-    } else {
-      PHK_TRY(phk_attention(S.q1, S.kv1, A.null_kv, A.q_scale, A.k_scale, bias, video_mask, nullptr, S.o1, &ag, s));
-    }
-    PHK_TRY(linear_fwd(prec, tc, S.o1, A.wo, S.x2, R, D, I, nullptr, S.x1, s));  // x2 = x1 + o Wo^T
-    const bool cross = Ly.has_cross && context;
-    if (cross) {
-      const phk_attn_t& Cx = Ly.cross_attn;
-      const int dc = Cx.dim_context;
-      S.ctxn = ar.f(CR * dc); S.ckv = ar.f(CR * 2 * I); S.xn2 = ar.f(R * D); S.q2 = ar.f(R * I); S.o2 = ar.f(R * I);
-      PHK_REQUIRE(S.ctxn && S.ckv && S.xn2 && S.q2 && S.o2, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (cross)");
-      PHK_TRY(phk_layernorm(context, Cx.ctx_g, Cx.ctx_b, S.ctxn, nullptr, CR, dc, 0, 0, 0, 0, s));
-      PHK_TRY(linear_fwd(prec, tc, S.ctxn, Cx.wkv, S.ckv, CR, 2 * I, dc, nullptr, nullptr, s));
-      PHK_TRY(phk_layernorm(S.x2, Cx.norm_g, Cx.norm_b, S.xn2, nullptr, R, D, 0, 0, 0, 0, s));
-      PHK_TRY(linear_fwd(prec, tc, S.xn2, Cx.wq, S.q2, R, I, D, nullptr, nullptr, s));
-      std::memset(&ag, 0, sizeof(ag));
-      ag.n_outer = b; ag.n_inner = 1; ag.n_q = n; ag.n_k = L; ag.heads = H; ag.dim_head = DH; ag.num_null_kv = Cx.num_null_kv;
-      ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)L * 2 * I; ag.k_tok = 2 * I;
-      ag.o_outer = ag.q_outer; ag.o_tok = I; ag.kv_outer_mod = b; ag.mask_outer_mod = b; ag.mask_off_from = -1; ag.scale = 8.f;
-      const DropSite d_cross = site(attn_p, l, 1);
-      if (d_cross.p > 0.f) {
-        PHK_REQUIRE(Cx.num_null_kv <= 8, PHK_E_UNSUPPORTED, "maskgit_train_step: more than 8 null key/values");
-        const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
-        PHK_TRY(attention_forward_dropout(S.q2, S.ckv, Cx, nullptr, text_mask, S.o2, g2, asc, st, d_cross));
-      } else {
-        PHK_TRY(phk_attention(S.q2, S.ckv, Cx.null_kv, Cx.q_scale, Cx.k_scale, nullptr, text_mask, nullptr, S.o2, &ag, s));
-      }
-      PHK_TRY(linear_fwd(prec, tc, S.o2, Cx.wo, S.x3, R, D, I, nullptr, S.x2, s));  // x3 = x2 + o2 Wo^T
-    } else {
-      PHK_CUDA(cudaMemcpyAsync(S.x3, S.x2, R * D * 4, cudaMemcpyDeviceToDevice, st));
-    }
-    // feed forward (attention.py:45-53)
-    PHK_TRY(phk_layernorm(S.x3, Ly.ff.ln_g, Ly.ff.ln_b, S.xn3, nullptr, R, D, 0, 0, 0, 0, s));
-    PHK_TRY(linear_fwd(prec, tc, S.xn3, Ly.ff.w1, S.h, R, 2 * inner, D, nullptr, nullptr, s));
-    const DropSite d_ff = site(ff_p, l, 2);
-    if (d_ff.p > 0.f) {
-      PHK_KERNEL_LAUNCH(geglu_dropout_kernel, dim3(ew_grid_fwd(R * inner)), dim3(256), (size_t)(0), st, S.h, S.g, R, inner, d_ff);
-      PHK_LAUNCH_CHECK();
-    } else {
-      PHK_TRY(phk_geglu(S.h, S.g, R, inner, s));
-    }
-    PHK_TRY(linear_fwd(prec, tc, S.g, Ly.ff.w2, xout, R, D, inner, nullptr, S.x3, s));  // x4 = x3 + g W2^T
-    xin = xout;
-  }
-  const float* xf = xin;
-  PHK_TRY(phk_layernorm(xf, T->out_g, T->out_b, emb, nullptr, R, D, 0, 0, 0, 0, s));
+  PHK_TRY(step_forward(S, !bce));
 
   // ---------------------------------------------------------------- head + loss -> demb
-  float* dxa = ar.f(R * D);
-  float* dxb = ar.f(R * D);
-  float* dtmp = ar.f(R * D);
+  Arena& ar = S.ar;
+  const int gb = step_gradient_buffers(S);
   float* row_loss = ar.f(R);
   float* cnt = ar.f(64);
-  float2* stats = reinterpret_cast<float2*>(ar.f(2 * (R > CR ? R : CR)));
-  PHK_REQUIRE(dxa && dxb && dtmp && row_loss && cnt && stats, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (bwd)");
+  const int sb = step_stats_buffer(S);
+  PHK_REQUIRE(gb == 0 && row_loss && cnt && sb == 0, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (bwd)");
   if (bce) {
     float* dscore = ar.f(R);
     PHK_REQUIRE(dscore, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small");
-    PHK_KERNEL_LAUNCH(bce_rows_kernel, dim3((unsigned)((R + 7) / 8)), dim3(256), (size_t)(0), st, emb, m->head_w, m->head_b, labels, loss_scale, row_loss, dscore, R, D);
+    PHK_KERNEL_LAUNCH(bce_rows_kernel, dim3((unsigned)((R + 7) / 8)), dim3(256), (size_t)(0), st, S.emb, m->head_w, m->head_b, labels, loss_scale, row_loss, dscore, R, D);
     PHK_LAUNCH_CHECK();
-    PHK_TRY(wgrad(dscore, emb, (float*)grads->head_w, R, 1, D, st));  // [1, dim]: not worth a tensor-core launch
+    PHK_TRY(wgrad(dscore, S.emb, (float*)grads->head_w, R, 1, D, st));  // [1, dim]: not worth a tensor-core launch
     PHK_TRY(colsum(dscore, R, 1, 1, (float*)grads->head_b, st));
-    PHK_KERNEL_LAUNCH(outer_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dscore, m->head_w, dtmp, R, D);
+    PHK_KERNEL_LAUNCH(outer_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dscore, m->head_w, S.dtmp, R, D);
     PHK_LAUNCH_CHECK();
   } else {
     float* logits = logits_out ? logits_out : ar.f(R * (int64_t)V);
     PHK_REQUIRE(logits, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (logits)");
-    PHK_TRY(linear_fwd(prec, tc, emb, m->head_w, logits, R, V, D, m->head_b, nullptr, s));
+    PHK_TRY(linear_fwd(prec, S.tc, S.emb, m->head_w, logits, R, V, D, m->head_b, nullptr, s));
     float* dl = logits;
     if (logits_out) {  // the caller keeps the logits (critic sampling, :646): differentiate a copy
       dl = ar.f(R * (int64_t)V);
@@ -1429,99 +1642,173 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
     PHK_LAUNCH_CHECK();
     PHK_KERNEL_LAUNCH(ce_rows_kernel, dim3((unsigned)R), dim3(256), (size_t)(0), st, dl, targets, token_mask, cnt, loss_scale, row_loss, V);
     PHK_LAUNCH_CHECK();
-    PHK_TRY(wgrad_p(prec, tc, dl, emb, (float*)grads->head_w, R, V, D, s));
+    PHK_TRY(wgrad_p(prec, S.tc, dl, S.emb, (float*)grads->head_w, R, V, D, s));
     PHK_TRY(colsum(dl, R, V, V, (float*)grads->head_b, st));
-    PHK_TRY(dgrad_p(prec, tc, dl, m->head_w, dtmp, R, V, D, 0, s));
+    PHK_TRY(dgrad_p(prec, S.tc, dl, m->head_w, S.dtmp, R, V, D, 0, s));
   }
   PHK_KERNEL_LAUNCH(loss_reduce_kernel, dim3(1), dim3(1024), (size_t)(0), st, row_loss, R, loss_out);
   PHK_LAUNCH_CHECK();
 
   // ---------------------------------------------------------------- backward through the transformer
-  int64_t inner_max = 0, dc_max = 0;
-  for (int l = 0; l < T->depth; ++l) {
-    if (T->layers[l].ff.inner > inner_max) inner_max = T->layers[l].ff.inner;
-    if (T->layers[l].has_cross && T->layers[l].cross_attn.dim_context > dc_max) dc_max = T->layers[l].cross_attn.dim_context;
+  return step_backward(S, nullptr, prog, nprog);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Backward from a caller-supplied gradient (include/phk.h, phk_maskgit_backward): stage 1 recomputes the forward of
+// the module call being differentiated, stage 2 starts from the upstream gradient instead of a loss.
+// Classifier-free-guidance pair: the forward ran 2b sequences, the second half under an all-false text mask, and
+// returned out = null + s (cond - null).  The head is linear, so with g = d/d(out):
+//   dW_head = g^T . (s E_cond + (1 - s) E_null),  db = colsum(g),  dE_cond = s (g . W),  dE_null = (1 - s) (g . W)
+// -- one wgrad against the mixed embeddings and one dgrad, never a [2 b n, V] gradient.
+// ------------------------------------------------------------------------------------------------------------------
+namespace phk {
+namespace {
+
+// out = s a + (1 - s) b
+__global__ void cfg_mix_kernel(const float* __restrict__ a, const float* __restrict__ b, float s, float* __restrict__ out,
+                               int64_t total) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] = s * a[i] + (1.0f - s) * b[i];
+}
+// d[half + i] = (1 - s) d[i], then d[i] = s d[i]: the gradient of both halves from that of the combined output
+__global__ void cfg_split_kernel(float* __restrict__ d, float s, int64_t half) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (int64_t)gridDim.x * blockDim.x) {
+    const float v = d[i];
+    d[half + i] = (1.0f - s) * v;
+    d[i] = s * v;
   }
-  float* dq = ar.f(R * I);
-  float* dkv = ar.f(R * 2 * I);
-  float* dob = ar.f(R * I);
-  float* dh = ar.f(R * 2 * inner_max);
-  float* dg = ar.f(R * inner_max);
-  float* dckv = context ? ar.f(CR * 2 * I) : nullptr;
-  float* dctxn = context ? ar.f(CR * (dc_max > 0 ? dc_max : 1)) : nullptr;
-  PHK_REQUIRE(dq && dkv && dob && dh && dg && (!context || (dckv && dctxn)), PHK_E_WORKSPACE,
-              "maskgit_train_step: workspace too small (gradients)");
-  float* dx = dxa;      // d loss / d (current residual stream)
-  float* dx_alt = dxb;
-  PHK_TRY(ln_backward(xf, T->out_g, dtmp, dx, 0, (float*)GT->out_g, nullptr, stats, R, D, st));
-  PHK_TRY(progress_mark(prog, nprog, 0, st));  // head + norm_out gradients final
-  for (int l = T->depth - 1; l >= 0; --l) {
-    const phk_layer_t& Ly = T->layers[l];
-    const phk_layer_t& Gy = GT->layers[l];
-    const LayerSave& S = sv[l];
-    const int inner = Ly.ff.inner;
-    // feed forward: x4 = x3 + geglu(LN(x3) W1^T) W2^T
-    PHK_TRY(dgrad_p(prec, tc, dx, Ly.ff.w2, dg, R, D, inner, 0, s));
-    PHK_TRY(wgrad_p(prec, tc, dx, S.g, (float*)Gy.ff.w2, R, D, inner, s));
-    PHK_KERNEL_LAUNCH(geglu_bwd_kernel, dim3(ew_grid(R * inner)), dim3(256), (size_t)(0), st, S.h, dg, dh, R, inner, site(ff_p, l, 2));
-    PHK_LAUNCH_CHECK();
-    PHK_TRY(wgrad_p(prec, tc, dh, S.xn3, (float*)Gy.ff.w1, R, 2 * inner, D, s));
-    PHK_TRY(dgrad_p(prec, tc, dh, Ly.ff.w1, dtmp, R, 2 * inner, D, 0, s));
-    PHK_TRY(ln_backward(S.x3, Ly.ff.ln_g, dtmp, dx, 1, (float*)Gy.ff.ln_g, (float*)Gy.ff.ln_b, stats, R, D, st));
-    // cross attention: x3 = x2 + attn(LN(x2) Wq^T, LN_ctx(context) Wkv^T) Wo^T
-    if (S.o2) {
-      const phk_attn_t& Cx = Ly.cross_attn;
-      const phk_attn_t& Gx = Gy.cross_attn;
-      const int dc = Cx.dim_context;
-      PHK_REQUIRE(Cx.num_null_kv <= 8, PHK_E_UNSUPPORTED, "maskgit_train_step: more than 8 null key/values");
-      PHK_TRY(dgrad_p(prec, tc, dx, Cx.wo, dob, R, D, I, 0, s));
-      PHK_TRY(wgrad_p(prec, tc, dx, S.o2, (float*)Gx.wo, R, D, I, s));
-      const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
-      PHK_TRY(attention_backward(S.q2, S.ckv, Cx, Gx, nullptr, text_mask, dob, dq, dckv, nullptr, g2, asc, st, prec == PHK_PREC_BF16,
-                                 site(attn_p, l, 1)));
-      PHK_TRY(wgrad_p(prec, tc, dq, S.xn2, (float*)Gx.wq, R, I, D, s));
-      PHK_TRY(dgrad_p(prec, tc, dq, Cx.wq, dtmp, R, I, D, 0, s));
-      PHK_TRY(ln_backward(S.x2, Cx.norm_g, dtmp, dx, 1, (float*)Gx.norm_g, nullptr, stats, R, D, st));
-      PHK_TRY(wgrad_p(prec, tc, dckv, S.ctxn, (float*)Gx.wkv, CR, 2 * I, dc, s));
-      PHK_TRY(dgrad_p(prec, tc, dckv, Cx.wkv, dctxn, CR, 2 * I, dc, 0, s));
-      PHK_TRY(ln_backward(context, Cx.ctx_g, dctxn, nullptr, 0, (float*)Gx.ctx_g, nullptr, stats, CR, dc, st));
+}
+// out[i] += a[i] + a[half + i]: the context gradient of both halves into the caller's
+__global__ void add_halves_kernel(const float* __restrict__ a, float* __restrict__ out, int64_t half) {
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < half; i += (int64_t)gridDim.x * blockDim.x)
+    out[i] += a[i] + a[half + i];
+}
+
+// pair inputs of the CFG recompute: ids, video mask and context twice, the text mask then zeros
+int64_t pair_input_floats(int64_t R, int64_t CR, int64_t dc) {
+  return 2 * R * 2 + (2 * R + 3) / 4 + (2 * CR + 3) / 4 + 2 * CR * dc + 4 * 64;
+}
+
+int64_t context_width(const phk_transformer_t* T) {
+  int64_t dc = 0;
+  for (int l = 0; l < T->depth; ++l)
+    if (T->layers[l].has_cross && T->layers[l].cross_attn.dim_context > dc) dc = T->layers[l].cross_attn.dim_context;
+  return dc;
+}
+
+}  // namespace
+}  // namespace phk
+
+extern "C" int64_t phk_maskgit_backward_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L,
+                                                        int32_t cfg_pair, int32_t head_kind, int32_t prec) {
+  if (!m || b <= 0 || n <= 0 || L < 0 || !m->transformer.layers) return -1;
+  if (head_kind != PHK_HEAD_LOGITS && head_kind != PHK_HEAD_EMBEDS && head_kind != PHK_HEAD_SCORE) return -1;
+  const bool pair = cfg_pair && L > 0;
+  const int32_t B = pair ? 2 * b : b;
+  const int64_t Rh = (int64_t)b * n, CRh = (int64_t)b * L, dc = context_width(&m->transformer);
+  int64_t head = 64;
+  if (pair) head += Rh * m->dim + pair_input_floats(Rh, CRh, dc) + 2 * CRh * dc;  // mixed embeddings; inputs; d context
+  return step_workspace_bytes(m, B, n, L, head, head_kind == PHK_HEAD_LOGITS, prec);
+}
+
+// See include/phk.h.
+extern "C" int phk_maskgit_backward(const phk_maskgit_t* m, const phk_maskgit_t* grads, const int64_t* ids, int32_t b,
+                                    int32_t n, int32_t pt, int32_t ph, int32_t pw, const float* context, int32_t L,
+                                    const uint8_t* text_mask, const uint8_t* video_mask, int32_t cfg_pair,
+                                    float cond_scale, int32_t head_kind, const float* upstream, float* d_context,
+                                    void* workspace, int64_t workspace_bytes, int32_t prec, phk_stream_t s) {
+  PHK_REQUIRE(m && grads && ids && upstream && workspace, PHK_E_ARG, "maskgit_backward: null pointer");
+  PHK_REQUIRE(b > 0 && n > 0 && (int64_t)pt * ph * pw == n, PHK_E_SHAPE, "video patch shape must cover the token sequence");
+  PHK_REQUIRE(n <= m->max_seq_len, PHK_E_SHAPE,
+              "the video token sequence length is greater than max_seq_len (phenaki_pytorch.py:196)");
+  PHK_REQUIRE(head_kind == PHK_HEAD_LOGITS || head_kind == PHK_HEAD_EMBEDS || head_kind == PHK_HEAD_SCORE, PHK_E_ARG,
+              "maskgit_backward: unknown head kind");
+  PHK_REQUIRE(head_kind != PHK_HEAD_LOGITS || !m->is_critic, PHK_E_ARG, "maskgit_backward: a TokenCritic has no logits head");
+  PHK_REQUIRE(!context || (text_mask && L > 0), PHK_E_ARG, "maskgit_backward: context without text mask / length");
+  PHK_REQUIRE(!d_context || context, PHK_E_ARG, "maskgit_backward: d_context without a context");
+  PHK_REQUIRE(prec == PHK_PREC_F32 || prec == PHK_PREC_BF16, PHK_E_ARG, "maskgit_backward: unknown precision mode");
+  if (!context) L = 0;
+  PHK_REQUIRE(workspace_bytes >= phk_maskgit_backward_workspace_bytes(m, b, n, L, cfg_pair, head_kind, prec), PHK_E_WORKSPACE,
+              "maskgit_backward: workspace too small");
+  const phk_transformer_t* T = &m->transformer;
+  const phk_transformer_t* GT = &grads->transformer;
+  PHK_REQUIRE(T->layers && GT->layers && T->depth > 0 && GT->depth == T->depth && !T->causal, PHK_E_ARG,
+              "maskgit_backward: transformer table / gradient table mismatch");
+  PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "maskgit_backward: dim must be a multiple of 4");
+  const int64_t dc = context_width(T);
+  for (int l = 0; l < T->depth; ++l)
+    PHK_REQUIRE(!context || !T->layers[l].has_cross || T->layers[l].cross_attn.dim_context == dc, PHK_E_UNSUPPORTED,
+                "maskgit_backward: cross-attention layers of different context widths");
+  // without a context both halves of a pair are the same function of the weights: out = cond, no pair to differentiate
+  const bool pair = cfg_pair && context;
+  const float sc = pair ? cond_scale : 1.0f;
+  cudaStream_t st = to_stream(s);
+  const int64_t Rh = (int64_t)b * n, CRh = (int64_t)b * L;
+  Step S;
+  S.m = m; S.grads = grads; S.ids = ids; S.b = pair ? 2 * b : b; S.n = n; S.pt = pt; S.ph = ph; S.pw = pw; S.L = L;
+  S.context = context; S.text_mask = text_mask; S.video_mask = video_mask; S.prec = prec; S.s = s;
+  S.ar = Arena{(char*)workspace, workspace_bytes, 0};
+  Arena& ar = S.ar;
+  float* ctx_grad = d_context;  // where stage 3 accumulates d/d(context): both halves of a pair, summed below
+  if (pair) {  // the 2b-sequence inputs of the forward's pair (phk_maskgit_forward, cfg_pair = 1)
+    int64_t* ids2 = reinterpret_cast<int64_t*>(ar.f(2 * Rh * 2));
+    uint8_t* vm2 = video_mask ? reinterpret_cast<uint8_t*>(ar.f((2 * Rh + 3) / 4)) : nullptr;
+    uint8_t* tm2 = reinterpret_cast<uint8_t*>(ar.f((2 * CRh + 3) / 4));
+    float* ctx2 = ar.f(2 * CRh * dc);
+    PHK_REQUIRE(ids2 && (!video_mask || vm2) && tm2 && ctx2, PHK_E_WORKSPACE, "maskgit_backward: workspace too small (pair)");
+    for (int h = 0; h < 2; ++h) {
+      PHK_CUDA(cudaMemcpyAsync(ids2 + h * Rh, ids, Rh * 8, cudaMemcpyDeviceToDevice, st));
+      if (video_mask) PHK_CUDA(cudaMemcpyAsync(vm2 + h * Rh, video_mask, Rh, cudaMemcpyDeviceToDevice, st));
+      PHK_CUDA(cudaMemcpyAsync(ctx2 + h * CRh * dc, context, CRh * dc * 4, cudaMemcpyDeviceToDevice, st));
     }
-    // self attention: x2 = x1 + attn(LN(x1) Wq^T, x1 Wkv^T) Wo^T
-    {
-      const phk_attn_t& A = Ly.self_attn;
-      const phk_attn_t& GA = Gy.self_attn;
-      PHK_TRY(dgrad_p(prec, tc, dx, A.wo, dob, R, D, I, 0, s));
-      PHK_TRY(wgrad_p(prec, tc, dx, S.o1, (float*)GA.wo, R, D, I, s));
-      const AttnBwdGeom g1{b, H, n, n, 0, DH};
-      PHK_TRY(attention_backward(S.q1, S.kv1, A, GA, bias, video_mask, dob, dq, dkv, dbias, g1, asc, st, prec == PHK_PREC_BF16,
-                                 site(attn_p, l, 0)));
-      PHK_TRY(wgrad_p(prec, tc, dq, S.xn1, (float*)GA.wq, R, I, D, s));
-      PHK_TRY(wgrad_p(prec, tc, dkv, S.x1, (float*)GA.wkv, R, 2 * I, D, s));
-      PHK_TRY(dgrad_p(prec, tc, dq, A.wq, dtmp, R, I, D, 0, s));
-      PHK_TRY(ln_backward(S.x1, A.norm_g, dtmp, dx, 1, (float*)GA.norm_g, nullptr, stats, R, D, st));
-      PHK_TRY(dgrad_p(prec, tc, dkv, A.wkv, dx, R, 2 * I, D, 1, s));  // the raw-x path of k, v
+    PHK_CUDA(cudaMemcpyAsync(tm2, text_mask, CRh, cudaMemcpyDeviceToDevice, st));
+    PHK_CUDA(cudaMemsetAsync(tm2 + CRh, 0, CRh, st));  // the null half: every text token masked out
+    S.ids = ids2; S.video_mask = vm2; S.text_mask = tm2; S.context = ctx2;
+    if (d_context) {
+      ctx_grad = ar.f(2 * CRh * dc);
+      PHK_REQUIRE(ctx_grad, PHK_E_WORKSPACE, "maskgit_backward: workspace too small (context gradient)");
+      PHK_CUDA(cudaMemsetAsync(ctx_grad, 0, 2 * CRh * dc * 4, st));
     }
-    // PEG: x1 = x0 + conv(x0) + b
-    PHK_TRY(colsum(dx, R, D, D, (float*)Gy.peg.b, st));
-    PHK_REQUIRE(D <= 128 * PEG_DW_MAXJ, PHK_E_UNSUPPORTED, "maskgit_train_step: dim > 1024");
-    PHK_KERNEL_LAUNCH(peg_bwd_dw_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, S.x0, dx, (float*)Gy.peg.w, R, pt, ph, pw, D, Ly.peg.causal ? 2 : 1);
-    PHK_LAUNCH_CHECK();
-    PHK_KERNEL_LAUNCH(peg_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, S.x0, Ly.peg.w, dx, dx_alt, pt, ph, pw, D, Ly.peg.causal ? 2 : 1);
-    PHK_LAUNCH_CHECK();
-    float* t = dx; dx = dx_alt; dx_alt = t;
-    // this layer's parameter gradients are final -- except, with a context, the cross-attention's context_norm / to_kv
-    // share nothing with other layers either; the position-bias gradient (dbias, all layers) is finished below
-    PHK_TRY(progress_mark(prog, nprog, 1 + (T->depth - 1 - l), st));
   }
-  // ---------------------------------------------------------------- embeddings, position-bias MLP
-  PHK_KERNEL_LAUNCH(embed_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, ids_in, dx, (float*)grads->token_emb, (float*)grads->pos_emb, n, D,
-                                               m->is_critic ? 1.0f : m->shrink_alpha, m->num_tokens + 1);
-  PHK_LAUNCH_CHECK();
-  if (m->has_bias) {
-    float* csc = ar.f(cpb_bwd_scratch_floats(m->pos_bias, pt, ph, pw));
-    PHK_REQUIRE(csc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (position-bias backward)");
-    PHK_TRY(cpb_backward(m->pos_bias, grads->pos_bias, dbias, pt, ph, pw, csc, st));
+  step_init(S);
+  const int D = S.D, V = m->num_tokens;
+
+  // ---------------------------------------------------------------- stage 1: the forward, saving activations
+  PHK_TRY(step_forward(S, head_kind == PHK_HEAD_LOGITS));
+
+  // ---------------------------------------------------------------- stage 2: upstream gradient -> d emb
+  PHK_REQUIRE(step_gradient_buffers(S) == 0 && step_stats_buffer(S) == 0, PHK_E_WORKSPACE,
+              "maskgit_backward: workspace too small (bwd)");
+  const float* emb_head = S.emb;  // what the head multiplied: the embeddings, or the pair's mix of both halves
+  if (pair && head_kind != PHK_HEAD_EMBEDS) {
+    float* mix = ar.f(Rh * D);
+    PHK_REQUIRE(mix, PHK_E_WORKSPACE, "maskgit_backward: workspace too small (mixed embeddings)");
+    PHK_KERNEL_LAUNCH(cfg_mix_kernel, dim3(ew_grid(Rh * D)), dim3(256), (size_t)(0), st, S.emb, S.emb + Rh * D, sc, mix, Rh * D);
+    PHK_LAUNCH_CHECK();
+    emb_head = mix;
   }
-  PHK_TRY(progress_mark(prog, nprog, T->depth + 1, st));
+  if (head_kind == PHK_HEAD_LOGITS) {  // dlogits [b n, V]
+    PHK_TRY(wgrad_p(prec, S.tc, upstream, emb_head, (float*)grads->head_w, Rh, V, D, s));
+    PHK_TRY(colsum(upstream, Rh, V, V, (float*)grads->head_b, st));
+    PHK_TRY(dgrad_p(prec, S.tc, upstream, m->head_w, S.dtmp, Rh, V, D, 0, s));
+  } else if (head_kind == PHK_HEAD_SCORE) {  // dscore [b n]: the BCE head's branch of the train step without the BCE
+    PHK_TRY(wgrad(upstream, emb_head, (float*)grads->head_w, Rh, 1, D, st));
+    PHK_TRY(colsum(upstream, Rh, 1, 1, (float*)grads->head_b, st));
+    PHK_KERNEL_LAUNCH(outer_kernel, dim3(ew_grid(Rh * D)), dim3(256), (size_t)(0), st, upstream, m->head_w, S.dtmp, Rh, D);
+    PHK_LAUNCH_CHECK();
+  } else {  // demb [b n, dim]: straight into the norm_out backward
+    PHK_CUDA(cudaMemcpyAsync(S.dtmp, upstream, Rh * D * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  if (pair) {
+    PHK_KERNEL_LAUNCH(cfg_split_kernel, dim3(ew_grid(Rh * D)), dim3(256), (size_t)(0), st, S.dtmp, sc, Rh * D);
+    PHK_LAUNCH_CHECK();
+  }
+
+  // ---------------------------------------------------------------- stage 3: transformer and embedding backward
+  PHK_TRY(step_backward(S, ctx_grad, nullptr, 0));
+  if (pair && d_context) {
+    PHK_KERNEL_LAUNCH(add_halves_kernel, dim3(ew_grid(CRh * dc)), dim3(256), (size_t)(0), st, ctx_grad, d_context, CRh * dc);
+    PHK_LAUNCH_CHECK();
+  }
   return 0;
 }

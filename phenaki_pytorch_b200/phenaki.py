@@ -384,6 +384,73 @@ class _TokenTransformer(nn.Module):
         gk.reduced = torch.cuda.Event()
         gk.reduced.record(side)
 
+    def _differentiable(self, run, owner, ids, patch_shape, *, context, text_mask, video_mask, cond_scale, head_kind,
+                        head=None):
+        """Returns ``run()`` -- the forward exactly as it runs under ``torch.no_grad`` -- and, when autograd wants a
+        gradient of it (grad mode on, and a parameter of ``owner`` or ``context`` requires grad), connects the result to
+        the hand-written backward (phk_maskgit_backward) through ``_ForwardBackwardFn``.
+        ids (b, n), patch_shape, context (the text embeddings, or None when the network ignores them), text_mask (after
+        the cond_drop_prob draw), video_mask, cond_scale (!= 1: the CFG pair) and head_kind (_lib.HEAD_*) describe
+        the call; ``head``: an nn.Linear(dim, 1) that replaces the network's own head (SelfCritic.to_pred)."""
+        params = list(owner.parameters())
+        if not torch.is_grad_enabled() or not (any(p.requires_grad for p in params)
+                                               or (context is not None and context.requires_grad)):
+            return run()
+        spec = dict(net=self, owner=owner, head=head, patch_shape=tuple(int(v) for v in patch_shape),
+                    cond_scale=float(cond_scale), head_kind=head_kind, sig=weights_signature(owner))
+        return _ForwardBackwardFn.apply(run, spec, ids, text_mask if context is not None else None, video_mask,
+                                        context, *params)
+
+    def _backward_from(self, spec, upstream, ids, text_mask, video_mask, context, want_context_grad):
+        """phk_maskgit_backward for one ``_differentiable`` call: ([gradient or None per parameter of the owner],
+        d context or None).  The gradients are copies: the flat bucket they were accumulated in is free again on
+        return."""
+        lib = L.lib()
+        owner, head, head_kind = spec["owner"], spec["head"], spec["head_kind"]
+        if weights_signature(owner) != spec["sig"]:
+            raise RuntimeError("a parameter of this module was modified or replaced between the forward and the backward: "
+                               "the backward recomputes the forward from the current weights, so it would differentiate "
+                               "another function")
+        ids = L.require_cuda(ids, "token ids", torch.int64)
+        b, n = ids.shape
+        dev = ids.device
+        with torch.cuda.device(dev):
+            table = self._table()
+            keep = Keep()
+            if head is not None:  # same body, another head (as in train_step)
+                table = L.MaskgitT.from_buffer_copy(table)
+                table.head_w, table.head_b, table.head_w_h = keep.t(head.weight), keep.t(head.bias), None
+            has_cross = context is not None
+            ctx_len = context.shape[1] if has_cross else 0
+            if has_cross:
+                context = L.require_cuda(context.detach(), "text embeds", torch.float32)
+                text_mask = L.require_cuda(text_mask.to(torch.uint8), "text mask")
+            if video_mask is not None:
+                video_mask = L.require_cuda(video_mask.to(torch.uint8), "video mask")
+            upstream = L.require_cuda(upstream.to(torch.float32), "upstream gradient")
+            cfg = spec["cond_scale"] != 1
+            prec = L.PREC_BF16 if self.precision == L.PREC_BF16 else L.PREC_F32  # split-bf16 is an inference mode
+            pt, ph, pw = spec["patch_shape"]
+            gtable, gk = self._grad_table(has_cross, owner=owner, head=head)
+            try:
+                nbytes = lib.phk_maskgit_backward_workspace_bytes(C.byref(table), b, n, ctx_len, int(cfg), head_kind, prec)
+                ws = self._ws.get(nbytes, dev)
+                d_context = torch.zeros_like(context) if has_cross and want_context_grad else None
+                L.check(lib.phk_maskgit_backward(C.byref(table), C.byref(gtable), L.ptr(ids), b, n, pt, ph, pw,
+                                                 L.ptr(context), ctx_len, L.ptr(text_mask), L.ptr(video_mask), int(cfg),
+                                                 spec["cond_scale"], head_kind, L.ptr(upstream), L.ptr(d_context),
+                                                 L.ptr(ws), ws.numel(), prec, L.stream_ptr()),
+                        "phk_maskgit_backward")
+                # the embeddings head leaves the network's own head out of the graph, as the reference's autograd does
+                unused = set(self.to_logits.parameters()) if head_kind == L.HEAD_EMBEDS else set()
+                grads = []
+                for p in owner.parameters():
+                    g = gk.grad_of(p)
+                    grads.append(None if g is None or p in unused else g.clone())
+            finally:
+                gk.busy = False
+        return grads, d_context
+
     def _check_ids(self, x):
         """nn.Embedding raises on an id outside the table (phenaki_pytorch.py:194); the kernels only clamp.  One device
         sync, paid at the public forward entries only (the sampling loop produces its ids itself)."""
@@ -435,26 +502,39 @@ class MaskGit(_TokenTransformer):
 
     def forward(self, x, cond_drop_prob=0.0, text_mask=None, video_mask=None, video_patch_shape=None,
                 return_embeds=False, context=None, **kwargs):
+        """phenaki_pytorch.py:163-213: logits (b, n, V), or the embeddings (b, n, dim) with ``return_embeds``.
+        Differentiable with respect to the parameters and ``context`` (``_ForwardBackwardFn``: the backward recomputes
+        the forward with saved activations, so it costs one training forward plus the backward).  Training-mode
+        dropout is not applied, here or in the backward (DESIGN.md section 8)."""
         assert x.ndim in {2, 4}, "video token ids must be of shape (batch, seq) or (batch, frame, height, width)"
         x, shape, ctx_kv, ctx_len, text_mask = self._prepare(x, text_mask, video_patch_shape, context, cond_drop_prob)
-        return self._run(x, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask, video_mask=video_mask,
-                         return_embeds=return_embeds)
+        run = partial(self._run, x, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask, video_mask=video_mask,
+                      return_embeds=return_embeds)
+        return self._differentiable(run, self, x, shape, context=context if ctx_kv is not None else None,
+                                    text_mask=text_mask, video_mask=video_mask, cond_scale=1.0,
+                                    head_kind=L.HEAD_EMBEDS if return_embeds else L.HEAD_LOGITS)
 
     def forward_with_cond_scale(self, x, *, cond_scale=3, text_mask=None, video_mask=None, video_patch_shape=None,
                                 context=None, return_embeds=False, **kwargs):
         """phenaki_pytorch.py:149-161.  Both passes run as ONE batch of 2b sequences (the second half sees
-        an all-False text mask) and are combined by phk_cfg_combine."""
+        an all-False text mask) and are combined by phk_cfg_combine.  Differentiable as ``forward`` is."""
         if cond_scale == 1:
             return self.forward(x, cond_drop_prob=0.0, text_mask=text_mask, video_mask=video_mask,
                                 video_patch_shape=video_patch_shape, context=context, return_embeds=return_embeds)
         x, shape, ctx_kv, ctx_len, text_mask = self._prepare(x, text_mask, video_patch_shape, context, 0.0)
-        both = self._run(x, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask, video_mask=video_mask,
-                         cfg_pair=True, return_embeds=return_embeds)
-        b = x.shape[0]
-        out = torch.empty_like(both[:b])
-        L.check(L.lib().phk_cfg_combine(L.ptr(both[:b]), L.ptr(both[b:]), float(cond_scale), L.ptr(out),
-                                        out.numel(), L.stream_ptr()), "phk_cfg_combine")
-        return out
+
+        def run():
+            both = self._run(x, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask, video_mask=video_mask,
+                             cfg_pair=True, return_embeds=return_embeds)
+            b = x.shape[0]
+            out = torch.empty_like(both[:b])
+            L.check(L.lib().phk_cfg_combine(L.ptr(both[:b]), L.ptr(both[b:]), float(cond_scale), L.ptr(out),
+                                            out.numel(), L.stream_ptr()), "phk_cfg_combine")
+            return out
+
+        return self._differentiable(run, self, x, shape, context=context if ctx_kv is not None else None,
+                                    text_mask=text_mask, video_mask=video_mask, cond_scale=cond_scale,
+                                    head_kind=L.HEAD_EMBEDS if return_embeds else L.HEAD_LOGITS)
 
 
 class TokenCritic(_TokenTransformer):
@@ -483,14 +563,22 @@ class TokenCritic(_TokenTransformer):
 
     def forward(self, x, text_mask=None, cond_drop_prob=None, context=None, video_mask=None,
                 video_patch_shape=None, **kwargs):
+        """phenaki_pytorch.py:265-302: scores (b, n).  Differentiable as MaskGit.forward is (recompute in backward, no
+        dropout)."""
         shape = tuple(video_patch_shape) if video_patch_shape is not None else tuple(x.shape[1:])
         x = x.reshape(x.shape[0], -1)
         if context is not None and cond_drop_prob is None:
             raise TypeError("cond_drop_prob must be given when a context is passed (phenaki_pytorch.py:286)")
         x, shape, ctx_kv, ctx_len, text_mask = self._prepare(x, text_mask, shape, context, cond_drop_prob)
-        emb = self._run(x, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask, video_mask=video_mask)
-        b, n = x.shape
-        return self._scores(emb, None, 1.0, b * n).reshape(b, n)
+
+        def run():
+            emb = self._run(x, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask, video_mask=video_mask)
+            b, n = x.shape
+            return self._scores(emb, None, 1.0, b * n).reshape(b, n)
+
+        return self._differentiable(run, self, x, shape, context=context if ctx_kv is not None else None,
+                                    text_mask=text_mask, video_mask=video_mask, cond_scale=1.0,
+                                    head_kind=L.HEAD_SCORE)
 
     def forward_with_cond_scale(self, x, *, cond_scale=3, text_mask=None, context=None, video_mask=None,
                                 video_patch_shape=None, **kwargs):
@@ -500,10 +588,16 @@ class TokenCritic(_TokenTransformer):
         shape = tuple(video_patch_shape) if video_patch_shape is not None else tuple(x.shape[1:])
         x = x.reshape(x.shape[0], -1)
         x, shape, ctx_kv, ctx_len, text_mask = self._prepare(x, text_mask, shape, context, 0.0)
-        both = self._run(x, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask, video_mask=video_mask,
-                         cfg_pair=True)
-        b, n = x.shape
-        return self._scores(both[:b], both[b:], cond_scale, b * n).reshape(b, n)
+
+        def run():
+            both = self._run(x, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask, video_mask=video_mask,
+                             cfg_pair=True)
+            b, n = x.shape
+            return self._scores(both[:b], both[b:], cond_scale, b * n).reshape(b, n)
+
+        return self._differentiable(run, self, x, shape, context=context if ctx_kv is not None else None,
+                                    text_mask=text_mask, video_mask=video_mask, cond_scale=cond_scale,
+                                    head_kind=L.HEAD_SCORE)
 
 
 class SelfCritic(nn.Module):
@@ -526,9 +620,30 @@ class SelfCritic(nn.Module):
         return out
 
     def forward(self, x, *args, **kwargs):
-        emb = self.maskgit(x, *args, return_embeds=True, **kwargs)
-        b, n = emb.shape[:2]
-        return self._head(emb, None, 1.0, b * n).reshape(b, n)
+        """phenaki_pytorch.py:334-336: scores (b, n).  Differentiable as MaskGit.forward is (recompute in backward, no
+        dropout); ``to_pred`` and the MaskGit body get gradients, MaskGit's ``to_logits`` none."""
+        mg = self.maskgit
+        kw = dict(zip(("cond_drop_prob", "text_mask", "video_mask", "video_patch_shape"), args), **kwargs)
+        context = kw.get("context")
+        if not torch.is_grad_enabled() or not (any(p.requires_grad for p in self.parameters())
+                                               or (context is not None and context.requires_grad)):
+            emb = self.maskgit(x, *args, return_embeds=True, **kwargs)
+            b, n = emb.shape[:2]
+            return self._head(emb, None, 1.0, b * n).reshape(b, n)
+        # differentiable: MaskGit.forward(return_embeds=True) and the head as one call of the hand-written backward
+        assert x.ndim in {2, 4}, "video token ids must be of shape (batch, seq) or (batch, frame, height, width)"
+        xx, shape, ctx_kv, ctx_len, text_mask = mg._prepare(x, kw.get("text_mask"), kw.get("video_patch_shape"), context,
+                                                            kw.get("cond_drop_prob", 0.0))
+
+        def run():
+            emb = mg._run(xx, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask,
+                          video_mask=kw.get("video_mask"), return_embeds=True)
+            b, n = emb.shape[:2]
+            return self._head(emb, None, 1.0, b * n).reshape(b, n)
+
+        return mg._differentiable(run, self, xx, shape, context=context if ctx_kv is not None else None,
+                                  text_mask=text_mask, video_mask=kw.get("video_mask"), cond_scale=1.0,
+                                  head_kind=L.HEAD_SCORE, head=self.to_pred[0])
 
     def train_step(self, ids_in, patch_shape, *, labels, **kw):
         """BCE training step of the self critic: the MaskGit body with ``to_pred`` as its head; the gradient bucket
@@ -541,10 +656,17 @@ class SelfCritic(nn.Module):
         mg = self.maskgit
         xx, shape, ctx_kv, ctx_len, text_mask = mg._prepare(x, kwargs.get("text_mask"), kwargs.get("video_patch_shape"),
                                                             kwargs.get("context"), 0.0)
-        both = mg._run(xx, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask,
-                       video_mask=kwargs.get("video_mask"), cfg_pair=True, return_embeds=True)
-        b, n = xx.shape
-        return self._head(both[:b], both[b:], cond_scale, b * n).reshape(b, n)
+
+        def run():
+            both = mg._run(xx, shape, ctx_kv=ctx_kv, ctx_len=ctx_len, text_mask=text_mask,
+                           video_mask=kwargs.get("video_mask"), cfg_pair=True, return_embeds=True)
+            b, n = xx.shape
+            return self._head(both[:b], both[b:], cond_scale, b * n).reshape(b, n)
+
+        context = kwargs.get("context")
+        return mg._differentiable(run, self, xx, shape, context=context if ctx_kv is not None else None,
+                                  text_mask=text_mask, video_mask=kwargs.get("video_mask"), cond_scale=cond_scale,
+                                  head_kind=L.HEAD_SCORE, head=self.to_pred[0])
 
 
 class _TrainStepFn(torch.autograd.Function):
@@ -570,6 +692,32 @@ class _TrainStepFn(torch.autograd.Function):
         out = (None, None, None, *[None if g is None else g * gout for g in ctx.grads])  # copies: the bucket is free again
         ctx.keep.busy = False
         return out
+
+
+class _ForwardBackwardFn(torch.autograd.Function):
+    """Makes the MaskGit / TokenCritic / SelfCritic forwards differentiable.  The forward runs the library's inference
+    forward unchanged (same launches, same values) and keeps only the call's inputs.  The backward recomputes the forward
+    with saved activations inside phk_maskgit_backward, as activation checkpointing does, and runs the hand-written
+    backward from the upstream gradient: a backward costs one training forward plus the backward of the training step.
+    Training-mode dropout is not applied by these forwards (DESIGN.md section 8), so the backward applies none either:
+    it differentiates the function the forward returned."""
+
+    @staticmethod
+    def forward(ctx, run, spec, ids, text_mask, video_mask, context, *params):
+        ctx.spec = spec
+        ctx.save_for_backward(ids, text_mask, video_mask, None if context is None else context.detach())
+        return run()
+
+    @staticmethod
+    def backward(ctx, gout):
+        if torch.is_grad_enabled():
+            raise RuntimeError("MaskGit / TokenCritic / SelfCritic forwards do not support create_graph=True: their "
+                               "backward is hand-written CUDA and builds no graph of its own")
+        ids, text_mask, video_mask, context = ctx.saved_tensors
+        spec = ctx.spec
+        grads, d_context = spec["net"]._backward_from(spec, gout, ids, text_mask, video_mask, context,
+                                                      ctx.needs_input_grad[5])
+        return (None, None, None, None, None, d_context, *grads)
 
 
 def get_mask_subset_with_prob(mask, prob, u=None):
