@@ -420,6 +420,23 @@ int phk_cvivit_decode(const phk_cvivit_dec_t* m, const int64_t* ids, const float
                       const float* spatial_bias, float* tap_codes, float* tap_temporal,
                       float* tap_spatial, phk_stream_t s);
 
+/* Backward of phk_cvivit_decode from a gradient the caller supplies: what `video = CViViT.decode(tokens);
+ * video.backward(dvideo)` (or the same through decode_from_codebook_indices(ids)) computes under torch autograd (cvivit.py:437-443, 476-516).
+ * The forward is recomputed with saved activations (activation checkpointing), then differentiated through
+ * to_pixels / to_pixels_first_frame, the spatial stack (and the spatial_rel_pos_bias MLP through its 2-D bias), the
+ * causal ALiBi temporal stack (PEG with the reference's raw-reshape layout) and, for ids, LFQ's project_out.
+ *   ids / tokens / B / Tp  the arguments of the phk_cvivit_decode call being differentiated (ids needs LFQ, codebook_bits > 0)
+ *   grads    a table of the SAME layout as `m` whose float pointers address ZERO-FILLED gradient buffers: the dec_*
+ *            transformers, spatial_bias, px_first_* / px_*, and vq_out_* when ids are given; every gradient is
+ *            ACCUMULATED.  With Tp == 1 the px_* gradients stay zero (the reference runs to_pixels on an empty batch).
+ *   dvideo   fp32 (B, C, 1 + (Tp-1)*pt, H, W), d out / d video
+ *   dtokens  NULL, or fp32 [B*Tp*H'*W', dim] (float-token decode only): receives d out / d tokens (written, not added)
+ * prec: PHK_PREC_F32 (fp32 products) or PHK_PREC_BF16 (the training step's bf16 products); no dropout is applied. */
+int64_t phk_cvivit_decode_backward_workspace_bytes(const phk_cvivit_dec_t* m, int32_t B, int32_t Tp, int32_t prec);
+int phk_cvivit_decode_backward(const phk_cvivit_dec_t* m, const phk_cvivit_dec_t* grads, const int64_t* ids,
+                               const float* tokens, int32_t B, int32_t Tp, const float* dvideo, float* dtokens,
+                               void* workspace, int64_t workspace_bytes, int32_t prec, phk_stream_t s);
+
 /* context_norm + to_kv of every cross-attention layer (attention.py:137-144).  Depends only on
  * the text embedding, so Phenaki.sample computes it once per call instead of once per forward.
  * context (b,L,dim_context) fp32; out_kv [depth, b*L, 2*heads*dim_head] fp32;

@@ -182,9 +182,12 @@ PROTOTYPES = {
     "phk_maskgit_backward_workspace_bytes": [C.POINTER(MaskgitT), i32, i32, i32, i32, i32, i32],
     "phk_maskgit_backward": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, i32,
                              f32, i32, vp, vp, vp, i64, i32, vp],
+    "phk_cvivit_decode_backward_workspace_bytes": [C.POINTER(CvivitDecT), i32, i32, i32],
+    "phk_cvivit_decode_backward": [C.POINTER(CvivitDecT), C.POINTER(CvivitDecT), vp, vp, i32, i32, vp, vp, vp, i64, i32,
+                                   vp],
 }
 _RESTYPES = {"phk_attention_tc_scratch_bytes": i64, "phk_head_sample_scratch_bytes": i64,
-             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_maskgit_train_dropout_counters": i64, "phk_maskgit_backward_workspace_bytes": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
+             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_maskgit_train_dropout_counters": i64, "phk_maskgit_backward_workspace_bytes": i64, "phk_cvivit_decode_backward_workspace_bytes": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
              "phk_cvivit_workspace_bytes": i64, "phk_cvivit_decode_workspace_bytes": i64, "phk_maskgit_workspace_bytes": i64}
 
 FAMILIES = ["patchify_ln", "layernorm", "gemm_f32", "gemm_bf16", "attention", "peg", "geglu", "lfq", "embed",

@@ -14,11 +14,13 @@
 // against the reference there.  In bf16 mode the products run on the tensor-core GEMM instead (see below).
 // With dropout (phk_dropout_t) the masks are regenerated from Philox counters wherever they are needed, never stored.
 // Checked against the reference's gradients on the CPU by tests/cuda_emu (this very source, g++-compiled) and on the GPU
-// by tests/test_gpu_train.py.
+// by tests/test_gpu_train.py.  The same layer code differentiates the C-ViViT decoder (phk_cvivit_decode_backward, at the
+// end of this file).
 #include "phk_common.cuh"
 // the kernels of this file are ordinary stream-ordered launches (they do not use programmatic dependent launch)
 #define PHK_KERNEL_LAUNCH(kernel, grid, block, smem, st, ...) PHK_CUDA(launch_plain(kernel, grid, block, smem, st, __VA_ARGS__))
 #include <cstring>
+#include <memory>
 #include <new>
 
 namespace phk {
@@ -1273,22 +1275,206 @@ void step_init(Step& S) {
   S.R = (int64_t)S.b * S.n; S.CR = (int64_t)S.b * S.L;
 }
 
+// ------------------------------------------------------------------------------------------------------------------
+// One transformer layer (attention.py:311-330): forward keeping its activations, and backward.  Shared by every stack
+// whose sequences are runs of n contiguous rows: MaskGit / TokenCritic (b videos of n tokens, PEG over (pt, ph, pw),
+// cross-attention to the text) and the two stacks of the C-ViViT decoder (phk_cvivit_decode_backward).
+// ------------------------------------------------------------------------------------------------------------------
+struct LayerCall {
+  const phk_transformer_t* T = nullptr;    // weights
+  const phk_transformer_t* GT = nullptr;   // gradient table of the same layout
+  int b = 0, n = 0;                        // b sequences of n contiguous rows
+  int pegB = 0, pegT = 0, pegH = 0, pegW = 0;  // video shape the layers' PEG runs over (layout 0 on the rows)
+  const float* bias = nullptr;             // self-attention additive bias [H, n, n], or NULL
+  float* dbias = nullptr;                  // its gradient, accumulated (NULL: the bias is a constant)
+  const uint8_t* key_mask = nullptr;       // self-attention key mask [b, n], or NULL
+  const float* context = nullptr;          // cross-attention context [b, L, dim_context], or NULL
+  int L = 0;
+  const uint8_t* text_mask = nullptr;      // [b, L]
+  int prec = PHK_PREC_F32;
+  phk_stream_t s = nullptr;
+  cudaStream_t st = nullptr;
+  TcScratch tc{nullptr, nullptr, 0};
+  float* asc = nullptr;                    // attention scratch: attn_bwd_scratch_floats of the larger attention
+};
+
+// Gradient scratch of layer_backward: dtmp [R, D], dq [R, I], dkv [R, 2I], dob [R, I], dh [R, 2 inner], dg [R, inner],
+// dckv [CR, 2I] / dctxn [CR, dim_context] (cross-attention only), LayerNorm statistics [max(R, CR)]
+struct LayerGrads { float *dtmp, *dq, *dkv, *dob, *dh, *dg, *dckv, *dctxn; float2* stats; };
+
+// Layer l of c.T on x0 [R, D]: every activation the backward reads is kept in Sv, the output lands in *xout (fresh).
+int layer_forward(const LayerCall& c, int l, const float* x0, LayerSave& Sv, float** xout, Arena& ar,
+                  const DropSite& d_self, const DropSite& d_cross, const DropSite& d_ff) {
+  const phk_transformer_t* T = c.T;
+  const phk_layer_t& Ly = T->layers[l];
+  const int b = c.b, n = c.n, L = c.L;
+  const int D = T->dim, H = T->heads, DH = T->dim_head, I = H * DH;
+  const int64_t R = (int64_t)b * n, CR = (int64_t)b * L;
+  const int prec = c.prec;
+  const phk_stream_t s = c.s;
+  const cudaStream_t st = c.st;
+  const TcScratch& tc = c.tc;
+  std::memset(&Sv, 0, sizeof(Sv));
+  const int inner = Ly.ff.inner;
+  Sv.x0 = const_cast<float*>(x0);
+  Sv.x1 = Ly.has_peg ? ar.f(R * D) : Sv.x0;  // without PEG the self-attention reads x0
+  Sv.xn1 = ar.f(R * D); Sv.q1 = ar.f(R * I); Sv.kv1 = ar.f(R * 2 * I); Sv.o1 = ar.f(R * I);
+  Sv.x2 = ar.f(R * D); Sv.x3 = ar.f(R * D); Sv.xn3 = ar.f(R * D); Sv.h = ar.f(R * 2 * (int64_t)inner); Sv.g = ar.f(R * (int64_t)inner);
+  *xout = ar.f(R * D);
+  PHK_REQUIRE(Sv.x1 && Sv.xn1 && Sv.q1 && Sv.kv1 && Sv.o1 && Sv.x2 && Sv.x3 && Sv.xn3 && Sv.h && Sv.g && *xout, PHK_E_WORKSPACE,
+              "train: workspace too small (activations)");
+  // x1 = peg(x0) + x0
+  if (Ly.has_peg) {
+    PHK_REQUIRE((int64_t)c.pegB * c.pegT * c.pegH * c.pegW == R, PHK_E_SHAPE, "train: PEG shape does not cover the rows");
+    PHK_TRY(phk_peg3d(Sv.x0, Ly.peg.w, Ly.peg.b, Sv.x1, c.pegB, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal, 0, s));
+  }
+  // self attention: q from LN(x1), k/v from RAW x1 (attention.py:140-144)
+  const phk_attn_t& A = Ly.self_attn;
+  phk_attn_geom_t ag;
+  PHK_TRY(phk_layernorm(Sv.x1, A.norm_g, A.norm_b, Sv.xn1, nullptr, R, D, 0, 0, 0, 0, s));
+  PHK_TRY(linear_fwd(prec, tc, Sv.xn1, A.wq, Sv.q1, R, I, D, nullptr, nullptr, s));
+  PHK_TRY(linear_fwd(prec, tc, Sv.x1, A.wkv, Sv.kv1, R, 2 * I, D, nullptr, nullptr, s));
+  std::memset(&ag, 0, sizeof(ag));
+  ag.n_outer = b; ag.n_inner = 1; ag.n_q = n; ag.n_k = n; ag.heads = H; ag.dim_head = DH; ag.num_null_kv = A.num_null_kv;
+  ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)n * 2 * I; ag.k_tok = 2 * I;
+  ag.o_outer = ag.q_outer; ag.o_tok = I; ag.mask_off_from = -1; ag.scale = 8.f;
+  PHK_REQUIRE(A.num_null_kv == 0, PHK_E_UNSUPPORTED, "train: self-attention null-kv is not supported");
+  if (d_self.p > 0.f) {
+    const AttnBwdGeom g1{b, H, n, n, 0, DH};
+    PHK_TRY(attention_forward_dropout(Sv.q1, Sv.kv1, A, c.bias, c.key_mask, Sv.o1, g1, c.asc, st, d_self));
+  } else {
+    PHK_TRY(phk_attention(Sv.q1, Sv.kv1, A.null_kv, A.q_scale, A.k_scale, c.bias, c.key_mask, nullptr, Sv.o1, &ag, s));
+  }
+  PHK_TRY(linear_fwd(prec, tc, Sv.o1, A.wo, Sv.x2, R, D, I, nullptr, Sv.x1, s));  // x2 = x1 + o Wo^T
+  if (Ly.has_cross && c.context) {
+    const phk_attn_t& Cx = Ly.cross_attn;
+    const int dc = Cx.dim_context;
+    Sv.ctxn = ar.f(CR * dc); Sv.ckv = ar.f(CR * 2 * I); Sv.xn2 = ar.f(R * D); Sv.q2 = ar.f(R * I); Sv.o2 = ar.f(R * I);
+    PHK_REQUIRE(Sv.ctxn && Sv.ckv && Sv.xn2 && Sv.q2 && Sv.o2, PHK_E_WORKSPACE, "train: workspace too small (cross)");
+    PHK_TRY(phk_layernorm(c.context, Cx.ctx_g, Cx.ctx_b, Sv.ctxn, nullptr, CR, dc, 0, 0, 0, 0, s));
+    PHK_TRY(linear_fwd(prec, tc, Sv.ctxn, Cx.wkv, Sv.ckv, CR, 2 * I, dc, nullptr, nullptr, s));
+    PHK_TRY(phk_layernorm(Sv.x2, Cx.norm_g, Cx.norm_b, Sv.xn2, nullptr, R, D, 0, 0, 0, 0, s));
+    PHK_TRY(linear_fwd(prec, tc, Sv.xn2, Cx.wq, Sv.q2, R, I, D, nullptr, nullptr, s));
+    std::memset(&ag, 0, sizeof(ag));
+    ag.n_outer = b; ag.n_inner = 1; ag.n_q = n; ag.n_k = L; ag.heads = H; ag.dim_head = DH; ag.num_null_kv = Cx.num_null_kv;
+    ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)L * 2 * I; ag.k_tok = 2 * I;
+    ag.o_outer = ag.q_outer; ag.o_tok = I; ag.kv_outer_mod = b; ag.mask_outer_mod = b; ag.mask_off_from = -1; ag.scale = 8.f;
+    if (d_cross.p > 0.f) {
+      PHK_REQUIRE(Cx.num_null_kv <= 8, PHK_E_UNSUPPORTED, "train: more than 8 null key/values");
+      const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
+      PHK_TRY(attention_forward_dropout(Sv.q2, Sv.ckv, Cx, nullptr, c.text_mask, Sv.o2, g2, c.asc, st, d_cross));
+    } else {
+      PHK_TRY(phk_attention(Sv.q2, Sv.ckv, Cx.null_kv, Cx.q_scale, Cx.k_scale, nullptr, c.text_mask, nullptr, Sv.o2, &ag, s));
+    }
+    PHK_TRY(linear_fwd(prec, tc, Sv.o2, Cx.wo, Sv.x3, R, D, I, nullptr, Sv.x2, s));  // x3 = x2 + o2 Wo^T
+  } else {
+    PHK_CUDA(cudaMemcpyAsync(Sv.x3, Sv.x2, R * D * 4, cudaMemcpyDeviceToDevice, st));
+  }
+  // feed forward (attention.py:45-53)
+  PHK_TRY(phk_layernorm(Sv.x3, Ly.ff.ln_g, Ly.ff.ln_b, Sv.xn3, nullptr, R, D, 0, 0, 0, 0, s));
+  PHK_TRY(linear_fwd(prec, tc, Sv.xn3, Ly.ff.w1, Sv.h, R, 2 * inner, D, nullptr, nullptr, s));
+  if (d_ff.p > 0.f) {
+    PHK_KERNEL_LAUNCH(geglu_dropout_kernel, dim3(ew_grid_fwd(R * inner)), dim3(256), (size_t)(0), st, Sv.h, Sv.g, R, inner, d_ff);
+    PHK_LAUNCH_CHECK();
+  } else {
+    PHK_TRY(phk_geglu(Sv.h, Sv.g, R, inner, s));
+  }
+  return linear_fwd(prec, tc, Sv.g, Ly.ff.w2, *xout, R, D, inner, nullptr, Sv.x3, s);  // x4 = x3 + g W2^T
+}
+
+// Backward of layer l: on entry *dx holds d/d(layer output), on return d/d(x0) (*dx and *dx_alt may swap).  Parameter
+// gradients accumulate into c.GT, the bias gradient into c.dbias; d_context (optional) accumulates d/d(context).
+int layer_backward(const LayerCall& c, int l, const LayerSave& Sv, float** dx, float** dx_alt, const LayerGrads& G,
+                   float* d_context, const DropSite& d_self, const DropSite& d_cross, const DropSite& d_ff) {
+  const phk_transformer_t* T = c.T;
+  const phk_layer_t& Ly = T->layers[l];
+  const phk_layer_t& Gy = c.GT->layers[l];
+  const int b = c.b, n = c.n, L = c.L;
+  const int D = T->dim, H = T->heads, DH = T->dim_head, I = H * DH;
+  const int64_t R = (int64_t)b * n, CR = (int64_t)b * L;
+  const int prec = c.prec;
+  const phk_stream_t s = c.s;
+  const cudaStream_t st = c.st;
+  const TcScratch& tc = c.tc;
+  const int inner = Ly.ff.inner;
+  float* d = *dx;
+  // feed forward: x4 = x3 + geglu(LN(x3) W1^T) W2^T
+  PHK_TRY(dgrad_p(prec, tc, d, Ly.ff.w2, G.dg, R, D, inner, 0, s));
+  PHK_TRY(wgrad_p(prec, tc, d, Sv.g, (float*)Gy.ff.w2, R, D, inner, s));
+  PHK_KERNEL_LAUNCH(geglu_bwd_kernel, dim3(ew_grid(R * inner)), dim3(256), (size_t)(0), st, Sv.h, G.dg, G.dh, R, inner, d_ff);
+  PHK_LAUNCH_CHECK();
+  PHK_TRY(wgrad_p(prec, tc, G.dh, Sv.xn3, (float*)Gy.ff.w1, R, 2 * inner, D, s));
+  PHK_TRY(dgrad_p(prec, tc, G.dh, Ly.ff.w1, G.dtmp, R, 2 * inner, D, 0, s));
+  PHK_TRY(ln_backward(Sv.x3, Ly.ff.ln_g, G.dtmp, d, 1, (float*)Gy.ff.ln_g, (float*)Gy.ff.ln_b, G.stats, R, D, st));
+  // cross attention: x3 = x2 + attn(LN(x2) Wq^T, LN_ctx(context) Wkv^T) Wo^T
+  if (Sv.o2) {
+    const phk_attn_t& Cx = Ly.cross_attn;
+    const phk_attn_t& Gx = Gy.cross_attn;
+    const int dc = Cx.dim_context;
+    PHK_REQUIRE(Cx.num_null_kv <= 8, PHK_E_UNSUPPORTED, "train: more than 8 null key/values");
+    PHK_TRY(dgrad_p(prec, tc, d, Cx.wo, G.dob, R, D, I, 0, s));
+    PHK_TRY(wgrad_p(prec, tc, d, Sv.o2, (float*)Gx.wo, R, D, I, s));
+    const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
+    PHK_TRY(attention_backward(Sv.q2, Sv.ckv, Cx, Gx, nullptr, c.text_mask, G.dob, G.dq, G.dckv, nullptr, g2, c.asc, st,
+                               prec == PHK_PREC_BF16, d_cross));
+    PHK_TRY(wgrad_p(prec, tc, G.dq, Sv.xn2, (float*)Gx.wq, R, I, D, s));
+    PHK_TRY(dgrad_p(prec, tc, G.dq, Cx.wq, G.dtmp, R, I, D, 0, s));
+    PHK_TRY(ln_backward(Sv.x2, Cx.norm_g, G.dtmp, d, 1, (float*)Gx.norm_g, nullptr, G.stats, R, D, st));
+    PHK_TRY(wgrad_p(prec, tc, G.dckv, Sv.ctxn, (float*)Gx.wkv, CR, 2 * I, dc, s));
+    PHK_TRY(dgrad_p(prec, tc, G.dckv, Cx.wkv, G.dctxn, CR, 2 * I, dc, 0, s));
+    // context_norm backward: d/d(context) accumulates over the layers when the caller asks for it
+    PHK_TRY(ln_backward(c.context, Cx.ctx_g, G.dctxn, d_context, d_context ? 1 : 0, (float*)Gx.ctx_g, nullptr, G.stats, CR, dc, st));
+  }
+  // self attention: x2 = x1 + attn(LN(x1) Wq^T, x1 Wkv^T) Wo^T
+  {
+    const phk_attn_t& A = Ly.self_attn;
+    const phk_attn_t& GA = Gy.self_attn;
+    PHK_TRY(dgrad_p(prec, tc, d, A.wo, G.dob, R, D, I, 0, s));
+    PHK_TRY(wgrad_p(prec, tc, d, Sv.o1, (float*)GA.wo, R, D, I, s));
+    const AttnBwdGeom g1{b, H, n, n, 0, DH};
+    PHK_TRY(attention_backward(Sv.q1, Sv.kv1, A, GA, c.bias, c.key_mask, G.dob, G.dq, G.dkv, c.dbias, g1, c.asc, st,
+                               prec == PHK_PREC_BF16, d_self));
+    PHK_TRY(wgrad_p(prec, tc, G.dq, Sv.xn1, (float*)GA.wq, R, I, D, s));
+    PHK_TRY(wgrad_p(prec, tc, G.dkv, Sv.x1, (float*)GA.wkv, R, 2 * I, D, s));
+    PHK_TRY(dgrad_p(prec, tc, G.dq, A.wq, G.dtmp, R, I, D, 0, s));
+    PHK_TRY(ln_backward(Sv.x1, A.norm_g, G.dtmp, d, 1, (float*)GA.norm_g, nullptr, G.stats, R, D, st));
+    PHK_TRY(dgrad_p(prec, tc, G.dkv, A.wkv, d, R, 2 * I, D, 1, s));  // the raw-x path of k, v
+  }
+  if (!Ly.has_peg) return 0;  // x1 = x0
+  // PEG: x1 = x0 + conv(x0) + b
+  PHK_TRY(colsum(d, R, D, D, (float*)Gy.peg.b, st));
+  PHK_REQUIRE(D <= 128 * PEG_DW_MAXJ, PHK_E_UNSUPPORTED, "train: PEG backward needs dim <= 1024");
+  PHK_KERNEL_LAUNCH(peg_bwd_dw_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, Sv.x0, d, (float*)Gy.peg.w, R, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal ? 2 : 1);
+  PHK_LAUNCH_CHECK();
+  PHK_KERNEL_LAUNCH(peg_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, Sv.x0, Ly.peg.w, d, *dx_alt, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal ? 2 : 1);
+  PHK_LAUNCH_CHECK();
+  *dx = *dx_alt;
+  *dx_alt = d;
+  return 0;
+}
+
+LayerCall step_layer_call(const Step& S) {
+  LayerCall c;
+  c.T = S.T; c.GT = S.GT; c.b = S.b; c.n = S.n;
+  c.pegB = S.b; c.pegT = S.pt; c.pegH = S.ph; c.pegW = S.pw;
+  c.bias = S.bias; c.dbias = S.dbias; c.key_mask = S.video_mask;
+  c.context = S.context; c.L = S.L; c.text_mask = S.text_mask;
+  c.prec = S.prec; c.s = S.s; c.st = S.st; c.tc = S.tc; c.asc = S.asc;
+  return c;
+}
+
 // Stage 1.  wide_head: the bf16 operand buffers must hold the V-wide operands of the logits head.
 int step_forward(Step& S, bool wide_head) {
   const phk_maskgit_t* m = S.m;
   const phk_transformer_t* T = S.T;
   const int b = S.b, n = S.n, pt = S.pt, ph = S.ph, pw = S.pw, L = S.L;
-  const int D = S.D, H = S.H, DH = S.DH, I = S.I;
+  const int D = S.D, H = S.H, DH = S.DH;
   const int64_t R = S.R, CR = S.CR;
-  const int prec = S.prec;
   const phk_stream_t s = S.s;
   const cudaStream_t st = S.st;
-  const float* context = S.context;
-  const uint8_t* text_mask = S.text_mask;
-  const uint8_t* video_mask = S.video_mask;
   Arena& ar = S.ar;
   TcScratch& tc = S.tc;
-  if (prec == PHK_PREC_BF16) {  // operand buffers of the wgmma products (activations stay fp32 everywhere else)
+  if (S.prec == PHK_PREC_BF16) {  // operand buffers of the wgmma products (activations stay fp32 everywhere else)
     tc.elems = tc_scratch_elems(m, R, CR, !wide_head);
     tc.a = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
     tc.b = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
@@ -1313,86 +1499,19 @@ int step_forward(Step& S, bool wide_head) {
   if (S.drop_on) {
     S.bases = new (std::nothrow) uint64_t[T->depth][3];
     PHK_REQUIRE(S.bases, PHK_E_ARG, "maskgit_train_step: out of host memory");
-    dropout_layout(m, b, n, context ? L : 0, S.bases);
+    dropout_layout(m, b, n, S.context ? L : 0, S.bases);
   }
   // the attention backward's scratch; the forward's explicit attention path (dropout) uses it too
   const int nk_cross = L + 8;
   const int64_t as1 = attn_bwd_scratch_floats(b, H, n, n, DH), as2 = attn_bwd_scratch_floats(b, H, n, nk_cross, DH);
   S.asc = ar.f(as1 > as2 ? as1 : as2);
   PHK_REQUIRE(S.asc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (attention scratch)");
-  float* asc = S.asc;
-  const float* bias = S.bias;
-  phk_attn_geom_t ag;
+  const LayerCall c = step_layer_call(S);
   const float* xin = x;
   for (int l = 0; l < T->depth; ++l) {
-    const phk_layer_t& Ly = T->layers[l];
-    LayerSave& Sv = S.sv[l];
-    std::memset(&Sv, 0, sizeof(Sv));
-    const int inner = Ly.ff.inner;
-    PHK_REQUIRE(Ly.has_peg, PHK_E_UNSUPPORTED, "maskgit_train_step: layers without PEG are not supported");
-    Sv.x0 = const_cast<float*>(xin);
-    Sv.x1 = ar.f(R * D); Sv.xn1 = ar.f(R * D); Sv.q1 = ar.f(R * I); Sv.kv1 = ar.f(R * 2 * I); Sv.o1 = ar.f(R * I);
-    Sv.x2 = ar.f(R * D); Sv.x3 = ar.f(R * D); Sv.xn3 = ar.f(R * D); Sv.h = ar.f(R * 2 * (int64_t)inner); Sv.g = ar.f(R * (int64_t)inner);
-    float* xout = ar.f(R * D);
-    PHK_REQUIRE(Sv.x1 && Sv.xn1 && Sv.q1 && Sv.kv1 && Sv.o1 && Sv.x2 && Sv.x3 && Sv.xn3 && Sv.h && Sv.g && xout, PHK_E_WORKSPACE,
-                "maskgit_train_step: workspace too small (activations)");
-    // x1 = peg(x0) + x0
-    PHK_TRY(phk_peg3d(Sv.x0, Ly.peg.w, Ly.peg.b, Sv.x1, b, pt, ph, pw, D, Ly.peg.causal, 0, s));
-    // self attention: q from LN(x1), k/v from RAW x1 (attention.py:140-144)
-    const phk_attn_t& A = Ly.self_attn;
-    PHK_TRY(phk_layernorm(Sv.x1, A.norm_g, A.norm_b, Sv.xn1, nullptr, R, D, 0, 0, 0, 0, s));
-    PHK_TRY(linear_fwd(prec, tc, Sv.xn1, A.wq, Sv.q1, R, I, D, nullptr, nullptr, s));
-    PHK_TRY(linear_fwd(prec, tc, Sv.x1, A.wkv, Sv.kv1, R, 2 * I, D, nullptr, nullptr, s));
-    std::memset(&ag, 0, sizeof(ag));
-    ag.n_outer = b; ag.n_inner = 1; ag.n_q = n; ag.n_k = n; ag.heads = H; ag.dim_head = DH; ag.num_null_kv = A.num_null_kv;
-    ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)n * 2 * I; ag.k_tok = 2 * I;
-    ag.o_outer = ag.q_outer; ag.o_tok = I; ag.mask_off_from = -1; ag.scale = 8.f;
-    PHK_REQUIRE(A.num_null_kv == 0, PHK_E_UNSUPPORTED, "maskgit_train_step: self-attention null-kv is not supported");
-    const DropSite d_self = S.site(S.attn_p, l, 0);
-    if (d_self.p > 0.f) {
-      const AttnBwdGeom g1{b, H, n, n, 0, DH};
-      PHK_TRY(attention_forward_dropout(Sv.q1, Sv.kv1, A, bias, video_mask, Sv.o1, g1, asc, st, d_self));
-    } else {
-      PHK_TRY(phk_attention(Sv.q1, Sv.kv1, A.null_kv, A.q_scale, A.k_scale, bias, video_mask, nullptr, Sv.o1, &ag, s));
-    }
-    PHK_TRY(linear_fwd(prec, tc, Sv.o1, A.wo, Sv.x2, R, D, I, nullptr, Sv.x1, s));  // x2 = x1 + o Wo^T
-    const bool cross = Ly.has_cross && context;
-    if (cross) {
-      const phk_attn_t& Cx = Ly.cross_attn;
-      const int dc = Cx.dim_context;
-      Sv.ctxn = ar.f(CR * dc); Sv.ckv = ar.f(CR * 2 * I); Sv.xn2 = ar.f(R * D); Sv.q2 = ar.f(R * I); Sv.o2 = ar.f(R * I);
-      PHK_REQUIRE(Sv.ctxn && Sv.ckv && Sv.xn2 && Sv.q2 && Sv.o2, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (cross)");
-      PHK_TRY(phk_layernorm(context, Cx.ctx_g, Cx.ctx_b, Sv.ctxn, nullptr, CR, dc, 0, 0, 0, 0, s));
-      PHK_TRY(linear_fwd(prec, tc, Sv.ctxn, Cx.wkv, Sv.ckv, CR, 2 * I, dc, nullptr, nullptr, s));
-      PHK_TRY(phk_layernorm(Sv.x2, Cx.norm_g, Cx.norm_b, Sv.xn2, nullptr, R, D, 0, 0, 0, 0, s));
-      PHK_TRY(linear_fwd(prec, tc, Sv.xn2, Cx.wq, Sv.q2, R, I, D, nullptr, nullptr, s));
-      std::memset(&ag, 0, sizeof(ag));
-      ag.n_outer = b; ag.n_inner = 1; ag.n_q = n; ag.n_k = L; ag.heads = H; ag.dim_head = DH; ag.num_null_kv = Cx.num_null_kv;
-      ag.q_outer = (int64_t)n * I; ag.q_tok = I; ag.k_outer = (int64_t)L * 2 * I; ag.k_tok = 2 * I;
-      ag.o_outer = ag.q_outer; ag.o_tok = I; ag.kv_outer_mod = b; ag.mask_outer_mod = b; ag.mask_off_from = -1; ag.scale = 8.f;
-      const DropSite d_cross = S.site(S.attn_p, l, 1);
-      if (d_cross.p > 0.f) {
-        PHK_REQUIRE(Cx.num_null_kv <= 8, PHK_E_UNSUPPORTED, "maskgit_train_step: more than 8 null key/values");
-        const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
-        PHK_TRY(attention_forward_dropout(Sv.q2, Sv.ckv, Cx, nullptr, text_mask, Sv.o2, g2, asc, st, d_cross));
-      } else {
-        PHK_TRY(phk_attention(Sv.q2, Sv.ckv, Cx.null_kv, Cx.q_scale, Cx.k_scale, nullptr, text_mask, nullptr, Sv.o2, &ag, s));
-      }
-      PHK_TRY(linear_fwd(prec, tc, Sv.o2, Cx.wo, Sv.x3, R, D, I, nullptr, Sv.x2, s));  // x3 = x2 + o2 Wo^T
-    } else {
-      PHK_CUDA(cudaMemcpyAsync(Sv.x3, Sv.x2, R * D * 4, cudaMemcpyDeviceToDevice, st));
-    }
-    // feed forward (attention.py:45-53)
-    PHK_TRY(phk_layernorm(Sv.x3, Ly.ff.ln_g, Ly.ff.ln_b, Sv.xn3, nullptr, R, D, 0, 0, 0, 0, s));
-    PHK_TRY(linear_fwd(prec, tc, Sv.xn3, Ly.ff.w1, Sv.h, R, 2 * inner, D, nullptr, nullptr, s));
-    const DropSite d_ff = S.site(S.ff_p, l, 2);
-    if (d_ff.p > 0.f) {
-      PHK_KERNEL_LAUNCH(geglu_dropout_kernel, dim3(ew_grid_fwd(R * inner)), dim3(256), (size_t)(0), st, Sv.h, Sv.g, R, inner, d_ff);
-      PHK_LAUNCH_CHECK();
-    } else {
-      PHK_TRY(phk_geglu(Sv.h, Sv.g, R, inner, s));
-    }
-    PHK_TRY(linear_fwd(prec, tc, Sv.g, Ly.ff.w2, xout, R, D, inner, nullptr, Sv.x3, s));  // x4 = x3 + g W2^T
+    PHK_REQUIRE(T->layers[l].has_peg, PHK_E_UNSUPPORTED, "maskgit_train_step: layers without PEG are not supported");
+    float* xout = nullptr;
+    PHK_TRY(layer_forward(c, l, xin, S.sv[l], &xout, ar, S.site(S.attn_p, l, 0), S.site(S.attn_p, l, 1), S.site(S.ff_p, l, 2)));
     xin = xout;
   }
   S.xf = xin;
@@ -1419,91 +1538,36 @@ int step_backward(Step& S, float* d_context, void** prog, int nprog) {
   const phk_maskgit_t* grads = S.grads;
   const phk_transformer_t* T = S.T;
   const phk_transformer_t* GT = S.GT;
-  const int b = S.b, n = S.n, pt = S.pt, ph = S.ph, pw = S.pw, L = S.L;
-  const int D = S.D, H = S.H, DH = S.DH, I = S.I;
+  const int n = S.n, pt = S.pt, ph = S.ph, pw = S.pw;
+  const int D = S.D, I = S.I;
   const int64_t R = S.R, CR = S.CR;
-  const int prec = S.prec;
-  const phk_stream_t s = S.s;
   const cudaStream_t st = S.st;
   const float* context = S.context;
-  const uint8_t* text_mask = S.text_mask;
-  const uint8_t* video_mask = S.video_mask;
   Arena& ar = S.ar;
-  const TcScratch& tc = S.tc;
-  float2* stats = S.stats;
   int64_t inner_max = 0, dc_max = 0;
   for (int l = 0; l < T->depth; ++l) {
     if (T->layers[l].ff.inner > inner_max) inner_max = T->layers[l].ff.inner;
     if (T->layers[l].has_cross && T->layers[l].cross_attn.dim_context > dc_max) dc_max = T->layers[l].cross_attn.dim_context;
   }
-  float* dq = ar.f(R * I);
-  float* dkv = ar.f(R * 2 * I);
-  float* dob = ar.f(R * I);
-  float* dh = ar.f(R * 2 * inner_max);
-  float* dg = ar.f(R * inner_max);
-  float* dckv = context ? ar.f(CR * 2 * I) : nullptr;
-  float* dctxn = context ? ar.f(CR * (dc_max > 0 ? dc_max : 1)) : nullptr;
-  PHK_REQUIRE(dq && dkv && dob && dh && dg && (!context || (dckv && dctxn)), PHK_E_WORKSPACE,
+  LayerGrads G;
+  G.dtmp = S.dtmp; G.stats = S.stats;
+  G.dq = ar.f(R * I);
+  G.dkv = ar.f(R * 2 * I);
+  G.dob = ar.f(R * I);
+  G.dh = ar.f(R * 2 * inner_max);
+  G.dg = ar.f(R * inner_max);
+  G.dckv = context ? ar.f(CR * 2 * I) : nullptr;
+  G.dctxn = context ? ar.f(CR * (dc_max > 0 ? dc_max : 1)) : nullptr;
+  PHK_REQUIRE(G.dq && G.dkv && G.dob && G.dh && G.dg && (!context || (G.dckv && G.dctxn)), PHK_E_WORKSPACE,
               "maskgit_train_step: workspace too small (gradients)");
   float* dx = S.dxa;      // d loss / d (current residual stream)
   float* dx_alt = S.dxb;
-  PHK_TRY(ln_backward(S.xf, T->out_g, S.dtmp, dx, 0, (float*)GT->out_g, nullptr, stats, R, D, st));
+  PHK_TRY(ln_backward(S.xf, T->out_g, S.dtmp, dx, 0, (float*)GT->out_g, nullptr, S.stats, R, D, st));
   PHK_TRY(progress_mark(prog, nprog, 0, st));  // head + norm_out gradients final
+  const LayerCall c = step_layer_call(S);
   for (int l = T->depth - 1; l >= 0; --l) {
-    const phk_layer_t& Ly = T->layers[l];
-    const phk_layer_t& Gy = GT->layers[l];
-    const LayerSave& Sv = S.sv[l];
-    const int inner = Ly.ff.inner;
-    // feed forward: x4 = x3 + geglu(LN(x3) W1^T) W2^T
-    PHK_TRY(dgrad_p(prec, tc, dx, Ly.ff.w2, dg, R, D, inner, 0, s));
-    PHK_TRY(wgrad_p(prec, tc, dx, Sv.g, (float*)Gy.ff.w2, R, D, inner, s));
-    PHK_KERNEL_LAUNCH(geglu_bwd_kernel, dim3(ew_grid(R * inner)), dim3(256), (size_t)(0), st, Sv.h, dg, dh, R, inner, S.site(S.ff_p, l, 2));
-    PHK_LAUNCH_CHECK();
-    PHK_TRY(wgrad_p(prec, tc, dh, Sv.xn3, (float*)Gy.ff.w1, R, 2 * inner, D, s));
-    PHK_TRY(dgrad_p(prec, tc, dh, Ly.ff.w1, S.dtmp, R, 2 * inner, D, 0, s));
-    PHK_TRY(ln_backward(Sv.x3, Ly.ff.ln_g, S.dtmp, dx, 1, (float*)Gy.ff.ln_g, (float*)Gy.ff.ln_b, stats, R, D, st));
-    // cross attention: x3 = x2 + attn(LN(x2) Wq^T, LN_ctx(context) Wkv^T) Wo^T
-    if (Sv.o2) {
-      const phk_attn_t& Cx = Ly.cross_attn;
-      const phk_attn_t& Gx = Gy.cross_attn;
-      const int dc = Cx.dim_context;
-      PHK_REQUIRE(Cx.num_null_kv <= 8, PHK_E_UNSUPPORTED, "maskgit_train_step: more than 8 null key/values");
-      PHK_TRY(dgrad_p(prec, tc, dx, Cx.wo, dob, R, D, I, 0, s));
-      PHK_TRY(wgrad_p(prec, tc, dx, Sv.o2, (float*)Gx.wo, R, D, I, s));
-      const AttnBwdGeom g2{b, H, n, L, Cx.num_null_kv, DH};
-      PHK_TRY(attention_backward(Sv.q2, Sv.ckv, Cx, Gx, nullptr, text_mask, dob, dq, dckv, nullptr, g2, S.asc, st, prec == PHK_PREC_BF16,
-                                 S.site(S.attn_p, l, 1)));
-      PHK_TRY(wgrad_p(prec, tc, dq, Sv.xn2, (float*)Gx.wq, R, I, D, s));
-      PHK_TRY(dgrad_p(prec, tc, dq, Cx.wq, S.dtmp, R, I, D, 0, s));
-      PHK_TRY(ln_backward(Sv.x2, Cx.norm_g, S.dtmp, dx, 1, (float*)Gx.norm_g, nullptr, stats, R, D, st));
-      PHK_TRY(wgrad_p(prec, tc, dckv, Sv.ctxn, (float*)Gx.wkv, CR, 2 * I, dc, s));
-      PHK_TRY(dgrad_p(prec, tc, dckv, Cx.wkv, dctxn, CR, 2 * I, dc, 0, s));
-      // context_norm backward: d/d(context) accumulates over the layers when the caller asks for it
-      PHK_TRY(ln_backward(context, Cx.ctx_g, dctxn, d_context, d_context ? 1 : 0, (float*)Gx.ctx_g, nullptr, stats, CR, dc, st));
-    }
-    // self attention: x2 = x1 + attn(LN(x1) Wq^T, x1 Wkv^T) Wo^T
-    {
-      const phk_attn_t& A = Ly.self_attn;
-      const phk_attn_t& GA = Gy.self_attn;
-      PHK_TRY(dgrad_p(prec, tc, dx, A.wo, dob, R, D, I, 0, s));
-      PHK_TRY(wgrad_p(prec, tc, dx, Sv.o1, (float*)GA.wo, R, D, I, s));
-      const AttnBwdGeom g1{b, H, n, n, 0, DH};
-      PHK_TRY(attention_backward(Sv.q1, Sv.kv1, A, GA, S.bias, video_mask, dob, dq, dkv, S.dbias, g1, S.asc, st, prec == PHK_PREC_BF16,
-                                 S.site(S.attn_p, l, 0)));
-      PHK_TRY(wgrad_p(prec, tc, dq, Sv.xn1, (float*)GA.wq, R, I, D, s));
-      PHK_TRY(wgrad_p(prec, tc, dkv, Sv.x1, (float*)GA.wkv, R, 2 * I, D, s));
-      PHK_TRY(dgrad_p(prec, tc, dq, A.wq, S.dtmp, R, I, D, 0, s));
-      PHK_TRY(ln_backward(Sv.x1, A.norm_g, S.dtmp, dx, 1, (float*)GA.norm_g, nullptr, stats, R, D, st));
-      PHK_TRY(dgrad_p(prec, tc, dkv, A.wkv, dx, R, 2 * I, D, 1, s));  // the raw-x path of k, v
-    }
-    // PEG: x1 = x0 + conv(x0) + b
-    PHK_TRY(colsum(dx, R, D, D, (float*)Gy.peg.b, st));
-    PHK_REQUIRE(D <= 128 * PEG_DW_MAXJ, PHK_E_UNSUPPORTED, "maskgit_train_step: dim > 1024");
-    PHK_KERNEL_LAUNCH(peg_bwd_dw_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, Sv.x0, dx, (float*)Gy.peg.w, R, pt, ph, pw, D, Ly.peg.causal ? 2 : 1);
-    PHK_LAUNCH_CHECK();
-    PHK_KERNEL_LAUNCH(peg_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, Sv.x0, Ly.peg.w, dx, dx_alt, pt, ph, pw, D, Ly.peg.causal ? 2 : 1);
-    PHK_LAUNCH_CHECK();
-    float* t = dx; dx = dx_alt; dx_alt = t;
+    PHK_TRY(layer_backward(c, l, S.sv[l], &dx, &dx_alt, G, d_context, S.site(S.attn_p, l, 0), S.site(S.attn_p, l, 1),
+                           S.site(S.ff_p, l, 2)));
     // this layer's parameter gradients are final -- except, with a context, the cross-attention's context_norm / to_kv
     // share nothing with other layers either; the position-bias gradient (dbias, all layers) is finished below
     PHK_TRY(progress_mark(prog, nprog, 1 + (T->depth - 1 - l), st));
@@ -1809,6 +1873,305 @@ extern "C" int phk_maskgit_backward(const phk_maskgit_t* m, const phk_maskgit_t*
   if (pair && d_context) {
     PHK_KERNEL_LAUNCH(add_halves_kernel, dim3(ew_grid(CRh * dc)), dim3(256), (size_t)(0), st, ctx_grad, d_context, CRh * dc);
     PHK_LAUNCH_CHECK();
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// C-ViViT decoder backward (include/phk.h, phk_cvivit_decode_backward): what autograd computes through CViViT.decode /
+// decode_from_codebook_indices (cvivit.py:437-443, 476-516).  The forward is recomputed with saved activations on the
+// layer code above, then differentiated from d video:
+//   temporal stack  rows permuted from (b t h w) to (b h w t) by one gather, so that its sequences are runs of T' rows and
+//                   the reference's raw x.reshape(b, t, h, w, d) of the (b h w, t, d) tensor (attention.py:71, the
+//                   forward's peg_layout 1) is layout-0 PEG on these rows; ALiBi and the causal fill are one constant
+//                   [H, T', T'] bias (-FLT_MAX above the diagonal: exact zeros in the softmax and in its backward)
+//   spatial stack   rows (b t h w), runs of h w rows, no PEG; the 2-D continuous position bias sends its gradient through
+//                   the bias MLP (cpb_backward with (h, w, 1))
+//   to_pixels       norm_out gathered into first-frame / remaining-frame rows as the forward does; d video gathered into
+//                   the same patch layout (the adjoint of phk_unpatchify); wgrad, bias column sum, dgrad per Linear
+//   project_out     (ids) wgrad against the +-1 codes rebuilt from the ids and the bias column sum; the ids get nothing
+// No dropout: the decode forward applies none.
+// ------------------------------------------------------------------------------------------------------------------
+namespace phk {
+namespace {
+
+// [B * Tp * hw, D] rows in (b, t, s) order -> (b, s, t) order (to_seq), or back
+__global__ void permute_bts_kernel(const float* __restrict__ src, float* __restrict__ dst, int B, int Tp, int hw, int D,
+                                   int to_seq) {
+  const int64_t total = (int64_t)B * Tp * hw * D;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / D;
+    const int d = (int)(i - r * D);
+    int64_t sr;
+    if (to_seq) {  // r = (b hw + s) Tp + t
+      const int t = (int)(r % Tp);
+      const int64_t bs = r / Tp;
+      sr = ((bs / hw) * Tp + t) * hw + bs % hw;
+    } else {       // r = (b Tp + t) hw + s
+      const int s = (int)(r % hw);
+      const int64_t bt = r / hw;
+      sr = ((bt / Tp) * hw + s) * Tp + bt % Tp;
+    }
+    dst[i] = src[sr * D + d];
+  }
+}
+
+// bias[h, i, j] = -|j - i| * slope[h] for j <= i, -FLT_MAX for j > i: ALiBi (attention.py:195-227) and the causal fill
+// (:170-172) of the temporal attention, with the forward kernel's arithmetic (attention.cu)
+__global__ void alibi_causal_bias_kernel(const float* __restrict__ slopes, float* __restrict__ bias, int H, int n) {
+  const int64_t total = (int64_t)H * n * n;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int j = (int)(idx % n), i = (int)((idx / n) % n), h = (int)(idx / ((int64_t)n * n));
+    bias[idx] = j > i ? -FLT_MAX : -fabsf((float)(j - i)) * slopes[h];
+  }
+}
+
+// full[(b Tp + t) hw + s] = first[b hw + s] (t = 0) or rest[(b (Tp - 1) + t - 1) hw + s] (t > 0), rows of D floats
+__global__ void frames_merge_kernel(const float* __restrict__ first, const float* __restrict__ rest, float* __restrict__ full,
+                                    int B, int Tp, int hw, int D) {
+  const int64_t total = (int64_t)B * Tp * hw * D;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / D;
+    const int d = (int)(i - r * D);
+    const int s = (int)(r % hw);
+    const int t = (int)((r / hw) % Tp);
+    const int64_t b = r / ((int64_t)hw * Tp);
+    full[i] = t == 0 ? first[(b * hw + s) * D + d] : rest[((b * (Tp - 1) + t - 1) * hw + s) * D + d];
+  }
+}
+
+// out[((b nt + t) hh + y) ww + x, ((c pt + k) p1 + i) p2 + j] = video[b, c, f0 + t pt + k, y p1 + i, x p2 + j]:
+// 'b c (t pt) (h p1) (w p2) -> (b t h w) (c pt p1 p2)', the adjoint of phk_unpatchify (cvivit.py:286-295)
+__global__ void patch_gather_kernel(const float* __restrict__ video, float* __restrict__ out, int B, int C, int F, int H,
+                                    int W, int f0, int nt, int pt, int p1, int p2) {
+  const int hh = H / p1, ww = W / p2, K = C * pt * p1 * p2;
+  const int64_t total = (int64_t)B * nt * hh * ww * K;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / K;
+    const int e = (int)(i - r * K);
+    const int x = (int)(r % ww), y = (int)((r / ww) % hh), t = (int)((r / ((int64_t)ww * hh)) % nt);
+    const int64_t b = r / ((int64_t)ww * hh * nt);
+    const int j = e % p2, ii = (e / p2) % p1, k = (e / (p2 * p1)) % pt, c = e / (p2 * p1 * pt);
+    out[i] = video[(((b * C + c) * F + f0 + (int64_t)t * pt + k) * H + (int64_t)y * p1 + ii) * W + (int64_t)x * p2 + j];
+  }
+}
+
+// codes[r, k] = +1 if bit (bits - 1 - k) of ids[r] is set, else -1 (indices_to_codes before project_out, oracle/lfq.py)
+__global__ void lfq_signs_kernel(const int64_t* __restrict__ ids, float* __restrict__ codes, int64_t rows, int bits) {
+  const int64_t total = rows * bits;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / bits;
+    const int k = (int)(i - r * bits);
+    codes[i] = ((ids[r] >> (bits - 1 - k)) & 1) ? 1.0f : -1.0f;
+  }
+}
+
+int64_t stack_inner(const phk_transformer_t* T) {
+  int64_t inner = 0;
+  for (int l = 0; l < T->depth; ++l) inner = T->layers[l].ff.inner > inner ? T->layers[l].ff.inner : inner;
+  return inner;
+}
+
+// one bf16 operand buffer of the decoder's tensor-core products (see tc_scratch_elems): every [rows, width] operand,
+// straight or transposed, with width up to K2 = C pt p1 p2 (the to_pixels output)
+int64_t dec_tc_scratch_elems(const phk_cvivit_dec_t* m, int64_t R, int64_t K2) {
+  const int64_t inner = stack_inner(&m->temporal) > stack_inner(&m->spatial) ? stack_inner(&m->temporal) : stack_inner(&m->spatial);
+  const int64_t I = (int64_t)m->heads * m->dim_head, D = m->dim;
+  int64_t width = 2 * inner;
+  if (2 * I > width) width = 2 * I;
+  if (D > width) width = D;
+  if (K2 > width) width = K2;
+  int64_t feat = D;
+  if (I > feat) feat = I;
+  if (inner > feat) feat = inner;
+  const int64_t tokens = pad8(R) + 8;
+  return (tokens > feat + 8 ? tokens : feat + 8) * (width + 8);
+}
+
+}  // namespace
+}  // namespace phk
+
+extern "C" int64_t phk_cvivit_decode_backward_workspace_bytes(const phk_cvivit_dec_t* m, int32_t B, int32_t Tp, int32_t prec) {
+  if (!m || B <= 0 || Tp <= 0 || !m->temporal.layers || !m->spatial.layers || m->temporal.depth <= 0 ||
+      m->spatial.depth <= 0 || m->patch_h <= 0 || m->patch_w <= 0 || m->patch_t <= 0 || m->image_h % m->patch_h != 0 ||
+      m->image_w % m->patch_w != 0)
+    return -1;
+  const int hh = m->image_h / m->patch_h, ww = m->image_w / m->patch_w, hw = hh * ww;
+  const int64_t R = (int64_t)B * Tp * hw, D = m->dim, H = m->heads, I = H * m->dim_head;
+  const int64_t K1 = (int64_t)m->channels * m->patch_h * m->patch_w, K2 = K1 * m->patch_t;
+  const int64_t rows1 = (int64_t)B * hw, rows2 = (int64_t)B * (Tp - 1) * hw;
+  const int64_t inner = stack_inner(&m->temporal) > stack_inner(&m->spatial) ? stack_inner(&m->temporal) : stack_inner(&m->spatial);
+  int64_t f = 2 * R * D;                                         // codes (b t h w), their (b h w t) copy
+  f += H * Tp * Tp + 2 * H * hw * hw + phk_cpb_scratch_floats(&m->spatial_bias, hh, ww, 1);  // biases, d spatial bias
+  const int64_t a1 = attn_bwd_scratch_floats(B * hw, (int)H, Tp, Tp, m->dim_head);
+  const int64_t a2 = attn_bwd_scratch_floats(B * Tp, (int)H, hw, hw, m->dim_head);
+  f += a1 > a2 ? a1 : a2;
+  for (int l = 0; l < m->temporal.depth; ++l) f += layer_save_floats(&m->temporal, m->temporal.layers[l], R, 0);
+  for (int l = 0; l < m->spatial.depth; ++l) f += layer_save_floats(&m->spatial, m->spatial.layers[l], R, 0);
+  f += 2 * R * D;                                                // temporal norm_out (b h w t), spatial input (b t h w)
+  f += (rows1 + (rows2 > 0 ? rows2 : 1)) * D;                   // spatial norm_out: first frame, remaining frames
+  f += R * (3 * D + 4 * I + 3 * inner) + 2 * R;                  // dxa dxb dtmp | dq dkv(2) dob | dh(2) dg | statistics
+  f += (rows1 * K1 > rows2 * K2 ? rows1 * K1 : rows2 * K2);      // d video in a patch layout
+  f += (rows1 + (rows2 > 0 ? rows2 : 1)) * D;                   // d norm_out: first frame, remaining frames
+  f += R * (m->codebook_bits > 0 ? m->codebook_bits : 1);        // +-1 codes
+  f += cpb_bwd_scratch_floats(m->spatial_bias, hh, ww, 1);
+  int64_t bytes = f * 4 + 256 * 64;
+  if (prec == PHK_PREC_BF16) bytes += 2 * (dec_tc_scratch_elems(m, R, K2) * 2 + 256);
+  return bytes;
+}
+
+// See include/phk.h.
+extern "C" int phk_cvivit_decode_backward(const phk_cvivit_dec_t* m, const phk_cvivit_dec_t* grads, const int64_t* ids,
+                                          const float* tokens, int32_t B, int32_t Tp, const float* dvideo, float* dtokens,
+                                          void* workspace, int64_t workspace_bytes, int32_t prec, phk_stream_t s) {
+  PHK_REQUIRE(m && grads && (ids || tokens) && dvideo && workspace, PHK_E_ARG, "cvivit_decode_backward: null pointer");
+  PHK_REQUIRE(!ids || !dtokens, PHK_E_ARG, "cvivit_decode_backward: dtokens belongs to the float-token decode (ids NULL)");
+  PHK_REQUIRE(prec == PHK_PREC_F32 || prec == PHK_PREC_BF16, PHK_E_ARG, "cvivit_decode_backward: unknown precision mode");
+  const int64_t need = phk_cvivit_decode_backward_workspace_bytes(m, B, Tp, prec);
+  PHK_REQUIRE(need > 0, PHK_E_ARG, "cvivit_decode_backward: bad model table or shape");
+  PHK_REQUIRE(workspace_bytes >= need, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
+  const phk_transformer_t* TT = &m->temporal;
+  const phk_transformer_t* TS = &m->spatial;
+  PHK_REQUIRE(grads->temporal.layers && grads->spatial.layers && grads->temporal.depth == TT->depth &&
+              grads->spatial.depth == TS->depth, PHK_E_ARG, "cvivit_decode_backward: weight table / gradient table mismatch");
+  PHK_REQUIRE(TT->causal && TT->alibi_slopes && !TS->causal, PHK_E_ARG,
+              "cvivit_decode_backward: the temporal stack is causal with ALiBi slopes, the spatial one is not");
+  PHK_REQUIRE(TT->dim == m->dim && TS->dim == m->dim && TT->heads == m->heads && TS->heads == m->heads &&
+              TT->dim_head == m->dim_head && TS->dim_head == m->dim_head, PHK_E_ARG,
+              "cvivit_decode_backward: transformer widths differ from the model's");
+  PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "cvivit_decode_backward: dim must be a multiple of 4");
+  for (int l = 0; l < TT->depth; ++l) PHK_REQUIRE(!TT->layers[l].has_cross, PHK_E_ARG, "cvivit_decode_backward: cross-attention layer");
+  for (int l = 0; l < TS->depth; ++l) PHK_REQUIRE(!TS->layers[l].has_cross, PHK_E_ARG, "cvivit_decode_backward: cross-attention layer");
+  PHK_REQUIRE(!ids || (m->codebook_bits > 0 && m->vq_out_w && m->vq_out_b && grads->vq_out_w && grads->vq_out_b), PHK_E_ARG,
+              "cvivit_decode_backward: ids need LFQ's project_out and its gradient");
+  const int hh = m->image_h / m->patch_h, ww = m->image_w / m->patch_w, hw = hh * ww;
+  const int D = m->dim, H = m->heads, DH = m->dim_head, I = H * DH, C = m->channels;
+  const int64_t R = (int64_t)B * Tp * hw, per = (int64_t)Tp * hw;
+  const int64_t K1 = (int64_t)C * m->patch_h * m->patch_w, K2 = K1 * m->patch_t;
+  const int64_t rows1 = (int64_t)B * hw, rows2 = (int64_t)B * (Tp - 1) * hw;
+  const int F = 1 + (Tp - 1) * m->patch_t;
+  const int64_t inner = stack_inner(TT) > stack_inner(TS) ? stack_inner(TT) : stack_inner(TS);
+  const cudaStream_t st = to_stream(s);
+  Arena ar{(char*)workspace, workspace_bytes, 0};
+  TcScratch tc{nullptr, nullptr, 0};
+  if (prec == PHK_PREC_BF16) {
+    tc.elems = dec_tc_scratch_elems(m, R, K2);
+    tc.a = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
+    tc.b = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
+    PHK_REQUIRE(tc.a && tc.b, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small (tensor-core operands)");
+  }
+  float* xc = ar.f(R * D);
+  float* xp = ar.f(R * D);
+  float* bias_t = ar.f((int64_t)H * Tp * Tp);
+  float* bias_s = ar.f((int64_t)H * hw * hw);
+  float* dbias_s = ar.f((int64_t)H * hw * hw);
+  float* cpb_sc = ar.f(phk_cpb_scratch_floats(&m->spatial_bias, hh, ww, 1));
+  const int64_t a1 = attn_bwd_scratch_floats(B * hw, H, Tp, Tp, DH), a2 = attn_bwd_scratch_floats(B * Tp, H, hw, hw, DH);
+  float* asc = ar.f(a1 > a2 ? a1 : a2);
+  PHK_REQUIRE(xc && xp && bias_t && bias_s && dbias_s && cpb_sc && asc, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
+
+  // ---------------------------------------------------------------- inputs, biases
+  const float* x_in = tokens;
+  if (ids) {
+    PHK_TRY(phk_lfq_codes(ids, m->vq_out_w, m->vq_out_b, xc, R, D, m->codebook_bits, s));
+    x_in = xc;
+  }
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, x_in, xp, B, Tp, hw, D, 1);
+  PHK_LAUNCH_CHECK();
+  PHK_KERNEL_LAUNCH(alibi_causal_bias_kernel, dim3(ew_grid((int64_t)H * Tp * Tp)), dim3(256), (size_t)(0), st, TT->alibi_slopes, bias_t, H, Tp);
+  PHK_LAUNCH_CHECK();
+  PHK_TRY(phk_cpb_bias(&m->spatial_bias, hh, ww, 1, cpb_sc, bias_s, s));
+  PHK_CUDA(cudaMemsetAsync(dbias_s, 0, (int64_t)H * hw * hw * 4, st));
+
+  // ---------------------------------------------------------------- forward, saving activations
+  const DropSite none{0.f, 0.f, 0u, 0u, 0u};
+  LayerCall ct;  // temporal: B h w sequences of T' rows
+  ct.T = TT; ct.GT = &grads->temporal; ct.b = B * hw; ct.n = Tp;
+  ct.pegB = B; ct.pegT = Tp; ct.pegH = hh; ct.pegW = ww;
+  ct.bias = bias_t; ct.prec = prec; ct.s = s; ct.st = st; ct.tc = tc; ct.asc = asc;
+  LayerCall cs = ct;  // spatial: B T' sequences of h w rows
+  cs.T = TS; cs.GT = &grads->spatial; cs.b = B * Tp; cs.n = hw; cs.bias = bias_s; cs.dbias = dbias_s;
+  std::unique_ptr<LayerSave[]> svT(new (std::nothrow) LayerSave[TT->depth]), svS(new (std::nothrow) LayerSave[TS->depth]);
+  PHK_REQUIRE(svT && svS, PHK_E_ARG, "cvivit_decode_backward: out of host memory");
+  const float* xin = xp;
+  for (int l = 0; l < TT->depth; ++l) {
+    float* xout = nullptr;
+    PHK_TRY(layer_forward(ct, l, xin, svT[l], &xout, ar, none, none, none));
+    xin = xout;
+  }
+  const float* xfT = xin;
+  float* nT = ar.f(R * D);
+  float* P = ar.f(R * D);
+  PHK_REQUIRE(nT && P, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
+  PHK_TRY(phk_layernorm(xfT, TT->out_g, TT->out_b, nT, nullptr, R, D, 0, 0, 0, 0, s));
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, nT, P, B, Tp, hw, D, 0);
+  PHK_LAUNCH_CHECK();
+  xin = P;
+  for (int l = 0; l < TS->depth; ++l) {
+    float* xout = nullptr;
+    PHK_TRY(layer_forward(cs, l, xin, svS[l], &xout, ar, none, none, none));
+    xin = xout;
+  }
+  const float* xfS = xin;
+  float* Ef = ar.f(rows1 * D);
+  float* Er = ar.f((rows2 > 0 ? rows2 : 1) * D);
+  PHK_REQUIRE(Ef && Er, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
+  PHK_TRY(phk_layernorm(xfS, TS->out_g, TS->out_b, Ef, nullptr, rows1, D, 0, -hw, per, 0, s));
+  if (Tp > 1) PHK_TRY(phk_layernorm(xfS, TS->out_g, TS->out_b, Er, nullptr, rows2, D, 0, -(per - hw), per, hw, s));
+
+  // ---------------------------------------------------------------- to_pixels_first_frame / to_pixels
+  LayerGrads G;
+  float* dx = ar.f(R * D);
+  float* dx_alt = ar.f(R * D);
+  G.dtmp = ar.f(R * D); G.dq = ar.f(R * I); G.dkv = ar.f(R * 2 * I); G.dob = ar.f(R * I);
+  G.dh = ar.f(R * 2 * inner); G.dg = ar.f(R * inner); G.dckv = nullptr; G.dctxn = nullptr;
+  G.stats = reinterpret_cast<float2*>(ar.f(2 * R));
+  float* dG = ar.f(rows1 * K1 > rows2 * K2 ? rows1 * K1 : rows2 * K2);
+  float* dEf = ar.f(rows1 * D);
+  float* dEr = ar.f((rows2 > 0 ? rows2 : 1) * D);
+  PHK_REQUIRE(dx && dx_alt && G.dtmp && G.dq && G.dkv && G.dob && G.dh && G.dg && G.stats && dG && dEf && dEr, PHK_E_WORKSPACE,
+              "cvivit_decode_backward: workspace too small (gradients)");
+  PHK_KERNEL_LAUNCH(patch_gather_kernel, dim3(ew_grid(rows1 * K1)), dim3(256), (size_t)(0), st, dvideo, dG, B, C, F, m->image_h, m->image_w, 0, 1, 1, m->patch_h, m->patch_w);
+  PHK_LAUNCH_CHECK();
+  PHK_TRY(wgrad_p(prec, tc, dG, Ef, (float*)grads->px_first_w, rows1, K1, D, s));
+  PHK_TRY(colsum(dG, rows1, (int)K1, K1, (float*)grads->px_first_b, st));
+  PHK_TRY(dgrad_p(prec, tc, dG, m->px_first_w, dEf, rows1, K1, D, 0, s));
+  if (Tp > 1) {  // (one latent frame: to_pixels sees an empty batch, its gradients stay the caller's zeros)
+    PHK_KERNEL_LAUNCH(patch_gather_kernel, dim3(ew_grid(rows2 * K2)), dim3(256), (size_t)(0), st, dvideo, dG, B, C, F, m->image_h, m->image_w, 1, Tp - 1, m->patch_t, m->patch_h, m->patch_w);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(wgrad_p(prec, tc, dG, Er, (float*)grads->px_w, rows2, K2, D, s));
+    PHK_TRY(colsum(dG, rows2, (int)K2, K2, (float*)grads->px_b, st));
+    PHK_TRY(dgrad_p(prec, tc, dG, m->px_w, dEr, rows2, K2, D, 0, s));
+  }
+  PHK_KERNEL_LAUNCH(frames_merge_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dEf, dEr, G.dtmp, B, Tp, hw, D);
+  PHK_LAUNCH_CHECK();
+
+  // ---------------------------------------------------------------- spatial stack, position-bias MLP
+  PHK_TRY(ln_backward(xfS, TS->out_g, G.dtmp, dx, 0, (float*)grads->spatial.out_g, nullptr, G.stats, R, D, st));
+  for (int l = TS->depth - 1; l >= 0; --l) PHK_TRY(layer_backward(cs, l, svS[l], &dx, &dx_alt, G, nullptr, none, none, none));
+  float* csc = ar.f(cpb_bwd_scratch_floats(m->spatial_bias, hh, ww, 1));
+  PHK_REQUIRE(csc, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small (position-bias backward)");
+  PHK_TRY(cpb_backward(m->spatial_bias, grads->spatial_bias, dbias_s, hh, ww, 1, csc, st));
+
+  // ---------------------------------------------------------------- temporal stack, rows (b h w t)
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 1);
+  PHK_LAUNCH_CHECK();
+  PHK_TRY(ln_backward(xfT, TT->out_g, G.dtmp, dx, 0, (float*)grads->temporal.out_g, nullptr, G.stats, R, D, st));
+  for (int l = TT->depth - 1; l >= 0; --l) PHK_TRY(layer_backward(ct, l, svT[l], &dx, &dx_alt, G, nullptr, none, none, none));
+
+  // ---------------------------------------------------------------- d tokens / project_out
+  if (!ids && !dtokens) return 0;
+  float* dcodes = dtokens ? dtokens : dx_alt;
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, dcodes, B, Tp, hw, D, 0);
+  PHK_LAUNCH_CHECK();
+  if (ids) {
+    const int bits = m->codebook_bits;
+    float* signs = ar.f(R * bits);
+    PHK_REQUIRE(signs, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small (codes)");
+    PHK_KERNEL_LAUNCH(lfq_signs_kernel, dim3(ew_grid(R * bits)), dim3(256), (size_t)(0), st, ids, signs, R, bits);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(wgrad(dcodes, signs, (float*)grads->vq_out_w, R, D, bits, st));  // [dim, bits]: not worth a tensor-core launch
+    PHK_TRY(colsum(dcodes, R, D, D, (float*)grads->vq_out_b, st));
   }
   return 0;
 }

@@ -15,8 +15,8 @@ import torch
 from torch import nn
 
 from . import _lib as L
-from .modules import (ContinuousPositionBias, Keep, Transformer, Workspace, _NoParams, cpb_table,
-                      transformer_table, weights_signature)
+from .modules import (ContinuousPositionBias, GradKeep, Keep, Transformer, Workspace, _NoParams, cpb_grad_table,
+                      cpb_table, transformer_grad_table, transformer_table, weights_signature)
 
 
 def _pair(v):
@@ -361,8 +361,11 @@ class CViViT(nn.Module):
         if return_only_codebook_ids:
             return self.encode_ids(video)
         if return_recons_only:
-            # decode(project_out(sign(project_in(tokens)))) = decode(indices_to_codes(ids))  (cvivit.py:570-581)
-            recon = self.decode_from_codebook_indices(self.encode_ids(video))
+            # decode(project_out(sign(project_in(tokens)))) = decode(indices_to_codes(ids))  (cvivit.py:570-581).  No graph:
+            # in training mode the reference's gradient runs through LFQ's straight-through estimator into the encoder,
+            # which this module does not differentiate -- decoder-only gradients here would be silently wrong
+            with torch.no_grad():
+                recon = self.decode_from_codebook_indices(self.encode_ids(video))
             return recon.squeeze(2) if is_image else recon
         raise NotImplementedError("C-ViViT training losses (reconstruction / GAN / perceptual, cvivit.py:576-671) "
                                   "are out of scope of the H100 hot path (SURVEY.md section 2 row 8)")
@@ -388,9 +391,76 @@ class CViViT(nn.Module):
                     "phk_cvivit_decode")
         return video
 
+    def _decoder_params(self, with_project_out):
+        """The parameters a decode reaches (cvivit.py:437-443, 476-516): both decoder stacks, to_pixels*, the spatial
+        position-bias MLP it shares with the encoder and, for LFQ ids, vq.project_out."""
+        mods = [self.dec_temporal_transformer, self.dec_spatial_transformer, self.to_pixels_first_frame, self.to_pixels,
+                self.spatial_rel_pos_bias]
+        if with_project_out:
+            mods.append(self.vq.project_out)
+        return [p for m in mods for p in m.parameters()]
+
+    def _dec_grad_table(self, params, with_project_out):
+        """Zero-filled gradient buffers of ``params`` and the phk_cvivit_dec_t-shaped table that addresses them."""
+        gk = GradKeep(params)
+        t = L.CvivitDecT()
+        t.dim, t.heads, t.dim_head, t.channels = self.dim, self.heads, self.dim_head, self.channels
+        t.image_h, t.image_w = self.image_size
+        t.patch_h, t.patch_w = self.patch_size
+        t.patch_t = self.temporal_patch_size
+        if with_project_out:
+            t.codebook_bits = self.vq.codebook_dim
+            t.vq_out_w, t.vq_out_b = gk.g(self.vq.project_out.weight), gk.g(self.vq.project_out.bias)
+        t.spatial_bias = cpb_grad_table(self.spatial_rel_pos_bias, gk)
+        t.temporal = transformer_grad_table(self.dec_temporal_transformer, gk, False)
+        t.spatial = transformer_grad_table(self.dec_spatial_transformer, gk, False)
+        f, r = self.to_pixels_first_frame[0], self.to_pixels[0]
+        t.px_first_w, t.px_first_b = gk.g(f.weight), gk.g(f.bias)
+        t.px_w, t.px_b = gk.g(r.weight), gk.g(r.bias)  # (one latent frame: zeros, as autograd gives an empty batch)
+        return t, gk
+
+    def _differentiable_decode(self, ids, tokens, b, tp, device, taps=None):
+        """``_decode`` exactly as it runs under ``torch.no_grad`` and, when autograd wants a gradient of it (grad mode on,
+        and a decoder-side parameter or ``tokens`` requires grad), connected to phk_cvivit_decode_backward through
+        ``_DecodeFn``."""
+        def run():
+            return self._decode(ids, None if tokens is None else tokens.detach(), b, tp, device, taps)
+
+        params = self._decoder_params(ids is not None)
+        if not torch.is_grad_enabled() or not (any(p.requires_grad for p in params)
+                                               or (tokens is not None and tokens.requires_grad)):
+            return run()
+        spec = dict(net=self, params=params, b=b, tp=tp, precision=self.precision, sig=weights_signature(self))
+        return _DecodeFn.apply(run, spec, ids, tokens, *params)
+
+    def _decode_backward(self, spec, dvideo, ids, tokens, want_tokens_grad):
+        """phk_cvivit_decode_backward for one ``_differentiable_decode`` call: ([gradient or None per parameter of
+        spec["params"]], d tokens or None)."""
+        if weights_signature(self) != spec["sig"]:
+            raise RuntimeError("a parameter of this module was modified or replaced between the decode and the backward: "
+                               "the backward recomputes the decode from the current weights, so it would differentiate "
+                               "another function")
+        lib = L.lib()
+        dvideo = L.require_cuda(dvideo.to(torch.float32), "upstream gradient")
+        dev = dvideo.device
+        b, tp = spec["b"], spec["tp"]
+        prec = L.PREC_BF16 if spec["precision"] == L.PREC_BF16 else L.PREC_F32  # split-bf16 is an inference mode
+        with torch.cuda.device(dev):
+            table = self._dec_table()
+            gtable, gk = self._dec_grad_table(spec["params"], ids is not None)
+            dtokens = torch.empty_like(tokens) if tokens is not None and want_tokens_grad else None
+            nbytes = lib.phk_cvivit_decode_backward_workspace_bytes(C.byref(table), b, tp, prec)
+            ws = self._ws.get(nbytes, dev)
+            L.check(lib.phk_cvivit_decode_backward(C.byref(table), C.byref(gtable), L.ptr(ids), L.ptr(tokens), b, tp,
+                                                   L.ptr(dvideo), L.ptr(dtokens), L.ptr(ws), ws.numel(), prec,
+                                                   L.stream_ptr()),
+                    "phk_cvivit_decode_backward")
+        return [gk.grad_of(p) for p in spec["params"]], dtokens
+
     def decode_from_codebook_indices(self, indices, taps=None):
         """ids (b, n) or (b, t, h, w) int64 CUDA -> video (b, c, f, H, W) fp32 (cvivit.py:437-443): LFQ
-        indices_to_codes, decoder transformers and to_pixels, all inside phk_cvivit_decode."""
+        indices_to_codes, decoder transformers and to_pixels, all inside phk_cvivit_decode.  Differentiable with
+        respect to the decoder's parameters (and LFQ's project_out): see ``decode``."""
         indices = L.require_cuda(indices, "indices", torch.int64)
         b = indices.shape[0]
         n = indices[0].numel()
@@ -399,15 +469,40 @@ class CViViT(nn.Module):
         if not self.lookup_free_quantization:
             # codes = vq.codebook[indices] (cvivit.py:441): a row gather (data movement), then decode of float tokens
             codes = self.vq.codebook.index_select(0, indices.reshape(-1)).reshape(b, n, self.dim).contiguous()
-            return self._decode(None, codes, b, n // per, indices.device, taps)
-        return self._decode(indices.reshape(b, n), None, b, n // per, indices.device, taps)
+            return self._differentiable_decode(None, codes, b, n // per, indices.device, taps)
+        return self._differentiable_decode(indices.reshape(b, n), None, b, n // per, indices.device, taps)
 
     def decode(self, tokens):
-        """tokens (b, t, h, w, d) or (b, (t h w), d) fp32 CUDA -> video (cvivit.py:476-516)."""
+        """tokens (b, t, h, w, d) or (b, (t h w), d) fp32 CUDA -> video (cvivit.py:476-516).  Differentiable: with grad
+        mode on and a decoder-side parameter or ``tokens`` requiring grad, ``f(video).backward()`` fills their gradients
+        through phk_cvivit_decode_backward, which recomputes the decode with saved activations."""
         tokens = L.require_cuda(tokens, "tokens", torch.float32)
         b, d = tokens.shape[0], tokens.shape[-1]
         assert d == self.dim
         n = tokens[0].numel() // d
         per = self.image_num_tokens
         assert n > 0 and n % per == 0
-        return self._decode(None, tokens.reshape(b, n, d), b, n // per, tokens.device)
+        return self._differentiable_decode(None, tokens.reshape(b, n, d), b, n // per, tokens.device)
+
+
+class _DecodeFn(torch.autograd.Function):
+    """Makes the C-ViViT decode differentiable.  The forward runs the library's decode unchanged (same launches, same
+    values) and keeps only its inputs; the backward recomputes it with saved activations inside
+    phk_cvivit_decode_backward, as activation checkpointing does.  The decode applies no dropout (DESIGN.md section 8),
+    so the backward applies none either: it differentiates the function the forward returned."""
+
+    @staticmethod
+    def forward(ctx, run, spec, ids, tokens, *params):
+        ctx.spec = spec
+        ctx.save_for_backward(ids, None if tokens is None else tokens.detach())
+        return run()
+
+    @staticmethod
+    def backward(ctx, dvideo):
+        if torch.is_grad_enabled():
+            raise RuntimeError("CViViT.decode does not support create_graph=True: its backward is hand-written CUDA and "
+                               "builds no graph of its own")
+        ids, tokens = ctx.saved_tensors
+        spec = ctx.spec
+        grads, dtokens = spec["net"]._decode_backward(spec, dvideo, ids, tokens, ctx.needs_input_grad[3])
+        return (None, None, None, dtokens, *grads)
