@@ -437,6 +437,38 @@ int phk_cvivit_decode_backward(const phk_cvivit_dec_t* m, const phk_cvivit_dec_t
                                const float* tokens, int32_t B, int32_t Tp, const float* dvideo, float* dtokens,
                                void* workspace, int64_t workspace_bytes, int32_t prec, phk_stream_t s);
 
+/* The reconstruction loss of CViViT.forward with use_vgg_and_gan=False (cvivit.py:584-590): F.mse_loss(video, recon), or
+ * with a frame mask the mean of the squared error over the selected frames (sum / (selected frames * C * H * W); an
+ * all-false mask gives NaN, as the reference does).  video / recon fp32 (B, C, F, H, W); frame_mask NULL or uint8 (B, F);
+ * scratch >= PHK_RECON_LOSS_SCRATCH_BYTES; loss_out one fp32 (device).  Fixed-order reduction without atomics: two calls
+ * give bit-identical losses. */
+#define PHK_RECON_LOSS_SCRATCH_BYTES 2048
+int phk_cvivit_recon_loss(const float* video, const float* recon, const uint8_t* frame_mask, int32_t B, int32_t C,
+                          int32_t F, int32_t H, int32_t W, void* scratch, float* loss_out, phk_stream_t s);
+
+/* Backward of `loss = CViViT(video, mask)` (use_vgg_and_gan=False, LFQ) for d loss and an optional d recon, as the
+ * reference's autograd computes it: d recon = d loss 2 / N mask (recon - video) + drecon, then the decoder backward of
+ * phk_cvivit_decode_backward from the FORWARD's ids, then LFQ: project_out's gradients and, with straight_through
+ * (training mode, upstream LFQ's x + (q - x).detach()), d x = d q = d z_dec W_out into project_in, the encoder's temporal
+ * and spatial stacks and to_patch_emb* (recomputed with saved activations), and finally the spatial_rel_pos_bias MLP over
+ * the bias gradient of both spatial stacks.  Without straight_through (eval mode) the encoder side gets nothing.
+ *   enc / dec          the weight tables of the forward (phk_cvivit_encode / phk_cvivit_decode)
+ *   enc_grads / dec_grads  tables of the same layouts addressing ZERO-FILLED gradient buffers, ACCUMULATED: the
+ *                      position-bias MLP's gradient goes to dec_grads->spatial_bias (enc_grads->spatial_bias is not used);
+ *                      with one latent frame the to_patch_emb / to_pixels gradients stay zero (empty batches)
+ *   video, recon       fp32 (B, C, F, H, W): the forward's input and reconstruction; ids the forward's (B, T', h, w) ids
+ *   frame_mask         NULL or uint8 (B, F), as for phk_cvivit_recon_loss
+ *   dloss              ONE fp32 on the device (the backward never synchronises the host); drecon NULL or like recon
+ *   dvideo             NULL, or fp32 like video: receives d loss / d video (written, not added)
+ * prec: PHK_PREC_F32 or PHK_PREC_BF16 (the training step's bf16 products); no dropout is applied. */
+int64_t phk_cvivit_backward_workspace_bytes(const phk_cvivit_t* enc, const phk_cvivit_dec_t* dec, int32_t B, int32_t F,
+                                            int32_t prec);
+int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* enc_grads, const phk_cvivit_dec_t* dec,
+                        const phk_cvivit_dec_t* dec_grads, const float* video, const float* recon, const int64_t* ids,
+                        const uint8_t* frame_mask, int32_t B, int32_t F, const float* dloss, const float* drecon,
+                        float* dvideo, int32_t straight_through, void* workspace, int64_t workspace_bytes, int32_t prec,
+                        phk_stream_t s);
+
 /* context_norm + to_kv of every cross-attention layer (attention.py:137-144).  Depends only on
  * the text embedding, so Phenaki.sample computes it once per call instead of once per forward.
  * context (b,L,dim_context) fp32; out_kv [depth, b*L, 2*heads*dim_head] fp32;

@@ -9,6 +9,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PHK_LIB") or os.path.join(_HERE, "libphk.so")  # PHK_LIB: an A/B build of the same ABI (tools/ only)
 
 PREC_F32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
+RECON_LOSS_SCRATCH_BYTES = 2048  # PHK_RECON_LOSS_SCRATCH_BYTES (include/phk.h)
 HEAD_LOGITS, HEAD_EMBEDS, HEAD_SCORE = 0, 1, 2  # phk_maskgit_backward head kinds
 
 
@@ -185,9 +186,13 @@ PROTOTYPES = {
     "phk_cvivit_decode_backward_workspace_bytes": [C.POINTER(CvivitDecT), i32, i32, i32],
     "phk_cvivit_decode_backward": [C.POINTER(CvivitDecT), C.POINTER(CvivitDecT), vp, vp, i32, i32, vp, vp, vp, i64, i32,
                                    vp],
+    "phk_cvivit_recon_loss": [vp, vp, vp, i32, i32, i32, i32, i32, vp, vp, vp],
+    "phk_cvivit_backward_workspace_bytes": [C.POINTER(CvivitT), C.POINTER(CvivitDecT), i32, i32, i32],
+    "phk_cvivit_backward": [C.POINTER(CvivitT), C.POINTER(CvivitT), C.POINTER(CvivitDecT), C.POINTER(CvivitDecT), vp, vp,
+                            vp, vp, i32, i32, vp, vp, vp, i32, vp, i64, i32, vp],
 }
 _RESTYPES = {"phk_attention_tc_scratch_bytes": i64, "phk_head_sample_scratch_bytes": i64,
-             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_maskgit_train_dropout_counters": i64, "phk_maskgit_backward_workspace_bytes": i64, "phk_cvivit_decode_backward_workspace_bytes": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
+             "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_maskgit_train_dropout_counters": i64, "phk_maskgit_backward_workspace_bytes": i64, "phk_cvivit_decode_backward_workspace_bytes": i64, "phk_cvivit_backward_workspace_bytes": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,
              "phk_cvivit_workspace_bytes": i64, "phk_cvivit_decode_workspace_bytes": i64, "phk_maskgit_workspace_bytes": i64}
 
 FAMILIES = ["patchify_ln", "layernorm", "gemm_f32", "gemm_bf16", "attention", "peg", "geglu", "lfq", "embed",

@@ -14,8 +14,8 @@
 // against the reference there.  In bf16 mode the products run on the tensor-core GEMM instead (see below).
 // With dropout (phk_dropout_t) the masks are regenerated from Philox counters wherever they are needed, never stored.
 // Checked against the reference's gradients on the CPU by tests/cuda_emu (this very source, g++-compiled) and on the GPU
-// by tests/test_gpu_train.py.  The same layer code differentiates the C-ViViT decoder (phk_cvivit_decode_backward, at the
-// end of this file).
+// by tests/test_gpu_train.py.  The same layer code differentiates the C-ViViT decoder (phk_cvivit_decode_backward) and the
+// tokenizer's reconstruction loss through decoder, LFQ and encoder (phk_cvivit_backward), at the end of this file.
 #include "phk_common.cuh"
 // the kernels of this file are ordinary stream-ordered launches (they do not use programmatic dependent launch)
 #define PHK_KERNEL_LAUNCH(kernel, grid, block, smem, st, ...) PHK_CUDA(launch_plain(kernel, grid, block, smem, st, __VA_ARGS__))
@@ -1278,7 +1278,8 @@ void step_init(Step& S) {
 // ------------------------------------------------------------------------------------------------------------------
 // One transformer layer (attention.py:311-330): forward keeping its activations, and backward.  Shared by every stack
 // whose sequences are runs of n contiguous rows: MaskGit / TokenCritic (b videos of n tokens, PEG over (pt, ph, pw),
-// cross-attention to the text) and the two stacks of the C-ViViT decoder (phk_cvivit_decode_backward).
+// cross-attention to the text) and the stacks of the C-ViViT encoder and decoder (phk_cvivit_backward,
+// phk_cvivit_decode_backward).
 // ------------------------------------------------------------------------------------------------------------------
 struct LayerCall {
   const phk_transformer_t* T = nullptr;    // weights
@@ -1890,7 +1891,8 @@ extern "C" int phk_maskgit_backward(const phk_maskgit_t* m, const phk_maskgit_t*
 //   to_pixels       norm_out gathered into first-frame / remaining-frame rows as the forward does; d video gathered into
 //                   the same patch layout (the adjoint of phk_unpatchify); wgrad, bias column sum, dgrad per Linear
 //   project_out     (ids) wgrad against the +-1 codes rebuilt from the ids and the bias column sum; the ids get nothing
-// No dropout: the decode forward applies none.
+// No dropout: the decode forward applies none.  phk_cvivit_backward runs the same decoder phase from d recon, then LFQ
+// and the encoder's stacks and patch embeddings (DESIGN.md section 7.3).
 // ------------------------------------------------------------------------------------------------------------------
 namespace phk {
 namespace {
@@ -1966,58 +1968,385 @@ __global__ void lfq_signs_kernel(const int64_t* __restrict__ ids, float* __restr
   }
 }
 
+// video[b, c, f0 + t pt + k, y p1 + i, x p2 + j] += rows[((b nt + t) hh + y) ww + x, ((c pt + k) p1 + i) p2 + j]: the
+// adjoint of patch_gather_kernel.  Patches tile the frames they cover, so every video element gets at most one term.
+__global__ void patch_scatter_add_kernel(const float* __restrict__ rows, float* __restrict__ video, int B, int C, int F,
+                                         int H, int W, int f0, int nt, int pt, int p1, int p2) {
+  const int hh = H / p1, ww = W / p2, K = C * pt * p1 * p2;
+  const int64_t total = (int64_t)B * nt * hh * ww * K;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / K;
+    const int e = (int)(i - r * K);
+    const int x = (int)(r % ww), y = (int)((r / ww) % hh), t = (int)((r / ((int64_t)ww * hh)) % nt);
+    const int64_t b = r / ((int64_t)ww * hh * nt);
+    const int j = e % p2, ii = (e / p2) % p1, k = (e / (p2 * p1)) % pt, c = e / (p2 * p1 * pt);
+    video[(((b * C + c) * F + f0 + (int64_t)t * pt + k) * H + (int64_t)y * p1 + ii) * W + (int64_t)x * p2 + j] += rows[i];
+  }
+}
+
+// first[b hw + s] = full[(b Tp) hw + s], rest[(b (Tp - 1) + t - 1) hw + s] = full[(b Tp + t) hw + s] (t > 0), rows of D
+// floats: the adjoint of frames_merge_kernel
+__global__ void frames_split_kernel(const float* __restrict__ full, float* __restrict__ first, float* __restrict__ rest,
+                                    int B, int Tp, int hw, int D) {
+  const int64_t total = (int64_t)B * Tp * hw * D;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / D;
+    const int d = (int)(i - r * D);
+    const int s = (int)(r % hw);
+    const int t = (int)((r / hw) % Tp);
+    const int64_t b = r / ((int64_t)hw * Tp);
+    if (t == 0) first[(b * hw + s) * D + d] = full[i];
+    else rest[((b * (Tp - 1) + t - 1) * hw + s) * D + d] = full[i];
+  }
+}
+
+// Number of (B, F) frames a frame mask selects (NULL: all of them), counted by one thread in a fixed order
+__device__ int64_t selected_frames(const uint8_t* __restrict__ mask, int B, int F) {
+  if (!mask) return (int64_t)B * F;
+  int64_t n = 0;
+  for (int i = 0; i < B * F; ++i) n += mask[i] != 0;
+  return n;
+}
+
+// Reconstruction loss (cvivit.py:584-590) over a (B, C, F, H, W) video: per-block fp64 partial sums of the masked squared
+// error over a fixed grid, then one block adds the partials in a fixed order.  No atomics: two calls give bit-identical
+// losses.
+constexpr int kLossBlocks = PHK_RECON_LOSS_SCRATCH_BYTES / 8;
+
+__global__ void __launch_bounds__(256) recon_loss_partial_kernel(const float* __restrict__ video,
+                                                                 const float* __restrict__ recon,
+                                                                 const uint8_t* __restrict__ mask, int C, int F,
+                                                                 int64_t frame_elems, int64_t total,
+                                                                 double* __restrict__ partial) {
+  __shared__ double red[256];
+  double a = 0.0;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    if (mask) {
+      const int64_t fr = i / frame_elems;  // ((b C + c) F + f)
+      if (!mask[(fr / ((int64_t)C * F)) * F + fr % F]) continue;
+    }
+    const float d = recon[i] - video[i];
+    a += (double)d * d;
+  }
+  red[threadIdx.x] = a;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) partial[blockIdx.x] = red[0];
+}
+
+__global__ void __launch_bounds__(256) recon_loss_final_kernel(const double* __restrict__ partial,
+                                                               const uint8_t* __restrict__ mask, int B, int C, int F,
+                                                               int64_t frame_elems, float* __restrict__ loss) {
+  __shared__ double red[256];
+  double a = 0.0;
+  for (int i = threadIdx.x; i < kLossBlocks; i += blockDim.x) a += partial[i];
+  red[threadIdx.x] = a;
+  __syncthreads();
+  for (int w = 128; w > 0; w >>= 1) {
+    if ((int)threadIdx.x < w) red[threadIdx.x] += red[threadIdx.x + w];
+    __syncthreads();
+  }
+  // an all-false mask gives 0 / 0 = NaN, as the reference's mean over an empty selection does
+  if (threadIdx.x == 0) *loss = (float)(red[0] / ((double)selected_frames(mask, B, F) * C * frame_elems));
+}
+
+// d recon = dloss 2 / N mask (recon - video) (+ the caller's d recon); d video = -(the same MSE term) (NULL: not wanted).
+// N = selected frames C H W; with nothing selected the MSE term is zero (the reference's mean over an empty selection
+// sends no gradient).
+__global__ void __launch_bounds__(256) recon_grad_kernel(const float* __restrict__ video, const float* __restrict__ recon,
+                                                         const uint8_t* __restrict__ mask, const float* __restrict__ dloss,
+                                                         const float* __restrict__ drecon_in, float* __restrict__ drecon,
+                                                         float* __restrict__ dvideo, int B, int C, int F,
+                                                         int64_t frame_elems) {
+  __shared__ float scale;
+  if (threadIdx.x == 0) {
+    const int64_t n = selected_frames(mask, B, F);
+    scale = n > 0 ? (float)(2.0 * (double)*dloss / ((double)n * C * frame_elems)) : 0.f;
+  }
+  __syncthreads();
+  const int64_t total = (int64_t)B * C * F * frame_elems;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    bool on = true;
+    if (mask) {
+      const int64_t fr = i / frame_elems;
+      on = mask[(fr / ((int64_t)C * F)) * F + fr % F] != 0;
+    }
+    const float g = on ? scale * (recon[i] - video[i]) : 0.f;
+    drecon[i] = drecon_in ? g + drecon_in[i] : g;
+    if (dvideo) dvideo[i] = -g;
+  }
+}
+
 int64_t stack_inner(const phk_transformer_t* T) {
   int64_t inner = 0;
   for (int l = 0; l < T->depth; ++l) inner = T->layers[l].ff.inner > inner ? T->layers[l].ff.inner : inner;
   return inner;
 }
 
-// one bf16 operand buffer of the decoder's tensor-core products (see tc_scratch_elems): every [rows, width] operand,
-// straight or transposed, with width up to K2 = C pt p1 p2 (the to_pixels output)
-int64_t dec_tc_scratch_elems(const phk_cvivit_dec_t* m, int64_t R, int64_t K2) {
-  const int64_t inner = stack_inner(&m->temporal) > stack_inner(&m->spatial) ? stack_inner(&m->temporal) : stack_inner(&m->spatial);
-  const int64_t I = (int64_t)m->heads * m->dim_head, D = m->dim;
-  int64_t width = 2 * inner;
-  if (2 * I > width) width = 2 * I;
-  if (D > width) width = D;
-  if (K2 > width) width = K2;
-  int64_t feat = D;
-  if (I > feat) feat = I;
-  if (inner > feat) feat = inner;
-  const int64_t tokens = pad8(R) + 8;
-  return (tokens > feat + 8 ? tokens : feat + 8) * (width + 8);
+int64_t imax(int64_t a, int64_t b) { return a > b ? a : b; }
+
+// Shapes of one C-ViViT backward: B videos of T' latent frames of hh x ww patches; R = B T' hh ww token rows;
+// rows1 / rows2 = the first-frame / remaining-frame rows; K1 / K2 = their patch widths; inner = the widest FF
+struct CvGeom {
+  int B = 0, Tp = 0, hh = 0, ww = 0, hw = 0, D = 0, H = 0, DH = 0, I = 0, C = 0, F = 0;
+  int64_t R = 0, rows1 = 0, rows2 = 0, K1 = 0, K2 = 0, inner = 0;
+};
+
+CvGeom cv_geom(const phk_cvivit_dec_t* m, int B, int Tp, int64_t inner) {
+  CvGeom g;
+  g.B = B; g.Tp = Tp; g.hh = m->image_h / m->patch_h; g.ww = m->image_w / m->patch_w; g.hw = g.hh * g.ww;
+  g.D = m->dim; g.H = m->heads; g.DH = m->dim_head; g.I = g.H * g.DH; g.C = m->channels; g.F = 1 + (Tp - 1) * m->patch_t;
+  g.R = (int64_t)B * Tp * g.hw; g.rows1 = (int64_t)B * g.hw; g.rows2 = (int64_t)B * (Tp - 1) * g.hw;
+  g.K1 = (int64_t)g.C * m->patch_h * m->patch_w; g.K2 = g.K1 * m->patch_t; g.inner = inner;
+  return g;
+}
+
+// one bf16 operand buffer of the C-ViViT backward's tensor-core products (see tc_scratch_elems): every [rows, width]
+// operand, straight or transposed, with width up to K2 = C pt p1 p2 (to_pixels / to_patch_emb)
+int64_t cv_tc_scratch_elems(const CvGeom& g) {
+  const int64_t width = imax(imax(2 * g.inner, 2 * (int64_t)g.I), imax(g.D, g.K2));
+  const int64_t feat = imax(imax(g.D, g.I), g.inner);
+  const int64_t tokens = pad8(g.R) + 8;
+  return imax(tokens, feat + 8) * (width + 8);
+}
+
+// Buffers of a C-ViViT backward that every phase uses: the tensor-core operand scratch, the constant attention biases,
+// the spatial position bias and its gradient (accumulated by every spatial stack), the attention and position-bias
+// scratch, the two gradient streams dx / dx_alt and the layers' gradient scratch
+struct CvShared {
+  TcScratch tc{nullptr, nullptr, 0};
+  float *bias_t = nullptr, *bias_s = nullptr, *dbias_s = nullptr, *cpb_sc = nullptr, *cpb_bwd_sc = nullptr, *asc = nullptr;
+  float *dx = nullptr, *dx_alt = nullptr;
+  LayerGrads G{};
+};
+
+int64_t cv_shared_floats(const CvGeom& g, const phk_cpb_t& cpb) {
+  const int64_t a1 = attn_bwd_scratch_floats(g.B * g.hw, g.H, g.Tp, g.Tp, g.DH);
+  const int64_t a2 = attn_bwd_scratch_floats(g.B * g.Tp, g.H, g.hw, g.hw, g.DH);
+  int64_t f = (int64_t)g.H * g.Tp * g.Tp + 2 * (int64_t)g.H * g.hw * g.hw;       // biases, d spatial bias
+  f += phk_cpb_scratch_floats(&cpb, g.hh, g.ww, 1) + cpb_bwd_scratch_floats(cpb, g.hh, g.ww, 1) + imax(a1, a2);
+  f += 2 * g.R * g.D;                                                             // dx, dx_alt
+  f += g.R * (g.D + 4 * (int64_t)g.I + 3 * g.inner) + 2 * g.R;                    // dtmp | dq dkv(2) dob | dh(2) dg | stats
+  return f;
+}
+int64_t cv_shared_bytes(const CvGeom& g, const phk_cpb_t& cpb, int prec) {
+  int64_t bytes = cv_shared_floats(g, cpb) * 4 + 256 * 24;
+  if (prec == PHK_PREC_BF16) bytes += 2 * (cv_tc_scratch_elems(g) * 2 + 256);
+  return bytes;
+}
+
+// Takes the shared buffers from `ar`, computes the spatial position bias and zeroes its gradient.
+int cv_shared_init(Arena& ar, const CvGeom& g, const phk_cpb_t& cpb, int prec, phk_stream_t s, CvShared& S) {
+  if (prec == PHK_PREC_BF16) {
+    S.tc.elems = cv_tc_scratch_elems(g);
+    S.tc.a = reinterpret_cast<__nv_bfloat16*>(ar.f((S.tc.elems + 1) / 2));
+    S.tc.b = reinterpret_cast<__nv_bfloat16*>(ar.f((S.tc.elems + 1) / 2));
+    PHK_REQUIRE(S.tc.a && S.tc.b, PHK_E_WORKSPACE, "cvivit backward: workspace too small (tensor-core operands)");
+  }
+  const int64_t a1 = attn_bwd_scratch_floats(g.B * g.hw, g.H, g.Tp, g.Tp, g.DH);
+  const int64_t a2 = attn_bwd_scratch_floats(g.B * g.Tp, g.H, g.hw, g.hw, g.DH);
+  S.bias_t = ar.f((int64_t)g.H * g.Tp * g.Tp);
+  S.bias_s = ar.f((int64_t)g.H * g.hw * g.hw);
+  S.dbias_s = ar.f((int64_t)g.H * g.hw * g.hw);
+  S.cpb_sc = ar.f(phk_cpb_scratch_floats(&cpb, g.hh, g.ww, 1));
+  S.cpb_bwd_sc = ar.f(cpb_bwd_scratch_floats(cpb, g.hh, g.ww, 1));
+  S.asc = ar.f(imax(a1, a2));
+  S.dx = ar.f(g.R * g.D);
+  S.dx_alt = ar.f(g.R * g.D);
+  LayerGrads& G = S.G;
+  G.dtmp = ar.f(g.R * g.D); G.dq = ar.f(g.R * g.I); G.dkv = ar.f(g.R * 2 * g.I); G.dob = ar.f(g.R * g.I);
+  G.dh = ar.f(g.R * 2 * g.inner); G.dg = ar.f(g.R * g.inner); G.dckv = nullptr; G.dctxn = nullptr;
+  G.stats = reinterpret_cast<float2*>(ar.f(2 * g.R));
+  PHK_REQUIRE(S.bias_t && S.bias_s && S.dbias_s && S.cpb_sc && S.cpb_bwd_sc && S.asc && S.dx && S.dx_alt && G.dtmp && G.dq &&
+              G.dkv && G.dob && G.dh && G.dg && G.stats, PHK_E_WORKSPACE, "cvivit backward: workspace too small");
+  PHK_TRY(phk_cpb_bias(&cpb, g.hh, g.ww, 1, S.cpb_sc, S.bias_s, s));
+  PHK_CUDA(cudaMemsetAsync(S.dbias_s, 0, (int64_t)g.H * g.hw * g.hw * 4, to_stream(s)));
+  return 0;
+}
+
+// The temporal stack of C-ViViT (encoder or decoder) on (b h w t) rows: B h w sequences of T' rows, layout-0 PEG over
+// (B, T', h, w) (the reference's raw reshape of these rows), ALiBi plus the causal fill as one constant bias, written
+// into S.bias_t here
+int temporal_call(const phk_transformer_t* T, const phk_transformer_t* GT, const CvGeom& g, const CvShared& S, int prec,
+                  phk_stream_t s, LayerCall* c) {
+  *c = LayerCall();
+  c->T = T; c->GT = GT; c->b = g.B * g.hw; c->n = g.Tp;
+  c->pegB = g.B; c->pegT = g.Tp; c->pegH = g.hh; c->pegW = g.ww;
+  c->bias = S.bias_t; c->prec = prec; c->s = s; c->st = to_stream(s); c->tc = S.tc; c->asc = S.asc;
+  PHK_KERNEL_LAUNCH(alibi_causal_bias_kernel, dim3(ew_grid((int64_t)g.H * g.Tp * g.Tp)), dim3(256), (size_t)(0), c->st, T->alibi_slopes, S.bias_t, g.H, g.Tp);
+  PHK_LAUNCH_CHECK();
+  return 0;
+}
+
+// The spatial stack on (b t h w) rows: B T' sequences of h w rows, no PEG, the 2-D position bias (its gradient
+// accumulates into S.dbias_s)
+LayerCall spatial_call(const phk_transformer_t* T, const phk_transformer_t* GT, const CvGeom& g, const CvShared& S,
+                       int prec, phk_stream_t s) {
+  LayerCall c;
+  c.T = T; c.GT = GT; c.b = g.B * g.Tp; c.n = g.hw;
+  c.pegB = g.B; c.pegT = g.Tp; c.pegH = g.hh; c.pegW = g.ww;
+  c.bias = S.bias_s; c.dbias = S.dbias_s; c.prec = prec; c.s = s; c.st = to_stream(s); c.tc = S.tc; c.asc = S.asc;
+  return c;
+}
+
+// Every layer of c.T on x (saving activations into sv[depth]); *xf = the stack's output before norm_out
+int stack_forward(const LayerCall& c, const float* x, LayerSave* sv, const float** xf, Arena& ar) {
+  const DropSite none{0.f, 0.f, 0u, 0u, 0u};
+  for (int l = 0; l < c.T->depth; ++l) {
+    float* xout = nullptr;
+    PHK_TRY(layer_forward(c, l, x, sv[l], &xout, ar, none, none, none));
+    x = xout;
+  }
+  *xf = x;
+  return 0;
+}
+
+// Backward of norm_out(stack(x)) from dy = d/d(norm_out output): on return *dx holds d/d(x) (*dx, *dx_alt may swap)
+int stack_backward(const LayerCall& c, const LayerSave* sv, const float* xf, const float* dy, float** dx, float** dx_alt,
+                   const LayerGrads& G) {
+  const DropSite none{0.f, 0.f, 0u, 0u, 0u};
+  const int64_t R = (int64_t)c.b * c.n;
+  PHK_TRY(ln_backward(xf, c.T->out_g, dy, *dx, 0, (float*)c.GT->out_g, nullptr, G.stats, R, c.T->dim, c.st));
+  for (int l = c.T->depth - 1; l >= 0; --l) PHK_TRY(layer_backward(c, l, sv[l], dx, dx_alt, G, nullptr, none, none, none));
+  return 0;
+}
+
+int64_t dec_phase_floats(const phk_cvivit_dec_t* m, const CvGeom& g) {
+  int64_t f = 2 * g.R * g.D;                                                     // codes (b t h w), their (b h w t) copy
+  for (int l = 0; l < m->temporal.depth; ++l) f += layer_save_floats(&m->temporal, m->temporal.layers[l], g.R, 0);
+  for (int l = 0; l < m->spatial.depth; ++l) f += layer_save_floats(&m->spatial, m->spatial.layers[l], g.R, 0);
+  f += 2 * g.R * g.D;                                                            // temporal norm_out (b h w t), spatial input
+  f += 2 * (g.rows1 + imax(g.rows2, 1)) * g.D;                                   // spatial norm_out and its gradient, split
+  f += imax(g.rows1 * g.K1, g.rows2 * g.K2);                                     // d video in a patch layout
+  f += g.R * imax(m->codebook_bits, 1);                                          // +-1 codes
+  return f + 256 * 16 / 4;
+}
+
+// The decoder half of both backward entry points: recomputes the decode with its activations saved in `ar` (a copy: all
+// of it is dead on return) and differentiates it from d video.  With ids, project_out's gradients are accumulated.
+// cpb_now: finish the position-bias MLP's gradient here; otherwise S.dbias_s is left to the caller.  dcodes_out (or
+// dtokens): receives d/d(decoder input) in (b t h w) rows, in dtokens when given, else in a free gradient stream of S.
+int decode_backward_phase(const phk_cvivit_dec_t* m, const phk_cvivit_dec_t* grads, const int64_t* ids, const float* tokens,
+                          const CvGeom& g, const float* dvideo, float* dtokens, const float** dcodes_out, const CvShared& S,
+                          Arena ar, bool cpb_now, int prec, phk_stream_t s) {
+  const phk_transformer_t* TT = &m->temporal;
+  const phk_transformer_t* TS = &m->spatial;
+  const int B = g.B, Tp = g.Tp, hw = g.hw, D = g.D, C = g.C, F = g.F;
+  const int64_t R = g.R, per = (int64_t)Tp * hw, K1 = g.K1, K2 = g.K2, rows1 = g.rows1, rows2 = g.rows2;
+  const cudaStream_t st = to_stream(s);
+  float* xc = ar.f(R * D);
+  float* xp = ar.f(R * D);
+  PHK_REQUIRE(xc && xp, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
+
+  // ---------------------------------------------------------------- inputs
+  const float* x_in = tokens;
+  if (ids) {
+    PHK_TRY(phk_lfq_codes(ids, m->vq_out_w, m->vq_out_b, xc, R, D, m->codebook_bits, s));
+    x_in = xc;
+  }
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, x_in, xp, B, Tp, hw, D, 1);
+  PHK_LAUNCH_CHECK();
+
+  // ---------------------------------------------------------------- forward, saving activations
+  LayerCall ct;
+  PHK_TRY(temporal_call(TT, &grads->temporal, g, S, prec, s, &ct));
+  const LayerCall cs = spatial_call(TS, &grads->spatial, g, S, prec, s);
+  std::unique_ptr<LayerSave[]> svT(new (std::nothrow) LayerSave[TT->depth]), svS(new (std::nothrow) LayerSave[TS->depth]);
+  PHK_REQUIRE(svT && svS, PHK_E_ARG, "cvivit_decode_backward: out of host memory");
+  const float* xfT = nullptr;
+  PHK_TRY(stack_forward(ct, xp, svT.get(), &xfT, ar));
+  float* nT = ar.f(R * D);
+  float* P = ar.f(R * D);
+  PHK_REQUIRE(nT && P, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
+  PHK_TRY(phk_layernorm(xfT, TT->out_g, TT->out_b, nT, nullptr, R, D, 0, 0, 0, 0, s));
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, nT, P, B, Tp, hw, D, 0);
+  PHK_LAUNCH_CHECK();
+  const float* xfS = nullptr;
+  PHK_TRY(stack_forward(cs, P, svS.get(), &xfS, ar));
+  float* Ef = ar.f(rows1 * D);
+  float* Er = ar.f((rows2 > 0 ? rows2 : 1) * D);
+  PHK_REQUIRE(Ef && Er, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
+  PHK_TRY(phk_layernorm(xfS, TS->out_g, TS->out_b, Ef, nullptr, rows1, D, 0, -hw, per, 0, s));
+  if (Tp > 1) PHK_TRY(phk_layernorm(xfS, TS->out_g, TS->out_b, Er, nullptr, rows2, D, 0, -(per - hw), per, hw, s));
+
+  // ---------------------------------------------------------------- to_pixels_first_frame / to_pixels
+  const LayerGrads& G = S.G;
+  float* dx = S.dx;
+  float* dx_alt = S.dx_alt;
+  float* dG = ar.f(imax(rows1 * K1, rows2 * K2));
+  float* dEf = ar.f(rows1 * D);
+  float* dEr = ar.f((rows2 > 0 ? rows2 : 1) * D);
+  PHK_REQUIRE(dG && dEf && dEr, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small (gradients)");
+  PHK_KERNEL_LAUNCH(patch_gather_kernel, dim3(ew_grid(rows1 * K1)), dim3(256), (size_t)(0), st, dvideo, dG, B, C, F, m->image_h, m->image_w, 0, 1, 1, m->patch_h, m->patch_w);
+  PHK_LAUNCH_CHECK();
+  PHK_TRY(wgrad_p(prec, S.tc, dG, Ef, (float*)grads->px_first_w, rows1, K1, D, s));
+  PHK_TRY(colsum(dG, rows1, (int)K1, K1, (float*)grads->px_first_b, st));
+  PHK_TRY(dgrad_p(prec, S.tc, dG, m->px_first_w, dEf, rows1, K1, D, 0, s));
+  if (Tp > 1) {  // (one latent frame: to_pixels sees an empty batch, its gradients stay the caller's zeros)
+    PHK_KERNEL_LAUNCH(patch_gather_kernel, dim3(ew_grid(rows2 * K2)), dim3(256), (size_t)(0), st, dvideo, dG, B, C, F, m->image_h, m->image_w, 1, Tp - 1, m->patch_t, m->patch_h, m->patch_w);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(wgrad_p(prec, S.tc, dG, Er, (float*)grads->px_w, rows2, K2, D, s));
+    PHK_TRY(colsum(dG, rows2, (int)K2, K2, (float*)grads->px_b, st));
+    PHK_TRY(dgrad_p(prec, S.tc, dG, m->px_w, dEr, rows2, K2, D, 0, s));
+  }
+  PHK_KERNEL_LAUNCH(frames_merge_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dEf, dEr, G.dtmp, B, Tp, hw, D);
+  PHK_LAUNCH_CHECK();
+
+  // ---------------------------------------------------------------- spatial stack, position-bias MLP
+  PHK_TRY(stack_backward(cs, svS.get(), xfS, G.dtmp, &dx, &dx_alt, G));
+  if (cpb_now) PHK_TRY(cpb_backward(m->spatial_bias, grads->spatial_bias, S.dbias_s, g.hh, g.ww, 1, S.cpb_bwd_sc, st));
+
+  // ---------------------------------------------------------------- temporal stack, rows (b h w t)
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 1);
+  PHK_LAUNCH_CHECK();
+  PHK_TRY(stack_backward(ct, svT.get(), xfT, G.dtmp, &dx, &dx_alt, G));
+
+  // ---------------------------------------------------------------- d tokens / project_out
+  if (!ids && !dtokens && !dcodes_out) return 0;
+  float* dcodes = dtokens ? dtokens : dx_alt;
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, dcodes, B, Tp, hw, D, 0);
+  PHK_LAUNCH_CHECK();
+  if (dcodes_out) *dcodes_out = dcodes;
+  if (ids) {
+    const int bits = m->codebook_bits;
+    float* signs = ar.f(R * bits);
+    PHK_REQUIRE(signs, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small (codes)");
+    PHK_KERNEL_LAUNCH(lfq_signs_kernel, dim3(ew_grid(R * bits)), dim3(256), (size_t)(0), st, ids, signs, R, bits);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(wgrad(dcodes, signs, (float*)grads->vq_out_w, R, D, bits, st));  // [dim, bits]: not worth a tensor-core launch
+    PHK_TRY(colsum(dcodes, R, D, D, (float*)grads->vq_out_b, st));
+  }
+  return 0;
+}
+
+int64_t enc_phase_floats(const phk_cvivit_t* m, const CvGeom& g, bool dvideo) {
+  const int64_t rows2 = imax(g.rows2, 1);
+  const int64_t patch = imax(g.rows1 * g.K1, g.rows2 * g.K2);
+  int64_t f = 2 * (g.rows1 * g.K1 + rows2 * g.K2);                               // raw patch rows, LN1 outputs
+  f += (g.rows1 + rows2) * g.D + g.R * g.D;                                      // Linear outputs, LN2 outputs (b t h w)
+  for (int l = 0; l < m->spatial.depth; ++l) f += layer_save_floats(&m->spatial, m->spatial.layers[l], g.R, 0);
+  for (int l = 0; l < m->temporal.depth; ++l) f += layer_save_floats(&m->temporal, m->temporal.layers[l], g.R, 0);
+  f += 4 * g.R * g.D;                                                            // norm_outs and their permuted copies
+  f += (g.rows1 + rows2) * g.D + imax(g.rows1, rows2) * g.D;                     // d LN2 outputs split, d Linear outputs
+  f += patch * (dvideo ? 2 : 1);                                                 // d LN1 outputs, d patch rows
+  return f + 256 * 24 / 4;
+}
+
+bool cvivit_shapes_ok(const phk_cvivit_dec_t* m, int32_t B, int32_t Tp) {
+  return m && B > 0 && Tp > 0 && m->temporal.layers && m->spatial.layers && m->temporal.depth > 0 && m->spatial.depth > 0 &&
+         m->patch_h > 0 && m->patch_w > 0 && m->patch_t > 0 && m->image_h % m->patch_h == 0 && m->image_w % m->patch_w == 0;
 }
 
 }  // namespace
 }  // namespace phk
 
 extern "C" int64_t phk_cvivit_decode_backward_workspace_bytes(const phk_cvivit_dec_t* m, int32_t B, int32_t Tp, int32_t prec) {
-  if (!m || B <= 0 || Tp <= 0 || !m->temporal.layers || !m->spatial.layers || m->temporal.depth <= 0 ||
-      m->spatial.depth <= 0 || m->patch_h <= 0 || m->patch_w <= 0 || m->patch_t <= 0 || m->image_h % m->patch_h != 0 ||
-      m->image_w % m->patch_w != 0)
-    return -1;
-  const int hh = m->image_h / m->patch_h, ww = m->image_w / m->patch_w, hw = hh * ww;
-  const int64_t R = (int64_t)B * Tp * hw, D = m->dim, H = m->heads, I = H * m->dim_head;
-  const int64_t K1 = (int64_t)m->channels * m->patch_h * m->patch_w, K2 = K1 * m->patch_t;
-  const int64_t rows1 = (int64_t)B * hw, rows2 = (int64_t)B * (Tp - 1) * hw;
-  const int64_t inner = stack_inner(&m->temporal) > stack_inner(&m->spatial) ? stack_inner(&m->temporal) : stack_inner(&m->spatial);
-  int64_t f = 2 * R * D;                                         // codes (b t h w), their (b h w t) copy
-  f += H * Tp * Tp + 2 * H * hw * hw + phk_cpb_scratch_floats(&m->spatial_bias, hh, ww, 1);  // biases, d spatial bias
-  const int64_t a1 = attn_bwd_scratch_floats(B * hw, (int)H, Tp, Tp, m->dim_head);
-  const int64_t a2 = attn_bwd_scratch_floats(B * Tp, (int)H, hw, hw, m->dim_head);
-  f += a1 > a2 ? a1 : a2;
-  for (int l = 0; l < m->temporal.depth; ++l) f += layer_save_floats(&m->temporal, m->temporal.layers[l], R, 0);
-  for (int l = 0; l < m->spatial.depth; ++l) f += layer_save_floats(&m->spatial, m->spatial.layers[l], R, 0);
-  f += 2 * R * D;                                                // temporal norm_out (b h w t), spatial input (b t h w)
-  f += (rows1 + (rows2 > 0 ? rows2 : 1)) * D;                   // spatial norm_out: first frame, remaining frames
-  f += R * (3 * D + 4 * I + 3 * inner) + 2 * R;                  // dxa dxb dtmp | dq dkv(2) dob | dh(2) dg | statistics
-  f += (rows1 * K1 > rows2 * K2 ? rows1 * K1 : rows2 * K2);      // d video in a patch layout
-  f += (rows1 + (rows2 > 0 ? rows2 : 1)) * D;                   // d norm_out: first frame, remaining frames
-  f += R * (m->codebook_bits > 0 ? m->codebook_bits : 1);        // +-1 codes
-  f += cpb_bwd_scratch_floats(m->spatial_bias, hh, ww, 1);
-  int64_t bytes = f * 4 + 256 * 64;
-  if (prec == PHK_PREC_BF16) bytes += 2 * (dec_tc_scratch_elems(m, R, K2) * 2 + 256);
-  return bytes;
+  if (!cvivit_shapes_ok(m, B, Tp)) return -1;
+  const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(&m->temporal), stack_inner(&m->spatial)));
+  return cv_shared_bytes(g, m->spatial_bias, prec) + dec_phase_floats(m, g) * 4;
 }
 
 // See include/phk.h.
@@ -2044,134 +2373,195 @@ extern "C" int phk_cvivit_decode_backward(const phk_cvivit_dec_t* m, const phk_c
   for (int l = 0; l < TS->depth; ++l) PHK_REQUIRE(!TS->layers[l].has_cross, PHK_E_ARG, "cvivit_decode_backward: cross-attention layer");
   PHK_REQUIRE(!ids || (m->codebook_bits > 0 && m->vq_out_w && m->vq_out_b && grads->vq_out_w && grads->vq_out_b), PHK_E_ARG,
               "cvivit_decode_backward: ids need LFQ's project_out and its gradient");
-  const int hh = m->image_h / m->patch_h, ww = m->image_w / m->patch_w, hw = hh * ww;
-  const int D = m->dim, H = m->heads, DH = m->dim_head, I = H * DH, C = m->channels;
-  const int64_t R = (int64_t)B * Tp * hw, per = (int64_t)Tp * hw;
-  const int64_t K1 = (int64_t)C * m->patch_h * m->patch_w, K2 = K1 * m->patch_t;
-  const int64_t rows1 = (int64_t)B * hw, rows2 = (int64_t)B * (Tp - 1) * hw;
-  const int F = 1 + (Tp - 1) * m->patch_t;
-  const int64_t inner = stack_inner(TT) > stack_inner(TS) ? stack_inner(TT) : stack_inner(TS);
+  const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(TT), stack_inner(TS)));
+  Arena ar{(char*)workspace, workspace_bytes, 0};
+  CvShared S;
+  PHK_TRY(cv_shared_init(ar, g, m->spatial_bias, prec, s, S));
+  return decode_backward_phase(m, grads, ids, tokens, g, dvideo, dtokens, nullptr, S, ar, true, prec, s);
+}
+
+// See include/phk.h.
+extern "C" int phk_cvivit_recon_loss(const float* video, const float* recon, const uint8_t* frame_mask, int32_t B,
+                                     int32_t C, int32_t F, int32_t H, int32_t W, void* scratch, float* loss_out,
+                                     phk_stream_t s) {
+  PHK_REQUIRE(video && recon && scratch && loss_out, PHK_E_ARG, "cvivit_recon_loss: null pointer");
+  PHK_REQUIRE(B > 0 && C > 0 && F > 0 && H > 0 && W > 0, PHK_E_ARG, "cvivit_recon_loss: bad size");
+  const cudaStream_t st = to_stream(s);
+  const int64_t frame = (int64_t)H * W, total = (int64_t)B * C * F * frame;
+  double* partial = reinterpret_cast<double*>(scratch);
+  PHK_KERNEL_LAUNCH(recon_loss_partial_kernel, dim3(kLossBlocks), dim3(256), (size_t)(0), st, video, recon, frame_mask, C, F, frame, total, partial);
+  PHK_LAUNCH_CHECK();
+  PHK_KERNEL_LAUNCH(recon_loss_final_kernel, dim3(1), dim3(256), (size_t)(0), st, (const double*)partial, frame_mask, B, C, F, frame, loss_out);
+  PHK_LAUNCH_CHECK();
+  return 0;
+}
+
+extern "C" int64_t phk_cvivit_backward_workspace_bytes(const phk_cvivit_t* enc, const phk_cvivit_dec_t* dec, int32_t B,
+                                                       int32_t F, int32_t prec) {
+  if (!enc || !dec || F <= 0 || dec->patch_t <= 0 || (F - 1) % dec->patch_t != 0) return -1;
+  const int Tp = 1 + (F - 1) / dec->patch_t;
+  if (!cvivit_shapes_ok(dec, B, Tp) || !enc->spatial.layers || !enc->temporal.layers || enc->spatial.depth <= 0 ||
+      enc->temporal.depth <= 0 || enc->codebook_bits <= 0)
+    return -1;
+  const int64_t inner = imax(imax(stack_inner(&dec->temporal), stack_inner(&dec->spatial)),
+                             imax(stack_inner(&enc->temporal), stack_inner(&enc->spatial)));
+  const CvGeom g = cv_geom(dec, B, Tp, inner);
+  const int64_t video = (int64_t)B * g.C * F * dec->image_h * dec->image_w;
+  const int64_t own = g.R * enc->codebook_bits + video + 256 * 4 / 4;            // d q, d recon
+  return cv_shared_bytes(g, dec->spatial_bias, prec) + (own + imax(dec_phase_floats(dec, g), enc_phase_floats(enc, g, true))) * 4;
+}
+
+// See include/phk.h.  Order: d recon; the decoder phase (as phk_cvivit_decode_backward, from the forward's ids); LFQ
+// (project_out's dgrad, the straight-through d x = d q, project_in); the encoder phase (recomputed with saved activations
+// in the space the decoder phase used, then differentiated down to the patch rows and d video); the position-bias MLP
+// once, over the bias gradient both spatial stacks accumulated.
+extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* enc_grads, const phk_cvivit_dec_t* dec,
+                                   const phk_cvivit_dec_t* dec_grads, const float* video, const float* recon,
+                                   const int64_t* ids, const uint8_t* frame_mask, int32_t B, int32_t F, const float* dloss,
+                                   const float* drecon, float* dvideo, int32_t straight_through, void* workspace,
+                                   int64_t workspace_bytes, int32_t prec, phk_stream_t s) {
+  PHK_REQUIRE(enc && enc_grads && dec && dec_grads && video && recon && ids && dloss && workspace, PHK_E_ARG,
+              "cvivit_backward: null pointer");
+  PHK_REQUIRE(prec == PHK_PREC_F32 || prec == PHK_PREC_BF16, PHK_E_ARG, "cvivit_backward: unknown precision mode");
+  const int64_t need = phk_cvivit_backward_workspace_bytes(enc, dec, B, F, prec);
+  PHK_REQUIRE(need > 0, PHK_E_ARG, "cvivit_backward: bad model table or shape (LFQ tokenizers only)");
+  PHK_REQUIRE(workspace_bytes >= need, PHK_E_WORKSPACE, "cvivit_backward: workspace too small");
+  PHK_REQUIRE(enc->dim == dec->dim && enc->heads == dec->heads && enc->dim_head == dec->dim_head &&
+              enc->channels == dec->channels && enc->image_h == dec->image_h && enc->image_w == dec->image_w &&
+              enc->patch_h == dec->patch_h && enc->patch_w == dec->patch_w && enc->patch_t == dec->patch_t &&
+              enc->codebook_bits == dec->codebook_bits, PHK_E_ARG, "cvivit_backward: encoder and decoder tables differ in shape");
+  const phk_transformer_t* ES = &enc->spatial;
+  const phk_transformer_t* ET = &enc->temporal;
+  PHK_REQUIRE(enc->vq_w && enc->vq_b && enc_grads->vq_w && enc_grads->vq_b && dec->vq_out_w && dec->vq_out_b &&
+              dec_grads->vq_out_w && dec_grads->vq_out_b, PHK_E_ARG, "cvivit_backward: LFQ's projections and their gradients");
+  PHK_REQUIRE(enc_grads->spatial.layers && enc_grads->temporal.layers && enc_grads->spatial.depth == ES->depth &&
+              enc_grads->temporal.depth == ET->depth && dec_grads->spatial.layers && dec_grads->temporal.layers &&
+              dec_grads->spatial.depth == dec->spatial.depth && dec_grads->temporal.depth == dec->temporal.depth, PHK_E_ARG,
+              "cvivit_backward: weight table / gradient table mismatch");
+  const phk_transformer_t* stacks[4] = {ES, ET, &dec->spatial, &dec->temporal};
+  for (int k = 0; k < 4; ++k) {
+    const phk_transformer_t* T = stacks[k];
+    PHK_REQUIRE(T->dim == dec->dim && T->heads == dec->heads && T->dim_head == dec->dim_head, PHK_E_ARG,
+                "cvivit_backward: transformer widths differ from the model's");
+    PHK_REQUIRE((k % 2 == 1) == (T->causal != 0) && (!T->causal || T->alibi_slopes), PHK_E_ARG,
+                "cvivit_backward: the temporal stacks are causal with ALiBi slopes, the spatial ones are not");
+    for (int l = 0; l < T->depth; ++l) PHK_REQUIRE(!T->layers[l].has_cross, PHK_E_ARG, "cvivit_backward: cross-attention layer");
+  }
+  PHK_REQUIRE(dec->dim % 4 == 0, PHK_E_UNSUPPORTED, "cvivit_backward: dim must be a multiple of 4");
+  const int Tp = 1 + (F - 1) / dec->patch_t;
+  const int64_t inner = imax(imax(stack_inner(&dec->temporal), stack_inner(&dec->spatial)), imax(stack_inner(ET), stack_inner(ES)));
+  const CvGeom g = cv_geom(dec, B, Tp, inner);
+  const int D = g.D, hw = g.hw, bits = enc->codebook_bits, C = g.C, H = dec->image_h, W = dec->image_w;
+  const int64_t R = g.R, rows1 = g.rows1, rows2 = g.rows2, K1 = g.K1, K2 = g.K2;
+  const int64_t nvideo = (int64_t)B * C * F * H * W;
   const cudaStream_t st = to_stream(s);
   Arena ar{(char*)workspace, workspace_bytes, 0};
-  TcScratch tc{nullptr, nullptr, 0};
-  if (prec == PHK_PREC_BF16) {
-    tc.elems = dec_tc_scratch_elems(m, R, K2);
-    tc.a = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
-    tc.b = reinterpret_cast<__nv_bfloat16*>(ar.f((tc.elems + 1) / 2));
-    PHK_REQUIRE(tc.a && tc.b, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small (tensor-core operands)");
-  }
-  float* xc = ar.f(R * D);
-  float* xp = ar.f(R * D);
-  float* bias_t = ar.f((int64_t)H * Tp * Tp);
-  float* bias_s = ar.f((int64_t)H * hw * hw);
-  float* dbias_s = ar.f((int64_t)H * hw * hw);
-  float* cpb_sc = ar.f(phk_cpb_scratch_floats(&m->spatial_bias, hh, ww, 1));
-  const int64_t a1 = attn_bwd_scratch_floats(B * hw, H, Tp, Tp, DH), a2 = attn_bwd_scratch_floats(B * Tp, H, hw, hw, DH);
-  float* asc = ar.f(a1 > a2 ? a1 : a2);
-  PHK_REQUIRE(xc && xp && bias_t && bias_s && dbias_s && cpb_sc && asc, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
+  CvShared S;
+  PHK_TRY(cv_shared_init(ar, g, dec->spatial_bias, prec, s, S));
+  float* dq = ar.f(R * bits);
+  float* drec = ar.f(nvideo);
+  PHK_REQUIRE(dq && drec, PHK_E_WORKSPACE, "cvivit_backward: workspace too small");
 
-  // ---------------------------------------------------------------- inputs, biases
-  const float* x_in = tokens;
-  if (ids) {
-    PHK_TRY(phk_lfq_codes(ids, m->vq_out_w, m->vq_out_b, xc, R, D, m->codebook_bits, s));
-    x_in = xc;
-  }
-  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, x_in, xp, B, Tp, hw, D, 1);
+  // ---------------------------------------------------------------- d recon (and the MSE term of d video)
+  PHK_KERNEL_LAUNCH(recon_grad_kernel, dim3(ew_grid(nvideo)), dim3(256), (size_t)(0), st, video, recon, frame_mask, dloss, drecon, drec, dvideo, B, C, F, (int64_t)H * W);
   PHK_LAUNCH_CHECK();
-  PHK_KERNEL_LAUNCH(alibi_causal_bias_kernel, dim3(ew_grid((int64_t)H * Tp * Tp)), dim3(256), (size_t)(0), st, TT->alibi_slopes, bias_t, H, Tp);
-  PHK_LAUNCH_CHECK();
-  PHK_TRY(phk_cpb_bias(&m->spatial_bias, hh, ww, 1, cpb_sc, bias_s, s));
-  PHK_CUDA(cudaMemsetAsync(dbias_s, 0, (int64_t)H * hw * hw * 4, st));
 
-  // ---------------------------------------------------------------- forward, saving activations
-  const DropSite none{0.f, 0.f, 0u, 0u, 0u};
-  LayerCall ct;  // temporal: B h w sequences of T' rows
-  ct.T = TT; ct.GT = &grads->temporal; ct.b = B * hw; ct.n = Tp;
-  ct.pegB = B; ct.pegT = Tp; ct.pegH = hh; ct.pegW = ww;
-  ct.bias = bias_t; ct.prec = prec; ct.s = s; ct.st = st; ct.tc = tc; ct.asc = asc;
-  LayerCall cs = ct;  // spatial: B T' sequences of h w rows
-  cs.T = TS; cs.GT = &grads->spatial; cs.b = B * Tp; cs.n = hw; cs.bias = bias_s; cs.dbias = dbias_s;
-  std::unique_ptr<LayerSave[]> svT(new (std::nothrow) LayerSave[TT->depth]), svS(new (std::nothrow) LayerSave[TS->depth]);
-  PHK_REQUIRE(svT && svS, PHK_E_ARG, "cvivit_decode_backward: out of host memory");
-  const float* xin = xp;
-  for (int l = 0; l < TT->depth; ++l) {
-    float* xout = nullptr;
-    PHK_TRY(layer_forward(ct, l, xin, svT[l], &xout, ar, none, none, none));
-    xin = xout;
-  }
-  const float* xfT = xin;
-  float* nT = ar.f(R * D);
-  float* P = ar.f(R * D);
-  PHK_REQUIRE(nT && P, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
-  PHK_TRY(phk_layernorm(xfT, TT->out_g, TT->out_b, nT, nullptr, R, D, 0, 0, 0, 0, s));
-  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, nT, P, B, Tp, hw, D, 0);
-  PHK_LAUNCH_CHECK();
-  xin = P;
-  for (int l = 0; l < TS->depth; ++l) {
-    float* xout = nullptr;
-    PHK_TRY(layer_forward(cs, l, xin, svS[l], &xout, ar, none, none, none));
-    xin = xout;
-  }
-  const float* xfS = xin;
-  float* Ef = ar.f(rows1 * D);
-  float* Er = ar.f((rows2 > 0 ? rows2 : 1) * D);
-  PHK_REQUIRE(Ef && Er, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
-  PHK_TRY(phk_layernorm(xfS, TS->out_g, TS->out_b, Ef, nullptr, rows1, D, 0, -hw, per, 0, s));
-  if (Tp > 1) PHK_TRY(phk_layernorm(xfS, TS->out_g, TS->out_b, Er, nullptr, rows2, D, 0, -(per - hw), per, hw, s));
+  // ---------------------------------------------------------------- decoder phase, from the forward's ids
+  const float* dcodes = nullptr;
+  PHK_TRY(decode_backward_phase(dec, dec_grads, ids, nullptr, g, drec, nullptr, &dcodes, S, ar, false, prec, s));
 
-  // ---------------------------------------------------------------- to_pixels_first_frame / to_pixels
-  LayerGrads G;
-  float* dx = ar.f(R * D);
-  float* dx_alt = ar.f(R * D);
-  G.dtmp = ar.f(R * D); G.dq = ar.f(R * I); G.dkv = ar.f(R * 2 * I); G.dob = ar.f(R * I);
-  G.dh = ar.f(R * 2 * inner); G.dg = ar.f(R * inner); G.dckv = nullptr; G.dctxn = nullptr;
-  G.stats = reinterpret_cast<float2*>(ar.f(2 * R));
-  float* dG = ar.f(rows1 * K1 > rows2 * K2 ? rows1 * K1 : rows2 * K2);
-  float* dEf = ar.f(rows1 * D);
-  float* dEr = ar.f((rows2 > 0 ? rows2 : 1) * D);
-  PHK_REQUIRE(dx && dx_alt && G.dtmp && G.dq && G.dkv && G.dob && G.dh && G.dg && G.stats && dG && dEf && dEr, PHK_E_WORKSPACE,
-              "cvivit_decode_backward: workspace too small (gradients)");
-  PHK_KERNEL_LAUNCH(patch_gather_kernel, dim3(ew_grid(rows1 * K1)), dim3(256), (size_t)(0), st, dvideo, dG, B, C, F, m->image_h, m->image_w, 0, 1, 1, m->patch_h, m->patch_w);
-  PHK_LAUNCH_CHECK();
-  PHK_TRY(wgrad_p(prec, tc, dG, Ef, (float*)grads->px_first_w, rows1, K1, D, s));
-  PHK_TRY(colsum(dG, rows1, (int)K1, K1, (float*)grads->px_first_b, st));
-  PHK_TRY(dgrad_p(prec, tc, dG, m->px_first_w, dEf, rows1, K1, D, 0, s));
-  if (Tp > 1) {  // (one latent frame: to_pixels sees an empty batch, its gradients stay the caller's zeros)
-    PHK_KERNEL_LAUNCH(patch_gather_kernel, dim3(ew_grid(rows2 * K2)), dim3(256), (size_t)(0), st, dvideo, dG, B, C, F, m->image_h, m->image_w, 1, Tp - 1, m->patch_t, m->patch_h, m->patch_w);
+  // ---------------------------------------------------------------- LFQ: d q = d z_dec W_out; straight through, d x = d q
+  if (straight_through) {
+    PHK_TRY(dgrad(dcodes, dec->vq_out_w, dq, R, D, bits, 0, st));  // [R, bits]: the LFQ products stay fp32 (bits wide)
+
+    // ---------------------------------------------------------------- encoder phase: recompute
+    Arena ea = ar;  // the decoder phase's space
+    const int64_t r2 = rows2 > 0 ? rows2 : 1;
+    float* X1 = ea.f(rows1 * K1); float* A1 = ea.f(rows1 * K1);
+    float* X2 = ea.f(r2 * K2); float* A2 = ea.f(r2 * K2);
+    float* Pe1 = ea.f(rows1 * D); float* Pe2 = ea.f(r2 * D);
+    float* x0 = ea.f(R * D);
+    PHK_REQUIRE(X1 && A1 && X2 && A2 && Pe1 && Pe2 && x0, PHK_E_WORKSPACE, "cvivit_backward: workspace too small (patches)");
+    PHK_KERNEL_LAUNCH(patch_gather_kernel, dim3(ew_grid(rows1 * K1)), dim3(256), (size_t)(0), st, video, X1, B, C, F, H, W, 0, 1, 1, enc->patch_h, enc->patch_w);
     PHK_LAUNCH_CHECK();
-    PHK_TRY(wgrad_p(prec, tc, dG, Er, (float*)grads->px_w, rows2, K2, D, s));
-    PHK_TRY(colsum(dG, rows2, (int)K2, K2, (float*)grads->px_b, st));
-    PHK_TRY(dgrad_p(prec, tc, dG, m->px_w, dEr, rows2, K2, D, 0, s));
-  }
-  PHK_KERNEL_LAUNCH(frames_merge_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dEf, dEr, G.dtmp, B, Tp, hw, D);
-  PHK_LAUNCH_CHECK();
-
-  // ---------------------------------------------------------------- spatial stack, position-bias MLP
-  PHK_TRY(ln_backward(xfS, TS->out_g, G.dtmp, dx, 0, (float*)grads->spatial.out_g, nullptr, G.stats, R, D, st));
-  for (int l = TS->depth - 1; l >= 0; --l) PHK_TRY(layer_backward(cs, l, svS[l], &dx, &dx_alt, G, nullptr, none, none, none));
-  float* csc = ar.f(cpb_bwd_scratch_floats(m->spatial_bias, hh, ww, 1));
-  PHK_REQUIRE(csc, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small (position-bias backward)");
-  PHK_TRY(cpb_backward(m->spatial_bias, grads->spatial_bias, dbias_s, hh, ww, 1, csc, st));
-
-  // ---------------------------------------------------------------- temporal stack, rows (b h w t)
-  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 1);
-  PHK_LAUNCH_CHECK();
-  PHK_TRY(ln_backward(xfT, TT->out_g, G.dtmp, dx, 0, (float*)grads->temporal.out_g, nullptr, G.stats, R, D, st));
-  for (int l = TT->depth - 1; l >= 0; --l) PHK_TRY(layer_backward(ct, l, svT[l], &dx, &dx_alt, G, nullptr, none, none, none));
-
-  // ---------------------------------------------------------------- d tokens / project_out
-  if (!ids && !dtokens) return 0;
-  float* dcodes = dtokens ? dtokens : dx_alt;
-  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, dcodes, B, Tp, hw, D, 0);
-  PHK_LAUNCH_CHECK();
-  if (ids) {
-    const int bits = m->codebook_bits;
-    float* signs = ar.f(R * bits);
-    PHK_REQUIRE(signs, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small (codes)");
-    PHK_KERNEL_LAUNCH(lfq_signs_kernel, dim3(ew_grid(R * bits)), dim3(256), (size_t)(0), st, ids, signs, R, bits);
+    PHK_TRY(phk_patchify_ln(video, B, C, F, H, W, 0, 1, 1, enc->patch_h, enc->patch_w, enc->pf_ln1_g, enc->pf_ln1_b, A1, 0, s));
+    PHK_TRY(linear_fwd(prec, S.tc, A1, enc->pf_w, Pe1, rows1, D, K1, enc->pf_b, nullptr, s));
+    PHK_TRY(phk_layernorm(Pe1, enc->pf_ln2_g, enc->pf_ln2_b, x0, nullptr, rows1, D, 0, hw, (int64_t)Tp * hw, 0, s));
+    if (rows2 > 0) {
+      PHK_KERNEL_LAUNCH(patch_gather_kernel, dim3(ew_grid(rows2 * K2)), dim3(256), (size_t)(0), st, video, X2, B, C, F, H, W, 1, Tp - 1, enc->patch_t, enc->patch_h, enc->patch_w);
+      PHK_LAUNCH_CHECK();
+      PHK_TRY(phk_patchify_ln(video, B, C, F, H, W, 1, Tp - 1, enc->patch_t, enc->patch_h, enc->patch_w, enc->pr_ln1_g,
+                              enc->pr_ln1_b, A2, 0, s));
+      PHK_TRY(linear_fwd(prec, S.tc, A2, enc->pr_w, Pe2, rows2, D, K2, enc->pr_b, nullptr, s));
+      PHK_TRY(phk_layernorm(Pe2, enc->pr_ln2_g, enc->pr_ln2_b, x0, nullptr, rows2, D, 0, (int64_t)(Tp - 1) * hw,
+                            (int64_t)Tp * hw, hw, s));
+    }
+    const LayerCall cs = spatial_call(ES, &enc_grads->spatial, g, S, prec, s);
+    LayerCall ct;
+    PHK_TRY(temporal_call(ET, &enc_grads->temporal, g, S, prec, s, &ct));
+    std::unique_ptr<LayerSave[]> svS(new (std::nothrow) LayerSave[ES->depth]), svT(new (std::nothrow) LayerSave[ET->depth]);
+    PHK_REQUIRE(svT && svS, PHK_E_ARG, "cvivit_backward: out of host memory");
+    const float* xfS = nullptr;
+    PHK_TRY(stack_forward(cs, x0, svS.get(), &xfS, ea));
+    float* nS = ea.f(R * D); float* Pt = ea.f(R * D);
+    PHK_REQUIRE(nS && Pt, PHK_E_WORKSPACE, "cvivit_backward: workspace too small");
+    PHK_TRY(phk_layernorm(xfS, ES->out_g, ES->out_b, nS, nullptr, R, D, 0, 0, 0, 0, s));
+    PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, nS, Pt, B, Tp, hw, D, 1);
     PHK_LAUNCH_CHECK();
-    PHK_TRY(wgrad(dcodes, signs, (float*)grads->vq_out_w, R, D, bits, st));  // [dim, bits]: not worth a tensor-core launch
-    PHK_TRY(colsum(dcodes, R, D, D, (float*)grads->vq_out_b, st));
+    const float* xfT = nullptr;
+    PHK_TRY(stack_forward(ct, Pt, svT.get(), &xfT, ea));
+    float* nT = ea.f(R * D); float* z = ea.f(R * D);
+    PHK_REQUIRE(nT && z, PHK_E_WORKSPACE, "cvivit_backward: workspace too small");
+    PHK_TRY(phk_layernorm(xfT, ET->out_g, ET->out_b, nT, nullptr, R, D, 0, 0, 0, 0, s));
+    PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, nT, z, B, Tp, hw, D, 0);
+    PHK_LAUNCH_CHECK();
+
+    // ---------------------------------------------------------------- project_in, then the two stacks
+    const LayerGrads& G = S.G;
+    float* dx = S.dx;
+    float* dx_alt = S.dx_alt;
+    PHK_TRY(wgrad(dq, z, (float*)enc_grads->vq_w, R, bits, D, st));
+    PHK_TRY(colsum(dq, R, bits, bits, (float*)enc_grads->vq_b, st));
+    PHK_TRY(dgrad(dq, enc->vq_w, dx, R, bits, D, 0, st));  // d(encoder output), (b t h w)
+    PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 1);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(stack_backward(ct, svT.get(), xfT, G.dtmp, &dx, &dx_alt, G));
+    PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 0);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(stack_backward(cs, svS.get(), xfS, G.dtmp, &dx, &dx_alt, G));
+
+    // ---------------------------------------------------------------- to_patch_emb_first_frame / to_patch_emb
+    float* dE1 = ea.f(rows1 * D); float* dE2 = ea.f(r2 * D);
+    float* dP = ea.f(imax(rows1, r2) * D);
+    float* dA = ea.f(imax(rows1 * K1, rows2 * K2));
+    float* dX = dvideo ? ea.f(imax(rows1 * K1, rows2 * K2)) : nullptr;
+    PHK_REQUIRE(dE1 && dE2 && dP && dA && (dX || !dvideo), PHK_E_WORKSPACE, "cvivit_backward: workspace too small (patch gradients)");
+    PHK_KERNEL_LAUNCH(frames_split_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, dE1, dE2, B, Tp, hw, D);
+    PHK_LAUNCH_CHECK();
+    struct Emb { const float *X, *A, *Pe, *dE, *ln1_g, *w, *ln2_g; const phk_cvivit_t* gr; int64_t rows, K; int f0, nt, pt; bool first; };
+    const Emb embs[2] = {{X1, A1, Pe1, dE1, enc->pf_ln1_g, enc->pf_w, enc->pf_ln2_g, enc_grads, rows1, K1, 0, 1, 1, true},
+                         {X2, A2, Pe2, dE2, enc->pr_ln1_g, enc->pr_w, enc->pr_ln2_g, enc_grads, rows2, K2, 1, Tp - 1, enc->patch_t, false}};
+    for (const Emb& e : embs) {
+      if (e.rows == 0) continue;  // (one latent frame: to_patch_emb sees an empty batch, its gradients stay zero)
+      float* g_ln1_g = (float*)(e.first ? e.gr->pf_ln1_g : e.gr->pr_ln1_g);
+      float* g_ln1_b = (float*)(e.first ? e.gr->pf_ln1_b : e.gr->pr_ln1_b);
+      float* g_w = (float*)(e.first ? e.gr->pf_w : e.gr->pr_w);
+      float* g_b = (float*)(e.first ? e.gr->pf_b : e.gr->pr_b);
+      float* g_ln2_g = (float*)(e.first ? e.gr->pf_ln2_g : e.gr->pr_ln2_g);
+      float* g_ln2_b = (float*)(e.first ? e.gr->pf_ln2_b : e.gr->pr_ln2_b);
+      // nn.LayerNorm with a bias parameter: dbeta is a gradient here
+      PHK_TRY(ln_backward(e.Pe, e.ln2_g, e.dE, dP, 0, g_ln2_g, g_ln2_b, G.stats, e.rows, D, st));
+      PHK_TRY(wgrad_p(prec, S.tc, dP, e.A, g_w, e.rows, D, e.K, s));
+      PHK_TRY(colsum(dP, e.rows, D, D, g_b, st));
+      PHK_TRY(dgrad_p(prec, S.tc, dP, e.w, dA, e.rows, D, e.K, 0, s));
+      PHK_TRY(ln_backward(e.X, e.ln1_g, dA, dX, 0, g_ln1_g, g_ln1_b, G.stats, e.rows, (int)e.K, st));
+      if (dvideo) {
+        PHK_KERNEL_LAUNCH(patch_scatter_add_kernel, dim3(ew_grid(e.rows * e.K)), dim3(256), (size_t)(0), st, (const float*)dX, dvideo, B, C, F, H, W, e.f0, e.nt, e.pt, enc->patch_h, enc->patch_w);
+        PHK_LAUNCH_CHECK();
+      }
+    }
   }
-  return 0;
+
+  // ---------------------------------------------------------------- position-bias MLP, once over both spatial stacks
+  return cpb_backward(dec->spatial_bias, dec_grads->spatial_bias, S.dbias_s, g.hh, g.ww, 1, S.cpb_bwd_sc, st);
 }

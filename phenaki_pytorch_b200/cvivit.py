@@ -3,8 +3,10 @@
 Same constructor keywords, attribute names and state-dict layout as the reference
 (/root/reference/phenaki_pytorch/cvivit.py:226-335); ``forward(video,
 return_only_codebook_ids=True)`` (cvivit.py:518-574) runs entirely in libphk.so
-(phk_cvivit_encode).  Training losses, discriminator and VGG (cvivit.py:59-213, 576-671) are out
-of scope (SURVEY.md section 2, rows 8/10) and raise.
+(phk_cvivit_encode).  With ``use_vgg_and_gan=False`` and LFQ, ``loss = forward(video)`` is the reference's
+reconstruction loss and ``loss.backward()`` fills the gradients through the decoder, LFQ's straight-through estimator
+and the encoder (phk_cvivit_backward).  The GAN / perceptual losses, discriminator and VGG (cvivit.py:59-213, 600-671)
+are out of scope (SURVEY.md section 2, rows 8/10) and raise.
 """
 import copy
 import ctypes as C
@@ -367,8 +369,118 @@ class CViViT(nn.Module):
             with torch.no_grad():
                 recon = self.decode_from_codebook_indices(self.encode_ids(video))
             return recon.squeeze(2) if is_image else recon
-        raise NotImplementedError("C-ViViT training losses (reconstruction / GAN / perceptual, cvivit.py:576-671) "
-                                  "are out of scope of the H100 hot path (SURVEY.md section 2 row 8)")
+        if self.use_vgg_and_gan or return_discr_loss:
+            raise NotImplementedError("C-ViViT GAN / perceptual training losses (cvivit.py:600-671) are out of scope of "
+                                      "the H100 hot path (SURVEY.md section 2 row 8): build with use_vgg_and_gan=False "
+                                      "for the reconstruction loss")
+        loss, recon = self._recon_loss(video, mask)
+        # the reference draws the discriminator's frame pick before it returns (cvivit.py:594): the same CPU draw keeps a
+        # seeded training script's later random numbers in step with it
+        torch.randn(video.shape[0], video.shape[2])
+        if return_recons:
+            return loss, (recon.squeeze(2) if is_image else recon)
+        return loss
+
+    # ---- reconstruction loss and its backward (cvivit.py:518-598 with use_vgg_and_gan=False) ------------------------
+    def _encoder_params(self):
+        """The parameters only the encode reaches: to_patch_emb*, both encoder stacks and LFQ's project_in."""
+        mods = [self.to_patch_emb_first_frame, self.to_patch_emb, self.enc_spatial_transformer,
+                self.enc_temporal_transformer, self.vq.project_in]
+        return [p for m in mods for p in m.parameters()]
+
+    def _recon_loss(self, video, mask):
+        """(loss, recon): the masked MSE of decode(encode(video)) against video, differentiable through
+        ``_ReconLossFn`` when grad mode is on and ``video`` or a parameter requires grad."""
+        video = L.require_cuda(video, "video", torch.float32)
+        b, c, f, *image_dims = video.shape
+        assert tuple(image_dims) == self.image_size and c == self.channels
+        assert (f - 1) % self.temporal_patch_size == 0, \
+            f"number of frames ({f}) minus one ({f - 1}) must be divisible by temporal patch size ({self.temporal_patch_size})"
+        if not self.lookup_free_quantization:
+            raise NotImplementedError("the reconstruction loss needs lookup_free_quantization=True: training the "
+                                      "cosine-sim VectorQuantize (EMA codebook updates, its own straight-through) is not "
+                                      "implemented")
+        if self.training and any(t.attn_dropout > 0 or t.ff_dropout > 0 for t in (
+                self.enc_spatial_transformer, self.enc_temporal_transformer, self.dec_spatial_transformer,
+                self.dec_temporal_transformer)):
+            raise NotImplementedError("C-ViViT dropout is not implemented: the encode and decode apply none "
+                                      "(DESIGN.md section 8); build with attn_dropout=ff_dropout=0 or call eval()")
+        if mask is not None:
+            mask = mask.to(video.device)
+            self.calculate_video_token_mask(video, mask)  # for its assertion only, as the reference (LFQ takes no mask)
+            mask = mask.to(torch.uint8).contiguous()
+        params = self._encoder_params() + self._decoder_params(True)
+        spec = dict(net=self, mask=mask, params=params, n_enc=len(self._encoder_params()), precision=self.precision,
+                    straight_through=self.vq.training, sig=weights_signature(self))
+        if torch.is_grad_enabled() and (video.requires_grad or any(p.requires_grad for p in params)):
+            return _ReconLossFn.apply(spec, video, *params)
+        return self._recon_forward(video.detach(), mask)[1:]
+
+    def _recon_forward(self, video, mask):
+        """(ids, loss, recon) of the inference path: phk_cvivit_encode, phk_cvivit_decode from the ids, the loss."""
+        b, c, f, h, w = video.shape
+        ids = self.encode_ids(video)
+        recon = self._decode(ids.reshape(b, -1), None, b, ids.shape[1], video.device)
+        lib = L.lib()
+        with torch.cuda.device(video.device):
+            loss = torch.empty((), dtype=torch.float32, device=video.device)
+            scratch = torch.empty(L.RECON_LOSS_SCRATCH_BYTES, dtype=torch.uint8, device=video.device)
+            L.check(lib.phk_cvivit_recon_loss(L.ptr(video), L.ptr(recon), L.ptr(mask), b, c, f, h, w, L.ptr(scratch),
+                                              L.ptr(loss), L.stream_ptr()), "phk_cvivit_recon_loss")
+        return ids, loss, recon
+
+    def _enc_grad_table(self, gk):
+        """The phk_cvivit_t-shaped table addressing the encoder side's gradient buffers in ``gk``."""
+        t = L.CvivitT()
+        t.dim, t.heads, t.dim_head, t.channels = self.dim, self.heads, self.dim_head, self.channels
+        t.image_h, t.image_w = self.image_size
+        t.patch_h, t.patch_w = self.patch_size
+        t.patch_t = self.temporal_patch_size
+        t.codebook_bits = self.vq.codebook_dim
+        f, r = self.to_patch_emb_first_frame, self.to_patch_emb
+        t.pf_ln1_g, t.pf_ln1_b, t.pf_w, t.pf_b = gk.g(f[1].weight), gk.g(f[1].bias), gk.g(f[2].weight), gk.g(f[2].bias)
+        t.pf_ln2_g, t.pf_ln2_b = gk.g(f[3].weight), gk.g(f[3].bias)
+        t.pr_ln1_g, t.pr_ln1_b, t.pr_w, t.pr_b = gk.g(r[1].weight), gk.g(r[1].bias), gk.g(r[2].weight), gk.g(r[2].bias)
+        t.pr_ln2_g, t.pr_ln2_b = gk.g(r[3].weight), gk.g(r[3].bias)
+        t.spatial = transformer_grad_table(self.enc_spatial_transformer, gk, False)
+        t.temporal = transformer_grad_table(self.enc_temporal_transformer, gk, False)
+        t.vq_w, t.vq_b = gk.g(self.vq.project_in.weight), gk.g(self.vq.project_in.bias)
+        return t
+
+    def _recon_backward(self, spec, video, ids, recon, dloss, drecon, want_video_grad):
+        """phk_cvivit_backward for one ``_ReconLossFn`` call: ([gradient or None per parameter of spec["params"]],
+        d video or None)."""
+        if weights_signature(self) != spec["sig"]:
+            raise RuntimeError("a parameter of this module was modified or replaced between the forward and the backward: "
+                               "the backward recomputes the forward from the current weights, so it would differentiate "
+                               "another function")
+        lib = L.lib()
+        dev = video.device
+        b, _, f = video.shape[:3]
+        prec = L.PREC_BF16 if spec["precision"] == L.PREC_BF16 else L.PREC_F32  # split-bf16 is an inference mode
+        straight = spec["straight_through"]
+        with torch.cuda.device(dev):
+            enc, dec = self._table(), self._dec_table()
+            gk = GradKeep(spec["params"])
+            egt = self._enc_grad_table(gk)
+            dgt = self._dec_grad_table(gk, True)
+            dloss = (torch.zeros((), dtype=torch.float32, device=dev) if dloss is None
+                     else dloss.to(dev, torch.float32).contiguous())
+            drecon = None if drecon is None else drecon.to(dev, torch.float32).reshape(recon.shape).contiguous()
+            dvideo = torch.empty_like(video) if want_video_grad else None
+            nbytes = lib.phk_cvivit_backward_workspace_bytes(C.byref(enc), C.byref(dec), b, f, prec)
+            if nbytes < 0:
+                raise L.PhkError("phk_cvivit_backward_workspace_bytes: unsupported configuration")
+            ws = self._ws.get(nbytes, dev)
+            L.check(lib.phk_cvivit_backward(C.byref(enc), C.byref(egt), C.byref(dec), C.byref(dgt), L.ptr(video),
+                                            L.ptr(recon), L.ptr(ids), L.ptr(spec["mask"]), b, f, L.ptr(dloss),
+                                            L.ptr(drecon), L.ptr(dvideo), int(straight), L.ptr(ws), ws.numel(), prec,
+                                            L.stream_ptr()),
+                    "phk_cvivit_backward")
+        grads = [gk.grad_of(p) for p in spec["params"]]
+        if not straight:  # eval mode: q is a constant, nothing reaches the encoder
+            grads[:spec["n_enc"]] = [None] * spec["n_enc"]
+        return grads, dvideo
 
     def _decode(self, ids, tokens, b, tp, device, taps=None):
         lib = L.lib()
@@ -400,9 +512,8 @@ class CViViT(nn.Module):
             mods.append(self.vq.project_out)
         return [p for m in mods for p in m.parameters()]
 
-    def _dec_grad_table(self, params, with_project_out):
-        """Zero-filled gradient buffers of ``params`` and the phk_cvivit_dec_t-shaped table that addresses them."""
-        gk = GradKeep(params)
+    def _dec_grad_table(self, gk, with_project_out):
+        """The phk_cvivit_dec_t-shaped table addressing the decoder side's gradient buffers in ``gk``."""
         t = L.CvivitDecT()
         t.dim, t.heads, t.dim_head, t.channels = self.dim, self.heads, self.dim_head, self.channels
         t.image_h, t.image_w = self.image_size
@@ -417,7 +528,7 @@ class CViViT(nn.Module):
         f, r = self.to_pixels_first_frame[0], self.to_pixels[0]
         t.px_first_w, t.px_first_b = gk.g(f.weight), gk.g(f.bias)
         t.px_w, t.px_b = gk.g(r.weight), gk.g(r.bias)  # (one latent frame: zeros, as autograd gives an empty batch)
-        return t, gk
+        return t
 
     def _differentiable_decode(self, ids, tokens, b, tp, device, taps=None):
         """``_decode`` exactly as it runs under ``torch.no_grad`` and, when autograd wants a gradient of it (grad mode on,
@@ -447,7 +558,8 @@ class CViViT(nn.Module):
         prec = L.PREC_BF16 if spec["precision"] == L.PREC_BF16 else L.PREC_F32  # split-bf16 is an inference mode
         with torch.cuda.device(dev):
             table = self._dec_table()
-            gtable, gk = self._dec_grad_table(spec["params"], ids is not None)
+            gk = GradKeep(spec["params"])
+            gtable = self._dec_grad_table(gk, ids is not None)
             dtokens = torch.empty_like(tokens) if tokens is not None and want_tokens_grad else None
             nbytes = lib.phk_cvivit_decode_backward_workspace_bytes(C.byref(table), b, tp, prec)
             ws = self._ws.get(nbytes, dev)
@@ -506,3 +618,29 @@ class _DecodeFn(torch.autograd.Function):
         spec = ctx.spec
         grads, dtokens = spec["net"]._decode_backward(spec, dvideo, ids, tokens, ctx.needs_input_grad[3])
         return (None, None, None, dtokens, *grads)
+
+
+class _ReconLossFn(torch.autograd.Function):
+    """Makes the C-ViViT reconstruction loss differentiable.  The forward runs the inference path unchanged (encode to
+    ids, decode from them, the loss kernel) and keeps the video, the ids, the reconstruction and the mask; the backward
+    recomputes the decoder and, in training mode, the encoder with saved activations inside phk_cvivit_backward.  It
+    decodes from the forward's ids, so it differentiates the function whose loss was returned even where a recomputed
+    projection would flip a sign; LFQ's straight-through estimator makes d x independent of the signs."""
+
+    @staticmethod
+    def forward(ctx, spec, video, *params):
+        ctx.set_materialize_grads(False)
+        ids, loss, recon = spec["net"]._recon_forward(video.detach(), spec["mask"])
+        ctx.spec = spec
+        ctx.save_for_backward(video.detach(), ids, recon)
+        return loss, recon
+
+    @staticmethod
+    def backward(ctx, dloss, drecon):
+        if torch.is_grad_enabled():
+            raise RuntimeError("the C-ViViT reconstruction loss does not support create_graph=True: its backward is "
+                               "hand-written CUDA and builds no graph of its own")
+        video, ids, recon = ctx.saved_tensors
+        spec = ctx.spec
+        grads, dvideo = spec["net"]._recon_backward(spec, video, ids, recon, dloss, drecon, ctx.needs_input_grad[1])
+        return (None, dvideo, *grads)
