@@ -437,6 +437,33 @@ int phk_cvivit_decode_backward(const phk_cvivit_dec_t* m, const phk_cvivit_dec_t
                                const float* tokens, int32_t B, int32_t Tp, const float* dvideo, float* dtokens,
                                void* workspace, int64_t workspace_bytes, int32_t prec, phk_stream_t s);
 
+/* CViViT.encode(tokens) (cvivit.py:449-474): the encoder's spatial stack over (b t) sequences with the 2-D position bias,
+ * then its causal ALiBi temporal stack over (b h w) sequences (PEG with the reference's raw-reshape layout), norm_out
+ * included.  No patch embedding, no quantiser: any table with both encoder stacks (LFQ or cosine-sim) serves.
+ *   tokens / out  fp32 [B*Tp*H'*W', dim] device, rows in (b,t,h,w) order; out receives the temporal stack's norm_out
+ *   spatial_bias  as for phk_cvivit_encode (NULL: recomputed inside)
+ * Eager launches (no CUDA-graph replay); prec: any precision mode, the forward of that mode's inference kernels. */
+int64_t phk_cvivit_encode_tokens_workspace_bytes(const phk_cvivit_t* m, int32_t B, int32_t Tp, int32_t prec);
+int phk_cvivit_encode_tokens(const phk_cvivit_t* m, const float* tokens, int32_t B, int32_t Tp, float* out,
+                             void* workspace, int64_t workspace_bytes, int32_t prec, const float* spatial_bias,
+                             phk_stream_t s);
+
+/* Backward of phk_cvivit_encode_tokens from a gradient the caller supplies: what `out = CViViT.encode(tokens);
+ * out.backward(dout)` computes under torch autograd (cvivit.py:449-474).  Both stacks are recomputed from the tokens with
+ * saved activations (activation checkpointing), then differentiated through the temporal stack (its norm_out included),
+ * the spatial stack and the spatial_rel_pos_bias MLP through its 2-D bias.
+ *   tokens / B / Tp  the arguments of the phk_cvivit_encode_tokens call being differentiated
+ *   grads    a table of the SAME layout as `m` whose float pointers address ZERO-FILLED gradient buffers: the spatial and
+ *            temporal transformers and spatial_bias; every gradient is ACCUMULATED.  The patch embeddings and the
+ *            quantiser are not read (their pointers may be NULL).
+ *   dout     fp32 [B*Tp*H'*W', dim], d loss / d out, (b,t,h,w) rows
+ *   dtokens  NULL, or fp32 like tokens: receives d loss / d tokens (written, not added)
+ * prec: PHK_PREC_F32 (fp32 products) or PHK_PREC_BF16 (the training step's bf16 products); no dropout is applied. */
+int64_t phk_cvivit_encode_backward_workspace_bytes(const phk_cvivit_t* m, int32_t B, int32_t Tp, int32_t prec);
+int phk_cvivit_encode_backward(const phk_cvivit_t* m, const phk_cvivit_t* grads, const float* tokens, int32_t B,
+                               int32_t Tp, const float* dout, float* dtokens, void* workspace,
+                               int64_t workspace_bytes, int32_t prec, phk_stream_t s);
+
 /* The reconstruction loss of CViViT.forward with use_vgg_and_gan=False (cvivit.py:584-590): F.mse_loss(video, recon), or
  * with a frame mask the mean of the squared error over the selected frames (sum / (selected frames * C * H * W); an
  * all-false mask gives NaN, as the reference does).  video / recon fp32 (B, C, F, H, W); frame_mask NULL or uint8 (B, F);

@@ -325,7 +325,7 @@ static int check_transformer(const phk_transformer_t* T) {
 
 using namespace phk;
 
-extern "C" int phk_version(void) { return 106; }
+extern "C" int phk_version(void) { return 107; }
 extern "C" const char* phk_last_error(void) { return g_err; }
 extern "C" int64_t phk_launch_count(void) { return g_launches.load(); }
 
@@ -382,6 +382,37 @@ extern "C" int64_t phk_cvivit_workspace_bytes(const phk_cvivit_t* m, int32_t B, 
     bytes += x3_bytes(R, k);
   }
   return bytes;
+}
+
+// The encoder's two stacks (cvivit.py:449-474) on the patch tokens in x, rows in (b,t,h,w) order (x is overwritten): the
+// spatial transformer over (b t) sequences with the 2-D position bias (computed into bias_buf when spatial_bias is NULL),
+// its norm_out into P, then the temporal transformer over (b h w) sequences in place, its stream alternating between P
+// and x.  out (NULL: not formed): the temporal norm_out, (b,t,h,w) rows; *xf: the temporal stream before norm_out.
+static int cvivit_encode_stacks(const phk_cvivit_t* m, int B, int Tp, int hh, int ww, float* x, float* x_alt, float* P,
+                                const float* spatial_bias, float* bias_buf, float* cpb_scratch, int prec, const Lin& lin,
+                                Arena tf, float* tap_spatial, float* out, float** xf, phk_stream_t s) {
+  const cudaStream_t st = to_stream(s);
+  const int hw = hh * ww;
+  const int64_t R = (int64_t)B * Tp * hw;
+  if (!spatial_bias) {
+    PHK_TRY(phk_cpb_bias(&m->spatial_bias, hh, ww, 1, cpb_scratch, bias_buf, s));
+    spatial_bias = bias_buf;
+  }
+  TfCall c;
+  std::memset(&c, 0, sizeof(c));
+  c.T = &m->spatial; c.x = x; c.x_alt = x_alt; c.R = R;
+  c.seq = SeqView{B * Tp, 1, hw, hw, 0, 1};
+  c.pegB = B; c.pegT = Tp; c.pegH = hh; c.pegW = ww; c.peg_layout = 0;
+  c.attn_bias = spatial_bias; c.ctx_mask_off_from = -1; c.prec = prec; c.lin = lin;
+  PHK_TRY(transformer_forward(c, tf, P, nullptr, st));  // P <- norm_out(spatial)
+  if (tap_spatial) PHK_CUDA(cudaMemcpyAsync(tap_spatial, P, R * m->dim * 4, cudaMemcpyDeviceToDevice, st));
+
+  c.T = &m->temporal; c.x = P; c.x_alt = x;
+  c.seq = SeqView{B, hw, Tp, (int64_t)Tp * hw, 1, hw};
+  c.peg_layout = 1;  // the reference's raw-reshape quirk (attention.py:71, cvivit.py:468-470)
+  c.attn_bias = nullptr;
+  c.x_final = xf;
+  return transformer_forward(c, tf, out, nullptr, st);
 }
 
 static int cvivit_encode_impl(const phk_cvivit_t* m, const float* video, int32_t B, int32_t F, int64_t* ids,
@@ -448,29 +479,12 @@ static int cvivit_encode_impl(const phk_cvivit_t* m, const float* video, int32_t
   if (tap_patch) PHK_CUDA(cudaMemcpyAsync(tap_patch, x, R * D * 4, cudaMemcpyDeviceToDevice, st));
 
   // ---- encode (cvivit.py:449-474): spatial over (b t), temporal over (b h w); no rearrange copies
-  if (!spatial_bias) {
-    PHK_TRY(phk_cpb_bias(&m->spatial_bias, hh, ww, 1, cpb_scratch, bias_buf, s));
-    spatial_bias = bias_buf;
-  }
-  Arena tf = ar;
-  TfCall c;
-  std::memset(&c, 0, sizeof(c));
-  c.T = &m->spatial; c.x = x; c.x_alt = x_alt; c.R = R;
-  c.seq = SeqView{B * Tp, 1, hw, hw, 0, 1};
-  c.pegB = B; c.pegT = Tp; c.pegH = hh; c.pegW = ww; c.peg_layout = 0;
-  c.attn_bias = spatial_bias; c.ctx_mask_off_from = -1; c.prec = prec; c.lin = lin;
-  PHK_TRY(transformer_forward(c, tf, P, nullptr, st));  // P <- norm_out(spatial)
-  if (tap_spatial) PHK_CUDA(cudaMemcpyAsync(tap_spatial, P, R * D * 4, cudaMemcpyDeviceToDevice, st));
-
-  c.T = &m->temporal; c.x = P; c.x_alt = x;
-  c.seq = SeqView{B, hw, Tp, (int64_t)Tp * hw, 1, hw};
-  c.peg_layout = 1;  // the reference's raw-reshape quirk (attention.py:71, cvivit.py:468-470)
-  c.attn_bias = nullptr;
   // norm_out of the temporal transformer is fused with the LFQ projection + sign quantisation (cvivit.py:562-574):
   // the normalised tokens are only written when a parity test taps them; ids come out in (b, t, h, w) order
+  Arena tf = ar;
   float* xf = nullptr;
-  c.x_final = &xf;
-  PHK_TRY(transformer_forward(c, tf, nullptr, nullptr, st));
+  PHK_TRY(cvivit_encode_stacks(m, B, Tp, hh, ww, x, x_alt, P, spatial_bias, bias_buf, cpb_scratch, prec, lin, tf,
+                               tap_spatial, nullptr, &xf, s));
   float* norm_buf = x_alt;  // not used by the temporal transformer (its stream alternates between P and x)
   if (m->codebook) {
     // lookup_free_quantization=False (cvivit.py:321, 568-570): norm_out, then the nearest unit codebook row by cosine
@@ -611,6 +625,73 @@ extern "C" int phk_cvivit_encode_host(const phk_cvivit_t* m, const float* host_v
   PHK_CUDA(cudaMemcpyAsync(host_ids, dev_ids, R * 8, cudaMemcpyDeviceToHost, st));
   PHK_CUDA(cudaStreamSynchronize(st));
   return 0;
+}
+
+// --------------------------------------------------------------------------------------------
+// CViViT.encode(tokens) (cvivit.py:449-474): the encoder's two stacks on patch tokens, eager launches
+// --------------------------------------------------------------------------------------------
+static bool cvivit_tokens_shape_ok(const phk_cvivit_t* m, int32_t B, int32_t Tp) {
+  return m && B > 0 && Tp > 0 && m->patch_h > 0 && m->patch_w > 0 && m->image_h % m->patch_h == 0 &&
+         m->image_w % m->patch_w == 0 && m->spatial.layers && m->temporal.layers && m->spatial.depth > 0 &&
+         m->temporal.depth > 0;
+}
+
+static int64_t encode_tokens_kmax(const phk_cvivit_t* m) {
+  return tf_kmax(&m->spatial) > tf_kmax(&m->temporal) ? tf_kmax(&m->spatial) : tf_kmax(&m->temporal);
+}
+
+// Carved by phk_cvivit_encode_tokens: x, x_alt, P [R, dim]; the position bias and its scratch; the split-bf16 operands;
+// then the transformers' scratch (one stack at a time).  256 bytes of alignment per piece.
+extern "C" int64_t phk_cvivit_encode_tokens_workspace_bytes(const phk_cvivit_t* m, int32_t B, int32_t Tp, int32_t prec) {
+  if (!cvivit_tokens_shape_ok(m, B, Tp) || !known_prec(prec)) return -1;
+  const int64_t hh = m->image_h / m->patch_h, ww = m->image_w / m->patch_w, hw = hh * ww;
+  const int64_t R = (int64_t)B * Tp * hw;
+  int64_t bytes = 256 * 8 + R * m->dim * 4 * 3;
+  bytes += (int64_t)m->heads * hw * hw * 4 + phk_cpb_scratch_floats(&m->spatial_bias, (int)hh, (int)ww, 1) * 4;
+  if (prec == PHK_PREC_BF16X3) bytes += x3_bytes(R, encode_tokens_kmax(m));
+  const int64_t a = tf_scratch_bytes(&m->spatial, R), b = tf_scratch_bytes(&m->temporal, R);
+  return bytes + (a > b ? a : b);
+}
+
+extern "C" int phk_cvivit_encode_tokens(const phk_cvivit_t* m, const float* tokens, int32_t B, int32_t Tp, float* out,
+                                        void* workspace, int64_t workspace_bytes, int32_t prec,
+                                        const float* spatial_bias, phk_stream_t s) {
+  PHK_REQUIRE(m && tokens && out && workspace, PHK_E_ARG, "cvivit_encode_tokens: null pointer");
+  PHK_REQUIRE(known_prec(prec), PHK_E_ARG, "cvivit_encode_tokens: unknown precision mode");
+  const int64_t need = phk_cvivit_encode_tokens_workspace_bytes(m, B, Tp, prec);
+  PHK_REQUIRE(need > 0, PHK_E_ARG, "cvivit_encode_tokens: bad model table or shape");
+  PHK_REQUIRE(workspace_bytes >= need, PHK_E_WORKSPACE, "cvivit_encode_tokens: workspace too small");
+  const phk_transformer_t* TS = &m->spatial;
+  const phk_transformer_t* TT = &m->temporal;
+  PHK_TRY(check_transformer(TS));
+  PHK_TRY(check_transformer(TT));
+  PHK_REQUIRE(TT->causal && TT->alibi_slopes && !TS->causal, PHK_E_ARG,
+              "cvivit_encode_tokens: the temporal stack is causal with ALiBi slopes, the spatial one is not");
+  PHK_REQUIRE(TT->dim == m->dim && TS->dim == m->dim && TT->heads == m->heads && TS->heads == m->heads &&
+              TT->dim_head == m->dim_head && TS->dim_head == m->dim_head, PHK_E_ARG,
+              "cvivit_encode_tokens: transformer widths differ from the model's");
+  PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "cvivit_encode_tokens: dim must be a multiple of 4");
+  for (int l = 0; l < TT->depth; ++l) PHK_REQUIRE(!TT->layers[l].has_cross, PHK_E_ARG, "cvivit_encode_tokens: cross-attention layer");
+  for (int l = 0; l < TS->depth; ++l) PHK_REQUIRE(!TS->layers[l].has_cross, PHK_E_ARG, "cvivit_encode_tokens: cross-attention layer");
+  const int hh = m->image_h / m->patch_h, ww = m->image_w / m->patch_w;
+  const int64_t R = (int64_t)B * Tp * hh * ww;
+  Arena ar{(char*)workspace, workspace_bytes, 0};
+  float* x = (float*)ar.take(R * m->dim * 4);
+  float* x_alt = (float*)ar.take(R * m->dim * 4);
+  float* P = (float*)ar.take(R * m->dim * 4);
+  float* bias_buf = (float*)ar.take((int64_t)m->heads * hh * ww * hh * ww * 4);
+  float* cpb_scratch = (float*)ar.take(phk_cpb_scratch_floats(&m->spatial_bias, hh, ww, 1) * 4);
+  PHK_REQUIRE(x && x_alt && P && bias_buf && cpb_scratch, PHK_E_WORKSPACE, "cvivit_encode_tokens: workspace too small");
+  Lin lin{prec, nullptr, 0};
+  if (prec == PHK_PREC_BF16X3) {
+    lin.a3_bytes = x3_bytes(R, encode_tokens_kmax(m));
+    lin.a3 = ar.take(lin.a3_bytes);
+    PHK_REQUIRE(lin.a3, PHK_E_WORKSPACE, "cvivit_encode_tokens: workspace too small (split operands)");
+  }
+  PHK_CUDA(cudaMemcpyAsync(x, tokens, R * m->dim * 4, cudaMemcpyDeviceToDevice, to_stream(s)));
+  float* xf = nullptr;
+  return cvivit_encode_stacks(m, B, Tp, hh, ww, x, x_alt, P, spatial_bias, bias_buf, cpb_scratch, prec, lin, ar, nullptr,
+                              out, &xf, s);
 }
 
 // --------------------------------------------------------------------------------------------

@@ -2095,7 +2095,8 @@ struct CvGeom {
   int64_t R = 0, rows1 = 0, rows2 = 0, K1 = 0, K2 = 0, inner = 0;
 };
 
-CvGeom cv_geom(const phk_cvivit_dec_t* m, int B, int Tp, int64_t inner) {
+template <class M>  // phk_cvivit_t or phk_cvivit_dec_t: both carry the geometry fields read here
+CvGeom cv_geom(const M* m, int B, int Tp, int64_t inner) {
   CvGeom g;
   g.B = B; g.Tp = Tp; g.hh = m->image_h / m->patch_h; g.ww = m->image_w / m->patch_w; g.hw = g.hh * g.ww;
   g.D = m->dim; g.H = m->heads; g.DH = m->dim_head; g.I = g.H * g.DH; g.C = m->channels; g.F = 1 + (Tp - 1) * m->patch_t;
@@ -2322,20 +2323,83 @@ int decode_backward_phase(const phk_cvivit_dec_t* m, const phk_cvivit_dec_t* gra
   return 0;
 }
 
+// Arena space of encode_backward_phase: the layers' saves, the spatial norm_out, its (b h w t) copy, the temporal norm_out
+int64_t enc_stacks_floats(const phk_cvivit_t* m, const CvGeom& g) {
+  int64_t f = 3 * g.R * g.D;
+  for (int l = 0; l < m->spatial.depth; ++l) f += layer_save_floats(&m->spatial, m->spatial.layers[l], g.R, 0);
+  for (int l = 0; l < m->temporal.depth; ++l) f += layer_save_floats(&m->temporal, m->temporal.layers[l], g.R, 0);
+  return f + 256 * 4 / 4;
+}
+
+// Arena space of phk_cvivit_backward's encoder phase (the stacks' space is dead before the patch gradients are taken,
+// but it is counted in full)
 int64_t enc_phase_floats(const phk_cvivit_t* m, const CvGeom& g, bool dvideo) {
   const int64_t rows2 = imax(g.rows2, 1);
   const int64_t patch = imax(g.rows1 * g.K1, g.rows2 * g.K2);
   int64_t f = 2 * (g.rows1 * g.K1 + rows2 * g.K2);                               // raw patch rows, LN1 outputs
-  f += (g.rows1 + rows2) * g.D + g.R * g.D;                                      // Linear outputs, LN2 outputs (b t h w)
-  for (int l = 0; l < m->spatial.depth; ++l) f += layer_save_floats(&m->spatial, m->spatial.layers[l], g.R, 0);
-  for (int l = 0; l < m->temporal.depth; ++l) f += layer_save_floats(&m->temporal, m->temporal.layers[l], g.R, 0);
-  f += 4 * g.R * g.D;                                                            // norm_outs and their permuted copies
+  f += (g.rows1 + rows2) * g.D + 2 * g.R * g.D;                                  // Linear outputs, LN2 outputs, z (b t h w)
+  f += enc_stacks_floats(m, g);
   f += (g.rows1 + rows2) * g.D + imax(g.rows1, rows2) * g.D;                     // d LN2 outputs split, d Linear outputs
   f += patch * (dvideo ? 2 : 1);                                                 // d LN1 outputs, d patch rows
-  return f + 256 * 24 / 4;
+  return f + 256 * 16 / 4;
 }
 
-bool cvivit_shapes_ok(const phk_cvivit_dec_t* m, int32_t B, int32_t Tp) {
+// The encoder stacks' half of both encoder backward entry points (cvivit.py:449-474): recomputes the spatial stack on x0
+// ((b t h w) rows) and the temporal stack on its permuted norm_out with their activations saved in `ar` (a copy: all of it
+// is dead on return), then differentiates norm_out(temporal) from dout ((b t h w) rows; it may be one of S's gradient
+// streams).  z (NULL: not formed): receives the recomputed output, (b t h w) rows.  On return *dx0 = d x0 in (b t h w)
+// rows, in a gradient stream of S; dtokens (NULL: not wanted) receives a copy (written, not added).  cpb_now: finish the
+// position-bias MLP's gradient here; otherwise S.dbias_s is left to the caller.
+int encode_backward_phase(const phk_cvivit_t* m, const phk_cvivit_t* grads, const float* x0, const CvGeom& g,
+                          const float* dout, float* z, float* dtokens, const float** dx0, const CvShared& S, Arena ar,
+                          bool cpb_now, int prec, phk_stream_t s) {
+  const phk_transformer_t* ES = &m->spatial;
+  const phk_transformer_t* ET = &m->temporal;
+  const int B = g.B, Tp = g.Tp, hw = g.hw, D = g.D;
+  const int64_t R = g.R;
+  const cudaStream_t st = to_stream(s);
+
+  // ---------------------------------------------------------------- forward, saving activations
+  const LayerCall cs = spatial_call(ES, &grads->spatial, g, S, prec, s);
+  LayerCall ct;
+  PHK_TRY(temporal_call(ET, &grads->temporal, g, S, prec, s, &ct));
+  std::unique_ptr<LayerSave[]> svS(new (std::nothrow) LayerSave[ES->depth]), svT(new (std::nothrow) LayerSave[ET->depth]);
+  PHK_REQUIRE(svT && svS, PHK_E_ARG, "cvivit_encode_backward: out of host memory");
+  const float* xfS = nullptr;
+  PHK_TRY(stack_forward(cs, x0, svS.get(), &xfS, ar));
+  float* nS = ar.f(R * D); float* Pt = ar.f(R * D);
+  PHK_REQUIRE(nS && Pt, PHK_E_WORKSPACE, "cvivit_encode_backward: workspace too small");
+  PHK_TRY(phk_layernorm(xfS, ES->out_g, ES->out_b, nS, nullptr, R, D, 0, 0, 0, 0, s));
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, nS, Pt, B, Tp, hw, D, 1);
+  PHK_LAUNCH_CHECK();
+  const float* xfT = nullptr;
+  PHK_TRY(stack_forward(ct, Pt, svT.get(), &xfT, ar));
+  if (z) {
+    float* nT = ar.f(R * D);
+    PHK_REQUIRE(nT, PHK_E_WORKSPACE, "cvivit_encode_backward: workspace too small");
+    PHK_TRY(phk_layernorm(xfT, ET->out_g, ET->out_b, nT, nullptr, R, D, 0, 0, 0, 0, s));
+    PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, nT, z, B, Tp, hw, D, 0);
+    PHK_LAUNCH_CHECK();
+  }
+
+  // ---------------------------------------------------------------- temporal stack on (b h w t) rows, then spatial
+  const LayerGrads& G = S.G;
+  float* dx = S.dx;
+  float* dx_alt = S.dx_alt;
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dout, G.dtmp, B, Tp, hw, D, 1);
+  PHK_LAUNCH_CHECK();
+  PHK_TRY(stack_backward(ct, svT.get(), xfT, G.dtmp, &dx, &dx_alt, G));
+  PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 0);
+  PHK_LAUNCH_CHECK();
+  PHK_TRY(stack_backward(cs, svS.get(), xfS, G.dtmp, &dx, &dx_alt, G));
+  if (dtokens) PHK_CUDA(cudaMemcpyAsync(dtokens, dx, R * D * 4, cudaMemcpyDeviceToDevice, st));
+  if (dx0) *dx0 = dx;
+  if (cpb_now) PHK_TRY(cpb_backward(m->spatial_bias, grads->spatial_bias, S.dbias_s, g.hh, g.ww, 1, S.cpb_bwd_sc, st));
+  return 0;
+}
+
+template <class M>  // phk_cvivit_t or phk_cvivit_dec_t
+bool cvivit_shapes_ok(const M* m, int32_t B, int32_t Tp) {
   return m && B > 0 && Tp > 0 && m->temporal.layers && m->spatial.layers && m->temporal.depth > 0 && m->spatial.depth > 0 &&
          m->patch_h > 0 && m->patch_w > 0 && m->patch_t > 0 && m->image_h % m->patch_h == 0 && m->image_w % m->patch_w == 0;
 }
@@ -2496,39 +2560,16 @@ extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* 
       PHK_TRY(phk_layernorm(Pe2, enc->pr_ln2_g, enc->pr_ln2_b, x0, nullptr, rows2, D, 0, (int64_t)(Tp - 1) * hw,
                             (int64_t)Tp * hw, hw, s));
     }
-    const LayerCall cs = spatial_call(ES, &enc_grads->spatial, g, S, prec, s);
-    LayerCall ct;
-    PHK_TRY(temporal_call(ET, &enc_grads->temporal, g, S, prec, s, &ct));
-    std::unique_ptr<LayerSave[]> svS(new (std::nothrow) LayerSave[ES->depth]), svT(new (std::nothrow) LayerSave[ET->depth]);
-    PHK_REQUIRE(svT && svS, PHK_E_ARG, "cvivit_backward: out of host memory");
-    const float* xfS = nullptr;
-    PHK_TRY(stack_forward(cs, x0, svS.get(), &xfS, ea));
-    float* nS = ea.f(R * D); float* Pt = ea.f(R * D);
-    PHK_REQUIRE(nS && Pt, PHK_E_WORKSPACE, "cvivit_backward: workspace too small");
-    PHK_TRY(phk_layernorm(xfS, ES->out_g, ES->out_b, nS, nullptr, R, D, 0, 0, 0, 0, s));
-    PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, nS, Pt, B, Tp, hw, D, 1);
-    PHK_LAUNCH_CHECK();
-    const float* xfT = nullptr;
-    PHK_TRY(stack_forward(ct, Pt, svT.get(), &xfT, ea));
-    float* nT = ea.f(R * D); float* z = ea.f(R * D);
-    PHK_REQUIRE(nT && z, PHK_E_WORKSPACE, "cvivit_backward: workspace too small");
-    PHK_TRY(phk_layernorm(xfT, ET->out_g, ET->out_b, nT, nullptr, R, D, 0, 0, 0, 0, s));
-    PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, nT, z, B, Tp, hw, D, 0);
-    PHK_LAUNCH_CHECK();
+    float* z = ea.f(R * D);
+    PHK_REQUIRE(z, PHK_E_WORKSPACE, "cvivit_backward: workspace too small");
 
-    // ---------------------------------------------------------------- project_in, then the two stacks
+    // ---------------------------------------------------------------- the two stacks, then project_in against their output
     const LayerGrads& G = S.G;
-    float* dx = S.dx;
-    float* dx_alt = S.dx_alt;
+    PHK_TRY(dgrad(dq, enc->vq_w, S.dx, R, bits, D, 0, st));  // d(encoder output), (b t h w)
+    const float* dx = nullptr;
+    PHK_TRY(encode_backward_phase(enc, enc_grads, x0, g, S.dx, z, nullptr, &dx, S, ea, false, prec, s));
     PHK_TRY(wgrad(dq, z, (float*)enc_grads->vq_w, R, bits, D, st));
     PHK_TRY(colsum(dq, R, bits, bits, (float*)enc_grads->vq_b, st));
-    PHK_TRY(dgrad(dq, enc->vq_w, dx, R, bits, D, 0, st));  // d(encoder output), (b t h w)
-    PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 1);
-    PHK_LAUNCH_CHECK();
-    PHK_TRY(stack_backward(ct, svT.get(), xfT, G.dtmp, &dx, &dx_alt, G));
-    PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 0);
-    PHK_LAUNCH_CHECK();
-    PHK_TRY(stack_backward(cs, svS.get(), xfS, G.dtmp, &dx, &dx_alt, G));
 
     // ---------------------------------------------------------------- to_patch_emb_first_frame / to_patch_emb
     float* dE1 = ea.f(rows1 * D); float* dE2 = ea.f(r2 * D);
@@ -2564,4 +2605,41 @@ extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* 
 
   // ---------------------------------------------------------------- position-bias MLP, once over both spatial stacks
   return cpb_backward(dec->spatial_bias, dec_grads->spatial_bias, S.dbias_s, g.hh, g.ww, 1, S.cpb_bwd_sc, st);
+}
+
+extern "C" int64_t phk_cvivit_encode_backward_workspace_bytes(const phk_cvivit_t* m, int32_t B, int32_t Tp, int32_t prec) {
+  if (!cvivit_shapes_ok(m, B, Tp)) return -1;
+  const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(&m->spatial), stack_inner(&m->temporal)));
+  return cv_shared_bytes(g, m->spatial_bias, prec) + enc_stacks_floats(m, g) * 4;
+}
+
+// See include/phk.h.
+extern "C" int phk_cvivit_encode_backward(const phk_cvivit_t* m, const phk_cvivit_t* grads, const float* tokens, int32_t B,
+                                          int32_t Tp, const float* dout, float* dtokens, void* workspace,
+                                          int64_t workspace_bytes, int32_t prec, phk_stream_t s) {
+  PHK_REQUIRE(m && grads && tokens && dout && workspace, PHK_E_ARG, "cvivit_encode_backward: null pointer");
+  PHK_REQUIRE(prec == PHK_PREC_F32 || prec == PHK_PREC_BF16, PHK_E_ARG, "cvivit_encode_backward: unknown precision mode");
+  const int64_t need = phk_cvivit_encode_backward_workspace_bytes(m, B, Tp, prec);
+  PHK_REQUIRE(need > 0, PHK_E_ARG, "cvivit_encode_backward: bad model table or shape");
+  PHK_REQUIRE(workspace_bytes >= need, PHK_E_WORKSPACE, "cvivit_encode_backward: workspace too small");
+  const phk_transformer_t* TS = &m->spatial;
+  const phk_transformer_t* TT = &m->temporal;
+  PHK_REQUIRE(grads->temporal.layers && grads->spatial.layers && grads->temporal.depth == TT->depth &&
+              grads->spatial.depth == TS->depth, PHK_E_ARG, "cvivit_encode_backward: weight table / gradient table mismatch");
+  const phk_cpb_t& gc = grads->spatial_bias;
+  PHK_REQUIRE(gc.w0 && gc.b0 && gc.w1 && gc.b1 && gc.w2 && gc.b2, PHK_E_ARG,
+              "cvivit_encode_backward: the gradient table has no position-bias MLP");
+  PHK_REQUIRE(TT->causal && TT->alibi_slopes && !TS->causal, PHK_E_ARG,
+              "cvivit_encode_backward: the temporal stack is causal with ALiBi slopes, the spatial one is not");
+  PHK_REQUIRE(TT->dim == m->dim && TS->dim == m->dim && TT->heads == m->heads && TS->heads == m->heads &&
+              TT->dim_head == m->dim_head && TS->dim_head == m->dim_head, PHK_E_ARG,
+              "cvivit_encode_backward: transformer widths differ from the model's");
+  PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "cvivit_encode_backward: dim must be a multiple of 4");
+  for (int l = 0; l < TT->depth; ++l) PHK_REQUIRE(!TT->layers[l].has_cross, PHK_E_ARG, "cvivit_encode_backward: cross-attention layer");
+  for (int l = 0; l < TS->depth; ++l) PHK_REQUIRE(!TS->layers[l].has_cross, PHK_E_ARG, "cvivit_encode_backward: cross-attention layer");
+  const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(TS), stack_inner(TT)));
+  Arena ar{(char*)workspace, workspace_bytes, 0};
+  CvShared S;
+  PHK_TRY(cv_shared_init(ar, g, m->spatial_bias, prec, s, S));
+  return encode_backward_phase(m, grads, tokens, g, dout, nullptr, dtokens, nullptr, S, ar, true, prec, s);
 }

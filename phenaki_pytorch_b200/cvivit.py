@@ -5,7 +5,8 @@ Same constructor keywords, attribute names and state-dict layout as the referenc
 return_only_codebook_ids=True)`` (cvivit.py:518-574) runs entirely in libphk.so
 (phk_cvivit_encode).  With ``use_vgg_and_gan=False`` and LFQ, ``loss = forward(video)`` is the reference's
 reconstruction loss and ``loss.backward()`` fills the gradients through the decoder, LFQ's straight-through estimator
-and the encoder (phk_cvivit_backward).  The GAN / perceptual losses, discriminator and VGG (cvivit.py:59-213, 600-671)
+and the encoder (phk_cvivit_backward).  ``encode(tokens)`` runs the encoder's two stacks on patch tokens
+(phk_cvivit_encode_tokens) and is differentiable through phk_cvivit_encode_backward.  The GAN / perceptual losses, discriminator and VGG (cvivit.py:59-213, 600-671)
 are out of scope (SURVEY.md section 2, rows 8/10) and raise.
 """
 import copy
@@ -429,22 +430,29 @@ class CViViT(nn.Module):
                                               L.ptr(loss), L.stream_ptr()), "phk_cvivit_recon_loss")
         return ids, loss, recon
 
-    def _enc_grad_table(self, gk):
-        """The phk_cvivit_t-shaped table addressing the encoder side's gradient buffers in ``gk``."""
+    def _enc_grad_table(self, gk, recon):
+        """The phk_cvivit_t-shaped table addressing the encoder side's gradient buffers in ``gk``: both stacks, plus
+        to_patch_emb* and LFQ's project_in for the reconstruction loss (``recon``; the position-bias MLP's gradient then
+        goes through the decoder's table), or the position-bias MLP for ``encode`` (no quantiser: cosine-sim modules too)."""
         t = L.CvivitT()
         t.dim, t.heads, t.dim_head, t.channels = self.dim, self.heads, self.dim_head, self.channels
         t.image_h, t.image_w = self.image_size
         t.patch_h, t.patch_w = self.patch_size
         t.patch_t = self.temporal_patch_size
-        t.codebook_bits = self.vq.codebook_dim
-        f, r = self.to_patch_emb_first_frame, self.to_patch_emb
-        t.pf_ln1_g, t.pf_ln1_b, t.pf_w, t.pf_b = gk.g(f[1].weight), gk.g(f[1].bias), gk.g(f[2].weight), gk.g(f[2].bias)
-        t.pf_ln2_g, t.pf_ln2_b = gk.g(f[3].weight), gk.g(f[3].bias)
-        t.pr_ln1_g, t.pr_ln1_b, t.pr_w, t.pr_b = gk.g(r[1].weight), gk.g(r[1].bias), gk.g(r[2].weight), gk.g(r[2].bias)
-        t.pr_ln2_g, t.pr_ln2_b = gk.g(r[3].weight), gk.g(r[3].bias)
+        if recon:
+            t.codebook_bits = self.vq.codebook_dim
+            f, r = self.to_patch_emb_first_frame, self.to_patch_emb
+            t.pf_ln1_g, t.pf_ln1_b = gk.g(f[1].weight), gk.g(f[1].bias)
+            t.pf_w, t.pf_b = gk.g(f[2].weight), gk.g(f[2].bias)
+            t.pf_ln2_g, t.pf_ln2_b = gk.g(f[3].weight), gk.g(f[3].bias)
+            t.pr_ln1_g, t.pr_ln1_b = gk.g(r[1].weight), gk.g(r[1].bias)
+            t.pr_w, t.pr_b = gk.g(r[2].weight), gk.g(r[2].bias)
+            t.pr_ln2_g, t.pr_ln2_b = gk.g(r[3].weight), gk.g(r[3].bias)
+            t.vq_w, t.vq_b = gk.g(self.vq.project_in.weight), gk.g(self.vq.project_in.bias)
+        else:
+            t.spatial_bias = cpb_grad_table(self.spatial_rel_pos_bias, gk)
         t.spatial = transformer_grad_table(self.enc_spatial_transformer, gk, False)
         t.temporal = transformer_grad_table(self.enc_temporal_transformer, gk, False)
-        t.vq_w, t.vq_b = gk.g(self.vq.project_in.weight), gk.g(self.vq.project_in.bias)
         return t
 
     def _recon_backward(self, spec, video, ids, recon, dloss, drecon, want_video_grad):
@@ -462,7 +470,7 @@ class CViViT(nn.Module):
         with torch.cuda.device(dev):
             enc, dec = self._table(), self._dec_table()
             gk = GradKeep(spec["params"])
-            egt = self._enc_grad_table(gk)
+            egt = self._enc_grad_table(gk, True)
             dgt = self._dec_grad_table(gk, True)
             dloss = (torch.zeros((), dtype=torch.float32, device=dev) if dloss is None
                      else dloss.to(dev, torch.float32).contiguous())
@@ -597,6 +605,80 @@ class CViViT(nn.Module):
         return self._differentiable_decode(None, tokens.reshape(b, n, d), b, n // per, tokens.device)
 
 
+    # ---- encode of patch tokens (cvivit.py:449-474) and its backward -------------------------------------------------
+    def _encode_params(self):
+        """The parameters ``encode`` reaches: both encoder stacks and the spatial position-bias MLP."""
+        mods = [self.enc_spatial_transformer, self.enc_temporal_transformer, self.spatial_rel_pos_bias]
+        return [p for m in mods for p in m.parameters()]
+
+    def _encode_tokens(self, tokens):
+        """phk_cvivit_encode_tokens on contiguous fp32 (b, t, h, w, dim) tokens: a new tensor of the same shape."""
+        lib = L.lib()
+        b, tp = tokens.shape[:2]
+        dev = tokens.device
+        with torch.cuda.device(dev):
+            table = self._table()
+            out = torch.empty_like(tokens)
+            nbytes = lib.phk_cvivit_encode_tokens_workspace_bytes(C.byref(table), b, tp, self.precision)
+            if nbytes < 0:
+                raise L.PhkError("phk_cvivit_encode_tokens_workspace_bytes: unsupported configuration")
+            ws = self._ws.get(nbytes, dev)
+            bias = self._spatial_bias(table, dev)
+            L.check(lib.phk_cvivit_encode_tokens(C.byref(table), L.ptr(tokens), b, tp, L.ptr(out), L.ptr(ws), ws.numel(),
+                                                 self.precision, L.ptr(bias), L.stream_ptr()),
+                    "phk_cvivit_encode_tokens")
+        return out
+
+    def _encode_backward(self, spec, dout, tokens, want_tokens_grad):
+        """phk_cvivit_encode_backward for one ``encode`` call: ([gradient or None per parameter of spec["params"]],
+        d tokens or None)."""
+        if weights_signature(self) != spec["sig"]:
+            raise RuntimeError("a parameter of this module was modified or replaced between the encode and the backward: "
+                               "the backward recomputes the encode from the current weights, so it would differentiate "
+                               "another function")
+        lib = L.lib()
+        dout = L.require_cuda(dout.to(torch.float32), "upstream gradient")
+        dev = dout.device
+        b, tp = spec["b"], spec["tp"]
+        prec = L.PREC_BF16 if spec["precision"] == L.PREC_BF16 else L.PREC_F32  # split-bf16 is an inference mode
+        with torch.cuda.device(dev):
+            table = self._table()
+            gk = GradKeep(spec["params"])
+            gtable = self._enc_grad_table(gk, False)
+            dtokens = torch.empty_like(tokens) if want_tokens_grad else None
+            nbytes = lib.phk_cvivit_encode_backward_workspace_bytes(C.byref(table), b, tp, prec)
+            if nbytes < 0:
+                raise L.PhkError("phk_cvivit_encode_backward_workspace_bytes: unsupported configuration")
+            ws = self._ws.get(nbytes, dev)
+            L.check(lib.phk_cvivit_encode_backward(C.byref(table), C.byref(gtable), L.ptr(tokens), b, tp, L.ptr(dout),
+                                                   L.ptr(dtokens), L.ptr(ws), ws.numel(), prec, L.stream_ptr()),
+                    "phk_cvivit_encode_backward")
+        return [gk.grad_of(p) for p in spec["params"]], dtokens
+
+    def encode(self, tokens):
+        """tokens (b, t, h, w, dim) fp32 CUDA, (h, w) = patch_height_width -> a new (b, t, h, w, dim) fp32 tensor: the
+        encoder's spatial and temporal transformers (cvivit.py:449-474), the temporal one's norm_out included.  The
+        quantiser is not involved.  Differentiable: with grad mode on and ``tokens`` or an encoder-stack / position-bias
+        parameter requiring grad, ``f(out).backward()`` fills their gradients through phk_cvivit_encode_backward, which
+        recomputes both stacks with saved activations.  No dropout is applied (DESIGN.md section 8)."""
+        assert tokens.ndim == 5, f"tokens must be (b, t, h, w, dim), got {tuple(tokens.shape)}"
+        b, t, h, w, d = tokens.shape
+        assert (h, w) == tuple(self.patch_height_width), \
+            f"tokens cover {h} x {w} patches, the module's frames {self.patch_height_width}"
+        assert d == self.dim, f"token width {d} is not the module's dim {self.dim}"
+        assert b > 0 and t > 0, "empty batch or no latent frames"
+        tokens = L.require_cuda(tokens, "tokens", torch.float32)
+
+        def run():
+            return self._encode_tokens(tokens.detach())
+
+        params = self._encode_params()
+        if not torch.is_grad_enabled() or not (tokens.requires_grad or any(p.requires_grad for p in params)):
+            return run()
+        spec = dict(net=self, params=params, b=b, tp=t, precision=self.precision, sig=weights_signature(self))
+        return _EncodeFn.apply(run, spec, tokens, *params)
+
+
 class _DecodeFn(torch.autograd.Function):
     """Makes the C-ViViT decode differentiable.  The forward runs the library's decode unchanged (same launches, same
     values) and keeps only its inputs; the backward recomputes it with saved activations inside
@@ -644,3 +726,26 @@ class _ReconLossFn(torch.autograd.Function):
         spec = ctx.spec
         grads, dvideo = spec["net"]._recon_backward(spec, video, ids, recon, dloss, drecon, ctx.needs_input_grad[1])
         return (None, dvideo, *grads)
+
+
+class _EncodeFn(torch.autograd.Function):
+    """Makes ``CViViT.encode(tokens)`` differentiable.  The forward runs the library's encoder stacks unchanged (same
+    launches, same values) and keeps only the detached tokens; the backward recomputes both stacks with saved
+    activations inside phk_cvivit_encode_backward.  No dropout either way: it differentiates the function the forward
+    returned."""
+
+    @staticmethod
+    def forward(ctx, run, spec, tokens, *params):
+        ctx.spec = spec
+        ctx.save_for_backward(tokens.detach())
+        return run()
+
+    @staticmethod
+    def backward(ctx, dout):
+        if torch.is_grad_enabled():
+            raise RuntimeError("CViViT.encode does not support create_graph=True: its backward is hand-written CUDA and "
+                               "builds no graph of its own")
+        tokens, = ctx.saved_tensors
+        spec = ctx.spec
+        grads, dtokens = spec["net"]._encode_backward(spec, dout, tokens, ctx.needs_input_grad[2])
+        return (None, None, dtokens, *grads)
