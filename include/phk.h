@@ -487,7 +487,21 @@ int phk_cvivit_recon_loss(const float* video, const float* recon, const uint8_t*
  *   frame_mask         NULL or uint8 (B, F), as for phk_cvivit_recon_loss
  *   dloss              ONE fp32 on the device (the backward never synchronises the host); drecon NULL or like recon
  *   dvideo             NULL, or fp32 like video: receives d loss / d video (written, not added)
- * prec: PHK_PREC_F32 or PHK_PREC_BF16 (the training step's bf16 products); no dropout is applied. */
+ * prec: PHK_PREC_F32 or PHK_PREC_BF16 (the training step's bf16 products); no dropout is applied.
+ * Data-parallel overlap: events registered with phk_train_set_progress_events before the call are recorded by it, on s,
+ * each once every gradient of its group is final, in this order (dS / dT: the stack depths of the table named):
+ *   1                 dec to_pixels_first_frame + to_pixels
+ *   dS(dec)           dec spatial: norm_out with layer dS-1, then layers dS-2 .. 0, one event each
+ *   dT(dec)           dec temporal: the same
+ *   1                 dec project_out (vq_out_*)
+ *   dT(enc)           enc temporal: norm_out with layer dT-1, then layers dT-2 .. 0      } empty groups without
+ *   dS(enc)           enc spatial: the same                                               } straight_through: their
+ *   1                 enc project_in (vq_*)                                               } events are recorded
+ *   1                 enc to_patch_emb_first_frame + to_patch_emb (pf_*, pr_*)            } all the same
+ *   1                 the position-bias MLP (dec_grads->spatial_bias); this last event also means "everything"
+ * phk_cvivit_backward_progress_groups returns that count (-1 on a bad table).  With no events registered the call issues
+ * the same launches in the same order; the events add records, nothing else. */
+int32_t phk_cvivit_backward_progress_groups(const phk_cvivit_t* enc, const phk_cvivit_dec_t* dec);
 int64_t phk_cvivit_backward_workspace_bytes(const phk_cvivit_t* enc, const phk_cvivit_dec_t* dec, int32_t B, int32_t F,
                                             int32_t prec);
 int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* enc_grads, const phk_cvivit_dec_t* dec,
@@ -678,7 +692,8 @@ int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_t* grads, c
                            const phk_dropout_t* dropout);
 /* Data-parallel overlap: `events` (cudaEvent_t handles, count >= depth + 2) are recorded by the NEXT phk_maskgit_train_step
  * call of the calling thread, on its stream, as gradient groups become final: events[0] head + norm_out, events[1 + k]
- * transformer layer depth-1-k, events[depth + 1] embeddings + position-bias MLP (= all).  One-shot; NULL clears. */
+ * transformer layer depth-1-k, events[depth + 1] embeddings + position-bias MLP (= all).  If the next such call is
+ * phk_cvivit_backward instead, it records them in its own group order (see there).  One-shot; NULL clears. */
 int phk_train_set_progress_events(void** events, int32_t count);
 
 /* Backward of a MaskGit / TokenCritic / SelfCritic forward from a gradient the caller supplies: what

@@ -194,6 +194,7 @@ PROTOTYPES = {
     "phk_cvivit_backward_workspace_bytes": [C.POINTER(CvivitT), C.POINTER(CvivitDecT), i32, i32, i32],
     "phk_cvivit_backward": [C.POINTER(CvivitT), C.POINTER(CvivitT), C.POINTER(CvivitDecT), C.POINTER(CvivitDecT), vp, vp,
                             vp, vp, i32, i32, vp, vp, vp, i32, vp, i64, i32, vp],
+    "phk_cvivit_backward_progress_groups": [C.POINTER(CvivitT), C.POINTER(CvivitDecT)],
 }
 _RESTYPES = {"phk_attention_tc_scratch_bytes": i64, "phk_head_sample_scratch_bytes": i64,
              "phk_maskgit_sample_workspace_bytes": i64, "phk_maskgit_demask_iteration_workspace_bytes": i64, "phk_sample_tail_scratch_bytes": i64, "phk_vq_cosine_scratch_bytes": i64, "phk_maskgit_train_workspace_bytes": i64, "phk_maskgit_train_dropout_counters": i64, "phk_maskgit_backward_workspace_bytes": i64, "phk_cvivit_decode_backward_workspace_bytes": i64, "phk_cvivit_backward_workspace_bytes": i64, "phk_cvivit_encode_tokens_workspace_bytes": i64, "phk_cvivit_encode_backward_workspace_bytes": i64, "phk_last_error": C.c_char_p, "phk_launch_count": i64, "phk_cpb_scratch_floats": i64,

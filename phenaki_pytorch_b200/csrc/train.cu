@@ -1190,10 +1190,11 @@ uint64_t dropout_layout(const phk_maskgit_t* m, int b, int n, int L, uint64_t (*
 
 using namespace phk;
 
-// Data-parallel overlap (SURVEY 8e): the caller may hand in CUDA events that the NEXT phk_maskgit_train_step call of this
-// thread records on its stream as groups of gradients become final -- events[0]: the head + norm_out, events[1 + k]:
-// transformer layer depth-1-k (backward order), events[depth + 1]: embeddings + position-bias MLP = everything.  A side
-// stream can then all-reduce each finished slice of the flat gradient bucket while the layers below still run.
+// Data-parallel overlap (SURVEY 8e): the caller may hand in CUDA events that the NEXT phk_maskgit_train_step or
+// phk_cvivit_backward call of this thread records on its stream as groups of gradients become final -- for the MaskGit
+// step events[0]: the head + norm_out, events[1 + k]: transformer layer depth-1-k (backward order), events[depth + 1]:
+// embeddings + position-bias MLP = everything; for C-ViViT see phk_cvivit_backward_progress_groups.  A side stream can
+// then all-reduce each finished slice of the flat gradient bucket while the layers below still run.
 static thread_local void** g_progress_events = nullptr;
 static thread_local int g_progress_count = 0;
 extern "C" int phk_train_set_progress_events(void** events, int32_t count) {
@@ -1204,6 +1205,16 @@ extern "C" int phk_train_set_progress_events(void** events, int32_t count) {
 static inline int progress_mark(void** ev, int n, int idx, cudaStream_t st) {
   if (ev && idx < n && ev[idx]) PHK_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(ev[idx]), st));
   return 0;
+}
+
+// The progress events of one C-ViViT backward, recorded in order: each progress_next closes the next group.  A NULL
+// Progress (the entry points that take no events) records nothing.
+struct Progress {
+  void** ev = nullptr;
+  int n = 0, next = 0;
+};
+static inline int progress_next(Progress* p, cudaStream_t st) {
+  return p ? progress_mark(p->ev, p->n, p->next++, st) : 0;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -2205,13 +2216,17 @@ int stack_forward(const LayerCall& c, const float* x, LayerSave* sv, const float
   return 0;
 }
 
-// Backward of norm_out(stack(x)) from dy = d/d(norm_out output): on return *dx holds d/d(x) (*dx, *dx_alt may swap)
+// Backward of norm_out(stack(x)) from dy = d/d(norm_out output): on return *dx holds d/d(x) (*dx, *dx_alt may swap).
+// prog: one event per layer, top layer (with norm_out) first
 int stack_backward(const LayerCall& c, const LayerSave* sv, const float* xf, const float* dy, float** dx, float** dx_alt,
-                   const LayerGrads& G) {
+                   const LayerGrads& G, Progress* prog) {
   const DropSite none{0.f, 0.f, 0u, 0u, 0u};
   const int64_t R = (int64_t)c.b * c.n;
   PHK_TRY(ln_backward(xf, c.T->out_g, dy, *dx, 0, (float*)c.GT->out_g, nullptr, G.stats, R, c.T->dim, c.st));
-  for (int l = c.T->depth - 1; l >= 0; --l) PHK_TRY(layer_backward(c, l, sv[l], dx, dx_alt, G, nullptr, none, none, none));
+  for (int l = c.T->depth - 1; l >= 0; --l) {
+    PHK_TRY(layer_backward(c, l, sv[l], dx, dx_alt, G, nullptr, none, none, none));
+    PHK_TRY(progress_next(prog, c.st));
+  }
   return 0;
 }
 
@@ -2230,9 +2245,10 @@ int64_t dec_phase_floats(const phk_cvivit_dec_t* m, const CvGeom& g) {
 // of it is dead on return) and differentiates it from d video.  With ids, project_out's gradients are accumulated.
 // cpb_now: finish the position-bias MLP's gradient here; otherwise S.dbias_s is left to the caller.  dcodes_out (or
 // dtokens): receives d/d(decoder input) in (b t h w) rows, in dtokens when given, else in a free gradient stream of S.
+// prog (NULL: none): one event after to_pixels*, one per spatial then temporal layer, one after project_out (ids only).
 int decode_backward_phase(const phk_cvivit_dec_t* m, const phk_cvivit_dec_t* grads, const int64_t* ids, const float* tokens,
                           const CvGeom& g, const float* dvideo, float* dtokens, const float** dcodes_out, const CvShared& S,
-                          Arena ar, bool cpb_now, int prec, phk_stream_t s) {
+                          Arena ar, bool cpb_now, int prec, phk_stream_t s, Progress* prog) {
   const phk_transformer_t* TT = &m->temporal;
   const phk_transformer_t* TS = &m->spatial;
   const int B = g.B, Tp = g.Tp, hw = g.hw, D = g.D, C = g.C, F = g.F;
@@ -2293,17 +2309,18 @@ int decode_backward_phase(const phk_cvivit_dec_t* m, const phk_cvivit_dec_t* gra
     PHK_TRY(colsum(dG, rows2, (int)K2, K2, (float*)grads->px_b, st));
     PHK_TRY(dgrad_p(prec, S.tc, dG, m->px_w, dEr, rows2, K2, D, 0, s));
   }
+  PHK_TRY(progress_next(prog, st));  // to_pixels_first_frame / to_pixels final
   PHK_KERNEL_LAUNCH(frames_merge_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dEf, dEr, G.dtmp, B, Tp, hw, D);
   PHK_LAUNCH_CHECK();
 
   // ---------------------------------------------------------------- spatial stack, position-bias MLP
-  PHK_TRY(stack_backward(cs, svS.get(), xfS, G.dtmp, &dx, &dx_alt, G));
+  PHK_TRY(stack_backward(cs, svS.get(), xfS, G.dtmp, &dx, &dx_alt, G, prog));
   if (cpb_now) PHK_TRY(cpb_backward(m->spatial_bias, grads->spatial_bias, S.dbias_s, g.hh, g.ww, 1, S.cpb_bwd_sc, st));
 
   // ---------------------------------------------------------------- temporal stack, rows (b h w t)
   PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 1);
   PHK_LAUNCH_CHECK();
-  PHK_TRY(stack_backward(ct, svT.get(), xfT, G.dtmp, &dx, &dx_alt, G));
+  PHK_TRY(stack_backward(ct, svT.get(), xfT, G.dtmp, &dx, &dx_alt, G, prog));
 
   // ---------------------------------------------------------------- d tokens / project_out
   if (!ids && !dtokens && !dcodes_out) return 0;
@@ -2319,6 +2336,7 @@ int decode_backward_phase(const phk_cvivit_dec_t* m, const phk_cvivit_dec_t* gra
     PHK_LAUNCH_CHECK();
     PHK_TRY(wgrad(dcodes, signs, (float*)grads->vq_out_w, R, D, bits, st));  // [dim, bits]: not worth a tensor-core launch
     PHK_TRY(colsum(dcodes, R, D, D, (float*)grads->vq_out_b, st));
+    PHK_TRY(progress_next(prog, st));  // project_out final
   }
   return 0;
 }
@@ -2349,10 +2367,11 @@ int64_t enc_phase_floats(const phk_cvivit_t* m, const CvGeom& g, bool dvideo) {
 // is dead on return), then differentiates norm_out(temporal) from dout ((b t h w) rows; it may be one of S's gradient
 // streams).  z (NULL: not formed): receives the recomputed output, (b t h w) rows.  On return *dx0 = d x0 in (b t h w)
 // rows, in a gradient stream of S; dtokens (NULL: not wanted) receives a copy (written, not added).  cpb_now: finish the
-// position-bias MLP's gradient here; otherwise S.dbias_s is left to the caller.
+// position-bias MLP's gradient here; otherwise S.dbias_s is left to the caller.  prog (NULL: none): one event per
+// temporal then spatial layer.
 int encode_backward_phase(const phk_cvivit_t* m, const phk_cvivit_t* grads, const float* x0, const CvGeom& g,
                           const float* dout, float* z, float* dtokens, const float** dx0, const CvShared& S, Arena ar,
-                          bool cpb_now, int prec, phk_stream_t s) {
+                          bool cpb_now, int prec, phk_stream_t s, Progress* prog) {
   const phk_transformer_t* ES = &m->spatial;
   const phk_transformer_t* ET = &m->temporal;
   const int B = g.B, Tp = g.Tp, hw = g.hw, D = g.D;
@@ -2388,10 +2407,10 @@ int encode_backward_phase(const phk_cvivit_t* m, const phk_cvivit_t* grads, cons
   float* dx_alt = S.dx_alt;
   PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dout, G.dtmp, B, Tp, hw, D, 1);
   PHK_LAUNCH_CHECK();
-  PHK_TRY(stack_backward(ct, svT.get(), xfT, G.dtmp, &dx, &dx_alt, G));
+  PHK_TRY(stack_backward(ct, svT.get(), xfT, G.dtmp, &dx, &dx_alt, G, prog));
   PHK_KERNEL_LAUNCH(permute_bts_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dx, G.dtmp, B, Tp, hw, D, 0);
   PHK_LAUNCH_CHECK();
-  PHK_TRY(stack_backward(cs, svS.get(), xfS, G.dtmp, &dx, &dx_alt, G));
+  PHK_TRY(stack_backward(cs, svS.get(), xfS, G.dtmp, &dx, &dx_alt, G, prog));
   if (dtokens) PHK_CUDA(cudaMemcpyAsync(dtokens, dx, R * D * 4, cudaMemcpyDeviceToDevice, st));
   if (dx0) *dx0 = dx;
   if (cpb_now) PHK_TRY(cpb_backward(m->spatial_bias, grads->spatial_bias, S.dbias_s, g.hh, g.ww, 1, S.cpb_bwd_sc, st));
@@ -2441,7 +2460,7 @@ extern "C" int phk_cvivit_decode_backward(const phk_cvivit_dec_t* m, const phk_c
   Arena ar{(char*)workspace, workspace_bytes, 0};
   CvShared S;
   PHK_TRY(cv_shared_init(ar, g, m->spatial_bias, prec, s, S));
-  return decode_backward_phase(m, grads, ids, tokens, g, dvideo, dtokens, nullptr, S, ar, true, prec, s);
+  return decode_backward_phase(m, grads, ids, tokens, g, dvideo, dtokens, nullptr, S, ar, true, prec, s, nullptr);
 }
 
 // See include/phk.h.
@@ -2475,6 +2494,15 @@ extern "C" int64_t phk_cvivit_backward_workspace_bytes(const phk_cvivit_t* enc, 
   return cv_shared_bytes(g, dec->spatial_bias, prec) + (own + imax(dec_phase_floats(dec, g), enc_phase_floats(enc, g, true))) * 4;
 }
 
+// See include/phk.h: to_pixels*, the decoder's spatial and temporal layers, project_out, the encoder's temporal and
+// spatial layers, project_in, to_patch_emb*, the position-bias MLP.
+extern "C" int32_t phk_cvivit_backward_progress_groups(const phk_cvivit_t* enc, const phk_cvivit_dec_t* dec) {
+  if (!enc || !dec || enc->spatial.depth <= 0 || enc->temporal.depth <= 0 || dec->spatial.depth <= 0 ||
+      dec->temporal.depth <= 0)
+    return -1;
+  return 1 + dec->spatial.depth + dec->temporal.depth + 1 + enc->temporal.depth + enc->spatial.depth + 1 + 1 + 1;
+}
+
 // See include/phk.h.  Order: d recon; the decoder phase (as phk_cvivit_decode_backward, from the forward's ids); LFQ
 // (project_out's dgrad, the straight-through d x = d q, project_in); the encoder phase (recomputed with saved activations
 // in the space the decoder phase used, then differentiated down to the patch rows and d video); the position-bias MLP
@@ -2484,6 +2512,8 @@ extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* 
                                    const int64_t* ids, const uint8_t* frame_mask, int32_t B, int32_t F, const float* dloss,
                                    const float* drecon, float* dvideo, int32_t straight_through, void* workspace,
                                    int64_t workspace_bytes, int32_t prec, phk_stream_t s) {
+  Progress prog{g_progress_events, g_progress_count, 0};  // one-shot: consumed by this call, even one that fails
+  g_progress_events = nullptr; g_progress_count = 0;
   PHK_REQUIRE(enc && enc_grads && dec && dec_grads && video && recon && ids && dloss && workspace, PHK_E_ARG,
               "cvivit_backward: null pointer");
   PHK_REQUIRE(prec == PHK_PREC_F32 || prec == PHK_PREC_BF16, PHK_E_ARG, "cvivit_backward: unknown precision mode");
@@ -2532,7 +2562,7 @@ extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* 
 
   // ---------------------------------------------------------------- decoder phase, from the forward's ids
   const float* dcodes = nullptr;
-  PHK_TRY(decode_backward_phase(dec, dec_grads, ids, nullptr, g, drec, nullptr, &dcodes, S, ar, false, prec, s));
+  PHK_TRY(decode_backward_phase(dec, dec_grads, ids, nullptr, g, drec, nullptr, &dcodes, S, ar, false, prec, s, &prog));
 
   // ---------------------------------------------------------------- LFQ: d q = d z_dec W_out; straight through, d x = d q
   if (straight_through) {
@@ -2567,9 +2597,10 @@ extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* 
     const LayerGrads& G = S.G;
     PHK_TRY(dgrad(dq, enc->vq_w, S.dx, R, bits, D, 0, st));  // d(encoder output), (b t h w)
     const float* dx = nullptr;
-    PHK_TRY(encode_backward_phase(enc, enc_grads, x0, g, S.dx, z, nullptr, &dx, S, ea, false, prec, s));
+    PHK_TRY(encode_backward_phase(enc, enc_grads, x0, g, S.dx, z, nullptr, &dx, S, ea, false, prec, s, &prog));
     PHK_TRY(wgrad(dq, z, (float*)enc_grads->vq_w, R, bits, D, st));
     PHK_TRY(colsum(dq, R, bits, bits, (float*)enc_grads->vq_b, st));
+    PHK_TRY(progress_next(&prog, st));  // project_in final
 
     // ---------------------------------------------------------------- to_patch_emb_first_frame / to_patch_emb
     float* dE1 = ea.f(rows1 * D); float* dE2 = ea.f(r2 * D);
@@ -2601,10 +2632,15 @@ extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* 
         PHK_LAUNCH_CHECK();
       }
     }
+    PHK_TRY(progress_next(&prog, st));  // to_patch_emb_first_frame / to_patch_emb final
+  } else {
+    // eval mode: the encoder's groups are empty, their events are recorded all the same (the count depends on the tables only)
+    for (int k = 0; k < ET->depth + ES->depth + 2; ++k) PHK_TRY(progress_next(&prog, st));
   }
 
   // ---------------------------------------------------------------- position-bias MLP, once over both spatial stacks
-  return cpb_backward(dec->spatial_bias, dec_grads->spatial_bias, S.dbias_s, g.hh, g.ww, 1, S.cpb_bwd_sc, st);
+  PHK_TRY(cpb_backward(dec->spatial_bias, dec_grads->spatial_bias, S.dbias_s, g.hh, g.ww, 1, S.cpb_bwd_sc, st));
+  return progress_next(&prog, st);  // the position-bias MLP final: every gradient is
 }
 
 extern "C" int64_t phk_cvivit_encode_backward_workspace_bytes(const phk_cvivit_t* m, int32_t B, int32_t Tp, int32_t prec) {
@@ -2641,5 +2677,5 @@ extern "C" int phk_cvivit_encode_backward(const phk_cvivit_t* m, const phk_cvivi
   Arena ar{(char*)workspace, workspace_bytes, 0};
   CvShared S;
   PHK_TRY(cv_shared_init(ar, g, m->spatial_bias, prec, s, S));
-  return encode_backward_phase(m, grads, tokens, g, dout, nullptr, dtokens, nullptr, S, ar, true, prec, s);
+  return encode_backward_phase(m, grads, tokens, g, dout, nullptr, dtokens, nullptr, S, ar, true, prec, s, nullptr);
 }

@@ -18,6 +18,7 @@ import torch
 from torch import nn
 
 from . import _lib as L
+from . import sharding
 from .modules import (ContinuousPositionBias, GradKeep, Keep, Transformer, Workspace, _NoParams, cpb_grad_table,
                       cpb_table, transformer_grad_table, transformer_table, weights_signature)
 
@@ -116,6 +117,8 @@ class CViViT(nn.Module):
         # built here: the tokenizer constructs with the reference's defaults, encodes and decodes, and loads the
         # reference's checkpoints (load_state_dict drops their `discr.*` entries); forward() raises for the loss paths.
         self.use_vgg_and_gan = use_vgg_and_gan
+        # data parallel without a DDP wrapper: see the docstring of forward()
+        self.sync_gradients = False
         self.precision = L.default_precision()
         self._tables = None
         self._sig = None
@@ -171,8 +174,11 @@ class CViViT(nn.Module):
         saved = (self._tables, self._sig, self._dec_tables, self._dec_sig, self._ws, self._bias_cache, self._ids_buf)
         self._tables, self._sig, self._dec_tables, self._dec_sig = None, None, None, None  # ctypes tables are not copyable
         self._ws, self._bias_cache, self._ids_buf = Workspace(), {}, {}
+        overlap = self.__dict__.pop("_overlap_cache", None)  # CUDA events and a stream (sharding.overlap_plan)
         c = copy.deepcopy(self)
         self._tables, self._sig, self._dec_tables, self._dec_sig, self._ws, self._bias_cache, self._ids_buf = saved
+        if overlap is not None:
+            self._overlap_cache = overlap
         return c.eval().to(device)
 
     def load_state_dict(self, state_dict, *args, **kwargs):
@@ -355,6 +361,19 @@ class CViViT(nn.Module):
 
     def forward(self, video, mask=None, return_recons=False, return_recons_only=False, return_discr_loss=False,
                 apply_grad_penalty=True, return_only_codebook_ids=False):
+        """The reference's ``CViViT.forward``.  With ``use_vgg_and_gan=False`` and LFQ, ``loss = forward(video)`` is the
+        reconstruction loss and ``loss.backward()`` fills the gradients (phk_cvivit_backward).
+
+        Data parallel: with ``self.sync_gradients = True`` (read when the loss is built) and a ``torch.distributed``
+        process group of more than one rank, ``loss.backward()`` hands every parameter the mean over the ranks of each
+        rank's gradient, as DistributedDataParallel does: each rank's loss stays the mean over its own shard (and its own
+        frame mask), ``video.grad`` stays the rank's own.  Under NCCL the all-reduce runs slice by slice on a side stream
+        while the backward still computes the slices it has not finished; other backends reduce the whole gradient bucket
+        after it.  The mean is linear, so averaging every micro-step of a gradient accumulation gives what DDP's
+        ``no_sync`` followed by one synced step gives.  Every rank has to call ``backward()`` on a batch of at least one
+        video each time: the all-reduce is a collective, and a rank that skips it leaves the others waiting.
+        The default is False, unlike ``Phenaki.sync_gradients`` (True): a single process and a module wrapped in torch
+        DDP behave as before, and DDP's own reduction is not doubled."""
         assert video.ndim in {4, 5}
         is_image = video.ndim == 4
         if is_image:
@@ -389,6 +408,23 @@ class CViViT(nn.Module):
                 self.enc_temporal_transformer, self.vq.project_in]
         return [p for m in mods for p in m.parameters()]
 
+    def _recon_gradient_groups(self):
+        """The parameters of phk_cvivit_backward's gradient groups, in the order it finishes them (include/phk.h):
+        to_pixels*, the decoder's spatial then temporal layers top-down (norm_out with the top layer), project_out, the
+        encoder's temporal then spatial layers the same way, project_in, to_patch_emb*, the position-bias MLP."""
+        def stack(tf):
+            layers = [list(tf.layers[i].parameters()) for i in reversed(range(tf.depth))]
+            layers[0] = list(tf.norm_out.parameters()) + layers[0]
+            return layers
+
+        return ([[*self.to_pixels_first_frame.parameters(), *self.to_pixels.parameters()]]
+                + stack(self.dec_spatial_transformer) + stack(self.dec_temporal_transformer)
+                + [list(self.vq.project_out.parameters())]
+                + stack(self.enc_temporal_transformer) + stack(self.enc_spatial_transformer)
+                + [list(self.vq.project_in.parameters()),
+                   [*self.to_patch_emb_first_frame.parameters(), *self.to_patch_emb.parameters()],
+                   list(self.spatial_rel_pos_bias.parameters())])
+
     def _recon_loss(self, video, mask):
         """(loss, recon): the masked MSE of decode(encode(video)) against video, differentiable through
         ``_ReconLossFn`` when grad mode is on and ``video`` or a parameter requires grad."""
@@ -412,7 +448,7 @@ class CViViT(nn.Module):
             mask = mask.to(torch.uint8).contiguous()
         params = self._encoder_params() + self._decoder_params(True)
         spec = dict(net=self, mask=mask, params=params, n_enc=len(self._encoder_params()), precision=self.precision,
-                    straight_through=self.vq.training, sig=weights_signature(self))
+                    straight_through=self.vq.training, sig=weights_signature(self), sync=bool(self.sync_gradients))
         if torch.is_grad_enabled() and (video.requires_grad or any(p.requires_grad for p in params)):
             return _ReconLossFn.apply(spec, video, *params)
         return self._recon_forward(video.detach(), mask)[1:]
@@ -469,7 +505,8 @@ class CViViT(nn.Module):
         straight = spec["straight_through"]
         with torch.cuda.device(dev):
             enc, dec = self._table(), self._dec_table()
-            gk = GradKeep(spec["params"])
+            groups = self._recon_gradient_groups()
+            gk = GradKeep(p for group in groups for p in group)  # each group one contiguous span of the bucket
             egt = self._enc_grad_table(gk, True)
             dgt = self._dec_grad_table(gk, True)
             dloss = (torch.zeros((), dtype=torch.float32, device=dev) if dloss is None
@@ -480,11 +517,24 @@ class CViViT(nn.Module):
             if nbytes < 0:
                 raise L.PhkError("phk_cvivit_backward_workspace_bytes: unsupported configuration")
             ws = self._ws.get(nbytes, dev)
+            plan = None
+            if spec["sync"]:
+                n_groups = lib.phk_cvivit_backward_progress_groups(C.byref(enc), C.byref(dec))
+                assert n_groups == len(groups), f"phk_cvivit_backward records {n_groups} events, not {len(groups)}"
+                plan = sharding.overlap_plan(self, gk.flat, n_groups, dev)
+            if plan is not None:  # the call records these events as gradient groups become final
+                spans = sharding.bucket_spans(gk.flat, gk.views, groups)
+                L.check(lib.phk_train_set_progress_events(plan["handles"], len(plan["events"])),
+                        "phk_train_set_progress_events")
             L.check(lib.phk_cvivit_backward(C.byref(enc), C.byref(egt), C.byref(dec), C.byref(dgt), L.ptr(video),
                                             L.ptr(recon), L.ptr(ids), L.ptr(spec["mask"]), b, f, L.ptr(dloss),
                                             L.ptr(drecon), L.ptr(dvideo), int(straight), L.ptr(ws), ws.numel(), prec,
                                             L.stream_ptr()),
                     "phk_cvivit_backward")
+            if plan is not None:
+                torch.cuda.current_stream().wait_event(sharding.launch_overlapped_all_reduce(gk.flat, plan, spans))
+            elif spec["sync"]:
+                sharding.all_reduce_mean_(gk.flat)
         grads = [gk.grad_of(p) for p in spec["params"]]
         if not straight:  # eval mode: q is a constant, nothing reaches the encoder
             grads[:spec["n_enc"]] = [None] * spec["n_enc"]

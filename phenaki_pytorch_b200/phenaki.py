@@ -310,7 +310,7 @@ class _TokenTransformer(nn.Module):
                                                L.stream_ptr(), dropout),
                     "phk_maskgit_train_step")
             if plan is not None:
-                self._launch_overlapped_all_reduce(gk, plan)
+                gk.reduced = sharding.launch_overlapped_all_reduce(gk.flat, plan, plan["groups"])
         return loss, gk, logits
 
     def _gradient_groups(self, gk, owner):
@@ -319,70 +319,25 @@ class _TokenTransformer(nn.Module):
         not be adjacent in the bucket (token_emb / pos_emb open it, the position-bias MLP sits behind the layers): adjacent
         spans are merged, every element of the bucket belongs to exactly one span."""
         depth = self.transformer.depth
-        base, esz = gk.flat.data_ptr(), gk.flat.element_size()
-        groups = [[] for _ in range(depth + 2)]  # spans [lo, hi) in elements, by completion index
+        groups = [[] for _ in range(depth + 2)]  # parameters by completion index
         for name, p in owner.named_parameters():
-            lo = (gk.views[p].data_ptr() - base) // esz
-            hi = lo + (p.numel() + 63) // 64 * 64
             idx = depth + 1  # embeddings, position-bias MLP: final at the very end
             if "transformer.layers." in name:
                 idx = 1 + (depth - 1 - int(name.split("transformer.layers.")[1].split(".")[0]))
             elif "norm_out" in name or "to_logits" in name or "to_pred" in name:
                 idx = 0
-            if p.numel():
-                groups[idx].append((lo, hi))
-        for i, spans in enumerate(groups):  # a group's parameters need not be adjacent in the bucket: merge what is
-            merged = []
-            for lo, hi in sorted(spans):
-                if merged and lo <= merged[-1][1]:
-                    merged[-1][1] = max(merged[-1][1], hi)
-                else:
-                    merged.append([lo, hi])
-            groups[i] = merged
-        flat = sorted(sp for spans in groups for sp in spans)
-        if any(a[1] > b[0] for a, b in zip(flat, flat[1:])):  # (padded spans of different groups overlap: no slicing)
-            return None
-        return groups
+            groups[idx].append(p)
+        return sharding.bucket_spans(gk.flat, gk.views, groups)
 
     def _overlap_plan(self, gk, owner, dev):
         """Data parallel, NCCL: slices of the flat gradient bucket in the order the backward finishes them (head +
         norm_out, layers depth-1 .. 0, embeddings + position-bias MLP) and one CUDA event per slice for
         phk_train_set_progress_events.  None when there is nothing to overlap (single process, non-NCCL backend)."""
-        import torch.distributed as dist
-        if not (dist.is_available() and dist.is_initialized() and dist.get_world_size() > 1 and gk.flat.is_cuda
-                and dist.get_backend() == "nccl"):
+        plan = sharding.overlap_plan(self, gk.flat, self.transformer.depth + 2, dev)
+        if plan is None:
             return None
         groups = self._gradient_groups(gk, owner)
-        if groups is None:
-            return None
-        depth = self.transformer.depth
-        cache = self.__dict__.setdefault("_overlap_cache", {})
-        key = (dev, depth)
-        if key not in cache:
-            events = [torch.cuda.Event() for _ in range(depth + 2)]
-            for e in events:
-                e.record()  # creates the CUDA event behind the (lazily initialised) torch object
-            handles = (C.c_void_p * len(events))(*[e.cuda_event for e in events])
-            cache[key] = dict(events=events, handles=handles, stream=torch.cuda.Stream(device=dev))
-        return dict(cache[key], groups=groups)
-
-    def _launch_overlapped_all_reduce(self, gk, plan):
-        """One all-reduce (mean) per finished slice on a side stream, each waiting only for its own event: the
-        collective of the head / upper layers runs while the layers below are still in their backward kernels."""
-        import torch.distributed as dist
-        side, world = plan["stream"], dist.get_world_size()
-        gk.flat.record_stream(side)
-        for ev, spans in zip(plan["events"], plan["groups"]):
-            if not spans:
-                continue
-            side.wait_event(ev)
-            with torch.cuda.stream(side):
-                for lo, hi in spans:
-                    part = gk.flat[lo:hi]
-                    dist.all_reduce(part, op=dist.ReduceOp.SUM)
-                    part.div_(world)
-        gk.reduced = torch.cuda.Event()
-        gk.reduced.record(side)
+        return None if groups is None else dict(plan, groups=groups)
 
     def _differentiable(self, run, owner, ids, patch_shape, *, context, text_mask, video_mask, cond_scale, head_kind,
                         head=None):

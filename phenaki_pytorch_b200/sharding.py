@@ -8,6 +8,8 @@ Training (SURVEY 8e / 8f-2) adds the one collective the reference implies (DDP's
 PhenakiTrainer): the training step writes every gradient of a network into ONE flat fp32 bucket
 (modules.GradKeep.flat), so the exchange is a single all-reduce over that buffer -- no bucket packing copy.
 """
+import ctypes
+
 import torch
 import torch.distributed as dist
 
@@ -81,3 +83,73 @@ def all_reduce_mean_(flat, group=None):
     dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=group)
     flat.div_(w)
     return flat
+
+
+# Test-only: take the overlapped path below in a one-rank NCCL group too, so that a single GPU exercises it (the mean
+# over one rank leaves every gradient bit for bit as it was).
+OVERLAP_AT_WORLD_SIZE_1 = False
+
+
+def bucket_spans(flat, views, groups):
+    """Slices of a flat gradient bucket (modules.GradKeep: ``views`` maps a parameter to its view of ``flat``) for
+    groups of parameters: per group, the [lo, hi) element spans its parameters' padded views cover, adjacent spans merged.
+    A group's parameters need not be adjacent in the bucket; zero-element parameters have no address and are skipped.
+    None when spans of different groups overlap (then the bucket cannot be sliced by group)."""
+    base, esz = flat.data_ptr(), flat.element_size()
+    out = []
+    for params in groups:
+        spans = []
+        for p in params:
+            if p.numel():
+                lo = (views[p].data_ptr() - base) // esz
+                spans.append((lo, lo + (p.numel() + 63) // 64 * 64))
+        merged = []
+        for lo, hi in sorted(spans):
+            if merged and lo <= merged[-1][1]:
+                merged[-1][1] = max(merged[-1][1], hi)
+            else:
+                merged.append([lo, hi])
+        out.append(merged)
+    flat_spans = sorted(sp for spans in out for sp in spans)
+    if any(a[1] > b[0] for a, b in zip(flat_spans, flat_spans[1:])):
+        return None
+    return out
+
+
+def overlap_plan(owner, flat, n_events, dev):
+    """Data parallel over NCCL (world size > 1, or OVERLAP_AT_WORLD_SIZE_1): dict(events, handles, stream) -- one CUDA
+    event per gradient group for phk_train_set_progress_events and the side stream the slices are reduced on, created
+    once per (device, n_events) and kept on ``owner``.  None when there is nothing to overlap (single process, non-NCCL
+    backend, CPU bucket)."""
+    if not (dist.is_available() and dist.is_initialized() and flat.is_cuda and dist.get_backend() == "nccl"
+            and (dist.get_world_size() > 1 or OVERLAP_AT_WORLD_SIZE_1)):
+        return None
+    cache = owner.__dict__.setdefault("_overlap_cache", {})
+    key = (dev, n_events)
+    if key not in cache:
+        events = [torch.cuda.Event() for _ in range(n_events)]
+        for e in events:
+            e.record()  # creates the CUDA event behind the (lazily initialised) torch object
+        handles = (ctypes.c_void_p * n_events)(*[e.cuda_event for e in events])
+        cache[key] = dict(events=events, handles=handles, stream=torch.cuda.Stream(device=dev))
+    return cache[key]
+
+
+def launch_overlapped_all_reduce(flat, plan, groups):
+    """One all-reduce (mean) per slice of ``flat`` on the plan's side stream, each group's slices waiting only for that
+    group's event (``groups``: bucket_spans, in event order): the collective of the groups the backward finished first
+    runs while it is still computing the rest.  Returns the event recorded on the side stream after the last slice."""
+    side, w = plan["stream"], dist.get_world_size()
+    flat.record_stream(side)
+    for ev, spans in zip(plan["events"], groups):
+        if not spans:
+            continue
+        side.wait_event(ev)
+        with torch.cuda.stream(side):
+            for lo, hi in spans:
+                part = flat[lo:hi]
+                dist.all_reduce(part, op=dist.ReduceOp.SUM)
+                part.div_(w)
+    done = torch.cuda.Event()
+    done.record(side)
+    return done
