@@ -676,7 +676,12 @@ int phk_debug_step_graph(int32_t on);
  *   given); the FF hidden [b*n, inner].  e is the row-major index in that shape.  The first site's base is offset, the
  *   next base is base + ceil(count / 4).  Every site takes its counters whatever the probabilities, so one step uses
  *   phk_maskgit_train_dropout_counters(m, b, n, L) counters from offset on (L = 0 without a context; -1 on bad
- *   arguments).  The workspace is the same with and without dropout. */
+ *   arguments).  The workspace is the same with and without dropout.
+ * d_context: NULL, or fp32 [b, L, dim_context] zero-filled by the caller, not aliasing `context` (PHK_E_ARG if it does;
+ *   NULL when `context` is NULL).  d(loss_scale * loss)/d(context) is ACCUMULATED into it over every cross-attention
+ *   layer, for the dropout masks the step drew.  It is the caller's own activation gradient: it is not part of the
+ *   gradient table and the progress events below say nothing about it (it is final when the call's work is).  The call
+ *   issues the same launches, in the same order, with the same workspace, whether d_context is NULL or not. */
 typedef struct phk_dropout {
   float attn_p, ff_p;
   uint64_t seed, offset;
@@ -689,7 +694,7 @@ int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_t* grads, c
                            int32_t pt, int32_t ph, int32_t pw, const float* context, int32_t L,
                            const uint8_t* text_mask, const uint8_t* video_mask, float loss_scale, float* loss_out,
                            float* logits_out, void* workspace, int64_t workspace_bytes, int32_t prec, phk_stream_t s,
-                           const phk_dropout_t* dropout);
+                           const phk_dropout_t* dropout, float* d_context);
 /* Data-parallel overlap: `events` (cudaEvent_t handles, count >= depth + 2) are recorded by the NEXT phk_maskgit_train_step
  * call of the calling thread, on its stream, as gradient groups become final: events[0] head + norm_out, events[1 + k]
  * transformer layer depth-1-k, events[depth + 1] embeddings + position-bias MLP (= all).  If the next such call is

@@ -179,7 +179,7 @@ PROTOTYPES = {
     "phk_maskgit_train_workspace_bytes": [C.POINTER(MaskgitT), i32, i32, i32, i32, i32],
     "phk_maskgit_train_dropout_counters": [C.POINTER(MaskgitT), i32, i32, i32],
     "phk_maskgit_train_step": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), vp, vp, vp, vp, i32, i32, i32, i32, i32, vp, i32,
-                               vp, vp, f32, vp, vp, vp, i64, i32, vp, C.POINTER(DropoutT)],
+                               vp, vp, f32, vp, vp, vp, i64, i32, vp, C.POINTER(DropoutT), vp],
     "phk_maskgit_backward_workspace_bytes": [C.POINTER(MaskgitT), i32, i32, i32, i32, i32, i32],
     "phk_maskgit_backward": [C.POINTER(MaskgitT), C.POINTER(MaskgitT), vp, i32, i32, i32, i32, i32, vp, i32, vp, vp, i32,
                              f32, i32, vp, vp, vp, i64, i32, vp],

@@ -325,7 +325,7 @@ static int check_transformer(const phk_transformer_t* T) {
 
 using namespace phk;
 
-extern "C" int phk_version(void) { return 108; }
+extern "C" int phk_version(void) { return 109; }
 extern "C" const char* phk_last_error(void) { return g_err; }
 extern "C" int64_t phk_launch_count(void) { return g_launches.load(); }
 

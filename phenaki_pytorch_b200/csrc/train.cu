@@ -1626,6 +1626,14 @@ int64_t step_workspace_bytes(const phk_maskgit_t* m, int32_t b, int32_t n, int32
   return bytes;
 }
 
+// widest dim_context of the cross-attention layers (0 without any)
+int64_t context_width(const phk_transformer_t* T) {
+  int64_t dc = 0;
+  for (int l = 0; l < T->depth; ++l)
+    if (T->layers[l].has_cross && T->layers[l].cross_attn.dim_context > dc) dc = T->layers[l].cross_attn.dim_context;
+  return dc;
+}
+
 }  // namespace
 }  // namespace phk
 
@@ -1650,7 +1658,7 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
                                       int32_t n, int32_t pt, int32_t ph, int32_t pw, const float* context, int32_t L,
                                       const uint8_t* text_mask, const uint8_t* video_mask, float loss_scale,
                                       float* loss_out, float* logits_out, void* workspace, int64_t workspace_bytes,
-                                      int32_t prec, phk_stream_t s, const phk_dropout_t* dropout) {
+                                      int32_t prec, phk_stream_t s, const phk_dropout_t* dropout, float* d_context) {
   PHK_REQUIRE(m && grads && ids_in && loss_out && workspace, PHK_E_ARG, "maskgit_train_step: null pointer");
   PHK_REQUIRE(b > 0 && n > 0 && (int64_t)pt * ph * pw == n, PHK_E_SHAPE, "video patch shape must cover the token sequence");
   PHK_REQUIRE(n <= m->max_seq_len, PHK_E_SHAPE,
@@ -1663,6 +1671,8 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   PHK_REQUIRE(bce || !m->is_critic, PHK_E_ARG, "maskgit_train_step: a TokenCritic table needs labels");
   PHK_REQUIRE(!(bce && logits_out), PHK_E_ARG, "maskgit_train_step: the critic head has no logits to hand back");
   PHK_REQUIRE(!context || (text_mask && L > 0), PHK_E_ARG, "maskgit_train_step: context without text mask / length");
+  PHK_REQUIRE(!d_context || context, PHK_E_ARG, "maskgit_train_step: d_context without a context");
+  PHK_REQUIRE(!d_context || (const float*)d_context != context, PHK_E_ARG, "maskgit_train_step: d_context aliases context");
   PHK_REQUIRE(prec == PHK_PREC_F32 || prec == PHK_PREC_BF16, PHK_E_ARG, "maskgit_train_step: unknown precision mode");
   PHK_REQUIRE(workspace_bytes >= phk_maskgit_train_workspace_bytes(m, b, n, L, bce ? 1 : 0, prec), PHK_E_WORKSPACE,
               "maskgit_train_step: workspace too small");
@@ -1671,6 +1681,12 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   PHK_REQUIRE(T->layers && GT->layers && T->depth > 0 && GT->depth == T->depth && !T->causal, PHK_E_ARG,
               "maskgit_train_step: transformer table / gradient table mismatch");
   PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "maskgit_train_step: dim must be a multiple of 4");
+  if (d_context) {  // one [b, L, dim_context] buffer takes the context gradient of every cross-attention layer
+    const int64_t dc = context_width(T);
+    for (int l = 0; l < T->depth; ++l)
+      PHK_REQUIRE(!T->layers[l].has_cross || T->layers[l].cross_attn.dim_context == dc, PHK_E_UNSUPPORTED,
+                  "maskgit_train_step: cross-attention layers of different context widths");
+  }
   PHK_REQUIRE(!dropout || (dropout->attn_p >= 0.f && dropout->attn_p <= 1.f && dropout->ff_p >= 0.f && dropout->ff_p <= 1.f),
               PHK_E_ARG, "maskgit_train_step: dropout probabilities must lie in [0, 1]");
   void** prog = g_progress_events;  // one-shot: consumed by this call
@@ -1726,7 +1742,8 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   PHK_LAUNCH_CHECK();
 
   // ---------------------------------------------------------------- backward through the transformer
-  return step_backward(S, nullptr, prog, nprog);
+  // (d_context: the context_norm backward each cross-attention layer runs for its gamma gradient also accumulates dx)
+  return step_backward(S, d_context, prog, nprog);
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1763,13 +1780,6 @@ __global__ void add_halves_kernel(const float* __restrict__ a, float* __restrict
 // pair inputs of the CFG recompute: ids, video mask and context twice, the text mask then zeros
 int64_t pair_input_floats(int64_t R, int64_t CR, int64_t dc) {
   return 2 * R * 2 + (2 * R + 3) / 4 + (2 * CR + 3) / 4 + 2 * CR * dc + 4 * 64;
-}
-
-int64_t context_width(const phk_transformer_t* T) {
-  int64_t dc = 0;
-  for (int l = 0; l < T->depth; ++l)
-    if (T->layers[l].has_cross && T->layers[l].cross_attn.dim_context > dc) dc = T->layers[l].cross_attn.dim_context;
-  return dc;
 }
 
 }  // namespace

@@ -209,10 +209,11 @@ class _TokenTransformer(nn.Module):
         if hit is not None and not hit[1].busy and hit[2] == [id(p) for p in (owner if owner is not None else self).parameters()]:
             hit[1].flat.zero_()
             hit[1].reduced = None
+            hit[1].d_context = None
             hit[1].busy = True
             return hit[0], hit[1]
         gk = GradKeep((owner if owner is not None else self).parameters())
-        gk.busy, gk.reduced = True, None
+        gk.busy, gk.reduced, gk.d_context = True, None, None
         t = L.MaskgitT()
         tf = self.transformer
         t.dim, t.heads, t.dim_head = tf.dim, tf.heads, tf.dim_head
@@ -238,9 +239,11 @@ class _TokenTransformer(nn.Module):
                    overlap_all_reduce=False):
         """One forward + loss + backward in libphk (phk_maskgit_train_step; ``self.precision`` selects fp32 FFMA or
         wgmma bf16 products, everything else is fp32 in both modes): returns (loss 0-d tensor,
-        GradKeep with d(loss_scale * loss)/d(parameter), logits or None).  ``labels`` given: Linear(dim, 1) head + BCE
-        with logits (TokenCritic; or ``head`` = SelfCritic.to_pred on this MaskGit, gradients laid out for
-        ``owner.parameters()``); otherwise masked cross entropy against ``targets`` at ``token_mask``.
+        GradKeep with d(loss_scale * loss)/d(parameter), logits or None).  When ``context`` requires grad and the network
+        has cross-attention, ``GradKeep.d_context`` is a new fp32 tensor of the context's shape holding
+        d(loss_scale * loss)/d(context); otherwise it is None and the step computes no context gradient.
+        ``labels`` given: Linear(dim, 1) head + BCE with logits (TokenCritic; or ``head`` = SelfCritic.to_pred on this
+        MaskGit, gradients laid out for ``owner.parameters()``); otherwise masked cross entropy against ``targets`` at ``token_mask``.
         In training mode (``self.training``) the transformer's ``attn_dropout`` / ``ff_dropout`` apply as the
         reference's nn.Dropout does; the masks come from fresh counters of the device's noise generator (include/phk.h,
         phk_dropout_t), so every call draws new masks and ``torch.manual_seed`` repeats them."""
@@ -285,6 +288,9 @@ class _TokenTransformer(nn.Module):
                 targets = L.require_cuda(targets.reshape(b, n), "target ids", torch.int64)
                 token_mask = L.require_cuda(token_mask.reshape(b, n).to(torch.uint8), "token mask")
             gtable, gk = self._grad_table(has_cross, owner=owner, head=head)
+            want_context_grad = has_cross and torch.is_grad_enabled() and context.requires_grad
+            d_context = torch.zeros_like(context) if want_context_grad else None
+            gk.d_context = d_context
             logits = None
             if keep_logits and not bce:
                 logits = torch.empty((b, n, table.num_tokens), dtype=torch.float32, device=dev)
@@ -307,7 +313,7 @@ class _TokenTransformer(nn.Module):
                                                L.ptr(token_mask), L.ptr(labels), b, n, pt, ph, pw, L.ptr(context),
                                                ctx_len, L.ptr(text_mask), L.ptr(video_mask), float(loss_scale),
                                                L.ptr(loss), L.ptr(logits), L.ptr(ws), ws.numel(), prec,
-                                               L.stream_ptr(), dropout),
+                                               L.stream_ptr(), dropout, L.ptr(d_context)),
                     "phk_maskgit_train_step")
             if plan is not None:
                 gk.reduced = sharding.launch_overlapped_all_reduce(gk.flat, plan, plan["groups"])
@@ -627,16 +633,21 @@ class SelfCritic(nn.Module):
 class _TrainStepFn(torch.autograd.Function):
     """Connects phk_maskgit_train_step to torch autograd: forward returns the loss that libphk computed, backward hands
     the gradients libphk computed in the same call to the parameters (scaled by the upstream gradient), so
-    ``loss.backward()`` followed by any torch optimizer works as with the reference."""
+    ``loss.backward()`` followed by any torch optimizer works as with the reference.  ``context``: the text embeddings
+    the step ran on (or None); their gradient is ``grad_keep.d_context``, the rank's own, never all-reduced."""
 
     @staticmethod
-    def forward(ctx, loss, grad_keep, sync, *params):
+    def forward(ctx, loss, grad_keep, sync, context, *params):
         ctx.keep, ctx.sync = grad_keep, sync
         ctx.grads = [grad_keep.grad_of(p) for p in params]
+        ctx.d_context = grad_keep.d_context
         return loss.clone()
 
     @staticmethod
     def backward(ctx, gout):
+        if ctx.needs_input_grad[3] and torch.is_grad_enabled():
+            raise RuntimeError("Phenaki.forward does not support create_graph=True with text embeddings that require grad: "
+                               "the training step's backward is hand-written CUDA and builds no graph of its own")
         if ctx.sync:  # data parallel: average the one flat gradient bucket over the ranks (DDP's all-reduce)
             reduced = getattr(ctx.keep, "reduced", None)
             if reduced is not None:  # already launched slice by slice on the side stream, overlapped with the backward
@@ -644,7 +655,8 @@ class _TrainStepFn(torch.autograd.Function):
             else:
                 sharding.all_reduce_mean_(ctx.keep.flat)
             ctx.sync = False
-        out = (None, None, None, *[None if g is None else g * gout for g in ctx.grads])  # copies: the bucket is free again
+        d_context = ctx.d_context * gout if ctx.needs_input_grad[3] and ctx.d_context is not None else None
+        out = (None, None, None, d_context, *[None if g is None else g * gout for g in ctx.grads])  # copies: the bucket is free again
         ctx.keep.busy = False
         return out
 
@@ -1021,7 +1033,10 @@ class Phenaki(nn.Module):
                 only_train_critic=False, draw_fn=None):
         """Training loss (phenaki_pytorch.py:562-687): masked-token cross entropy of MaskGit (+ TokenCritic BCE).
         The returned scalar is connected to the parameters through ``_TrainStepFn``: ``loss.backward()`` fills
-        ``p.grad`` with the gradients the hand-written backward kernels computed (phk_maskgit_train_step).
+        ``p.grad`` with the gradients the hand-written backward kernels computed (phk_maskgit_train_step), and
+        ``text_embeds.grad`` when the caller's ``text_embeds`` requires grad: MaskGit's cross entropy and, with a
+        cross-attention TokenCritic or a SelfCritic, the critic's BCE times ``critic_loss_weight`` (only the latter with
+        ``only_train_critic``, as in the reference).  Embeddings computed from ``texts`` carry no gradient.
         ``draw_fn(shape, tag)`` (tests) injects the draws 'rand_step' (b,), 'perm' (b, n) and 'gumbel' (b, n, V).
         ``maskgit.precision`` selects fp32 (parity) or bf16 tensor-core products.  Validated on the H100 against the
         reference's autograd loss and every parameter gradient (tests/test_gpu_train.py, both precision modes)."""
@@ -1077,7 +1092,7 @@ class Phenaki(nn.Module):
         else:
             ce, gk, logits = mg.train_step(masked_input, patch_shape, targets=ids, token_mask=mask_token_mask,
                                            keep_logits=need_critic, overlap_all_reduce=self.sync_gradients, **kw)
-            loss = _TrainStepFn.apply(ce, gk, self.sync_gradients, *mg.parameters())
+            loss = _TrainStepFn.apply(ce, gk, self.sync_gradients, text_embeds, *mg.parameters())
         if not need_critic:
             return loss
         # sample the predicted masked tokens (:646) and train the critic to tell which ones were changed (:650-675)
@@ -1100,7 +1115,7 @@ class Phenaki(nn.Module):
         # (a SelfCritic differentiates MaskGit a second time: autograd adds the two contributions to p.grad)
         bce, cgk, _ = self.critic.train_step(critic_input, patch_shape, labels=labels,
                                              overlap_all_reduce=self.sync_gradients, **ckw)
-        critic_loss = _TrainStepFn.apply(bce, cgk, self.sync_gradients, *self.critic.parameters())
+        critic_loss = _TrainStepFn.apply(bce, cgk, self.sync_gradients, ckw.get("context"), *self.critic.parameters())
         return critic_loss * weight if loss is None else loss + critic_loss * weight
 
 
