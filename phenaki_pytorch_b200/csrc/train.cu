@@ -19,6 +19,7 @@
 #include "phk_common.cuh"
 // the kernels of this file are ordinary stream-ordered launches (they do not use programmatic dependent launch)
 #define PHK_KERNEL_LAUNCH(kernel, grid, block, smem, st, ...) PHK_CUDA(launch_plain(kernel, grid, block, smem, st, __VA_ARGS__))
+#include <cstdio>
 #include <cstring>
 #include <memory>
 #include <new>
@@ -1634,6 +1635,42 @@ int64_t context_width(const phk_transformer_t* T) {
   return dc;
 }
 
+// set_error with the calling entry point's name in front ("entry: msg"), for the checks several entry points share
+void set_entry_error(const char* entry, const char* msg) {
+  char buf[256];
+  std::snprintf(buf, sizeof(buf), "%s: %s", entry, msg);
+  set_error(buf);
+}
+#define PHK_REQUIRE_IN(entry, cond, code, msg) \
+  do { if (!(cond)) { set_entry_error(entry, msg); return (code); } } while (0)
+
+// The argument and table checks of phk_maskgit_train_step and phk_maskgit_backward.  same_context_widths: every
+// cross-attention layer must take contexts of one width (one buffer of the context serves them all).
+int check_maskgit_call(const char* entry, const phk_maskgit_t* m, const phk_maskgit_t* grads, const int64_t* ids,
+                       const void* workspace, int32_t b, int32_t n, int32_t pt, int32_t ph, int32_t pw, const float* context,
+                       int32_t L, const uint8_t* text_mask, const float* d_context, int32_t prec, bool same_context_widths) {
+  PHK_REQUIRE_IN(entry, m && grads && ids && workspace, PHK_E_ARG, "null pointer");
+  PHK_REQUIRE_IN(entry, b > 0 && n > 0 && (int64_t)pt * ph * pw == n, PHK_E_SHAPE,
+                 "video patch shape must cover the token sequence");
+  PHK_REQUIRE_IN(entry, n <= m->max_seq_len, PHK_E_SHAPE,
+                 "the video token sequence length is greater than max_seq_len (phenaki_pytorch.py:196)");
+  PHK_REQUIRE_IN(entry, !context || (text_mask && L > 0), PHK_E_ARG, "context without text mask / length");
+  PHK_REQUIRE_IN(entry, !d_context || context, PHK_E_ARG, "d_context without a context");
+  PHK_REQUIRE_IN(entry, prec == PHK_PREC_F32 || prec == PHK_PREC_BF16, PHK_E_ARG, "unknown precision mode");
+  const phk_transformer_t* T = &m->transformer;
+  const phk_transformer_t* GT = &grads->transformer;
+  PHK_REQUIRE_IN(entry, T->layers && GT->layers && T->depth > 0 && GT->depth == T->depth && !T->causal, PHK_E_ARG,
+                 "transformer table / gradient table mismatch");
+  PHK_REQUIRE_IN(entry, m->dim % 4 == 0, PHK_E_UNSUPPORTED, "dim must be a multiple of 4");
+  if (same_context_widths) {
+    const int64_t dc = context_width(T);
+    for (int l = 0; l < T->depth; ++l)
+      PHK_REQUIRE_IN(entry, !T->layers[l].has_cross || T->layers[l].cross_attn.dim_context == dc, PHK_E_UNSUPPORTED,
+                     "cross-attention layers of different context widths");
+  }
+  return 0;
+}
+
 }  // namespace
 }  // namespace phk
 
@@ -1659,10 +1696,10 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
                                       const uint8_t* text_mask, const uint8_t* video_mask, float loss_scale,
                                       float* loss_out, float* logits_out, void* workspace, int64_t workspace_bytes,
                                       int32_t prec, phk_stream_t s, const phk_dropout_t* dropout, float* d_context) {
-  PHK_REQUIRE(m && grads && ids_in && loss_out && workspace, PHK_E_ARG, "maskgit_train_step: null pointer");
-  PHK_REQUIRE(b > 0 && n > 0 && (int64_t)pt * ph * pw == n, PHK_E_SHAPE, "video patch shape must cover the token sequence");
-  PHK_REQUIRE(n <= m->max_seq_len, PHK_E_SHAPE,
-              "the video token sequence length is greater than max_seq_len (phenaki_pytorch.py:196)");
+  PHK_REQUIRE(loss_out, PHK_E_ARG, "maskgit_train_step: null pointer");
+  // the context's gradient buffer serves every cross-attention layer
+  PHK_TRY(check_maskgit_call("maskgit_train_step", m, grads, ids_in, workspace, b, n, pt, ph, pw, context, L, text_mask,
+                             d_context, prec, d_context != nullptr));
   // head: labels given -> Linear(dim, 1) + BCE with logits (TokenCritic, or SelfCritic.to_pred on a MaskGit body,
   // phenaki_pytorch.py:307-336); otherwise to_logits + masked cross entropy
   const bool bce = labels != nullptr;
@@ -1670,23 +1707,9 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
               "maskgit_train_step: pass labels (critic head) or targets + token_mask (MaskGit head)");
   PHK_REQUIRE(bce || !m->is_critic, PHK_E_ARG, "maskgit_train_step: a TokenCritic table needs labels");
   PHK_REQUIRE(!(bce && logits_out), PHK_E_ARG, "maskgit_train_step: the critic head has no logits to hand back");
-  PHK_REQUIRE(!context || (text_mask && L > 0), PHK_E_ARG, "maskgit_train_step: context without text mask / length");
-  PHK_REQUIRE(!d_context || context, PHK_E_ARG, "maskgit_train_step: d_context without a context");
   PHK_REQUIRE(!d_context || (const float*)d_context != context, PHK_E_ARG, "maskgit_train_step: d_context aliases context");
-  PHK_REQUIRE(prec == PHK_PREC_F32 || prec == PHK_PREC_BF16, PHK_E_ARG, "maskgit_train_step: unknown precision mode");
   PHK_REQUIRE(workspace_bytes >= phk_maskgit_train_workspace_bytes(m, b, n, L, bce ? 1 : 0, prec), PHK_E_WORKSPACE,
               "maskgit_train_step: workspace too small");
-  const phk_transformer_t* T = &m->transformer;
-  const phk_transformer_t* GT = &grads->transformer;
-  PHK_REQUIRE(T->layers && GT->layers && T->depth > 0 && GT->depth == T->depth && !T->causal, PHK_E_ARG,
-              "maskgit_train_step: transformer table / gradient table mismatch");
-  PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "maskgit_train_step: dim must be a multiple of 4");
-  if (d_context) {  // one [b, L, dim_context] buffer takes the context gradient of every cross-attention layer
-    const int64_t dc = context_width(T);
-    for (int l = 0; l < T->depth; ++l)
-      PHK_REQUIRE(!T->layers[l].has_cross || T->layers[l].cross_attn.dim_context == dc, PHK_E_UNSUPPORTED,
-                  "maskgit_train_step: cross-attention layers of different context widths");
-  }
   PHK_REQUIRE(!dropout || (dropout->attn_p >= 0.f && dropout->attn_p <= 1.f && dropout->ff_p >= 0.f && dropout->ff_p <= 1.f),
               PHK_E_ARG, "maskgit_train_step: dropout probabilities must lie in [0, 1]");
   void** prog = g_progress_events;  // one-shot: consumed by this call
@@ -1803,28 +1826,17 @@ extern "C" int phk_maskgit_backward(const phk_maskgit_t* m, const phk_maskgit_t*
                                     const uint8_t* text_mask, const uint8_t* video_mask, int32_t cfg_pair,
                                     float cond_scale, int32_t head_kind, const float* upstream, float* d_context,
                                     void* workspace, int64_t workspace_bytes, int32_t prec, phk_stream_t s) {
-  PHK_REQUIRE(m && grads && ids && upstream && workspace, PHK_E_ARG, "maskgit_backward: null pointer");
-  PHK_REQUIRE(b > 0 && n > 0 && (int64_t)pt * ph * pw == n, PHK_E_SHAPE, "video patch shape must cover the token sequence");
-  PHK_REQUIRE(n <= m->max_seq_len, PHK_E_SHAPE,
-              "the video token sequence length is greater than max_seq_len (phenaki_pytorch.py:196)");
+  PHK_REQUIRE(upstream, PHK_E_ARG, "maskgit_backward: null pointer");
+  // the pair's copy of the context serves every cross-attention layer
+  PHK_TRY(check_maskgit_call("maskgit_backward", m, grads, ids, workspace, b, n, pt, ph, pw, context, L, text_mask,
+                             d_context, prec, context != nullptr));
   PHK_REQUIRE(head_kind == PHK_HEAD_LOGITS || head_kind == PHK_HEAD_EMBEDS || head_kind == PHK_HEAD_SCORE, PHK_E_ARG,
               "maskgit_backward: unknown head kind");
   PHK_REQUIRE(head_kind != PHK_HEAD_LOGITS || !m->is_critic, PHK_E_ARG, "maskgit_backward: a TokenCritic has no logits head");
-  PHK_REQUIRE(!context || (text_mask && L > 0), PHK_E_ARG, "maskgit_backward: context without text mask / length");
-  PHK_REQUIRE(!d_context || context, PHK_E_ARG, "maskgit_backward: d_context without a context");
-  PHK_REQUIRE(prec == PHK_PREC_F32 || prec == PHK_PREC_BF16, PHK_E_ARG, "maskgit_backward: unknown precision mode");
   if (!context) L = 0;
   PHK_REQUIRE(workspace_bytes >= phk_maskgit_backward_workspace_bytes(m, b, n, L, cfg_pair, head_kind, prec), PHK_E_WORKSPACE,
               "maskgit_backward: workspace too small");
-  const phk_transformer_t* T = &m->transformer;
-  const phk_transformer_t* GT = &grads->transformer;
-  PHK_REQUIRE(T->layers && GT->layers && T->depth > 0 && GT->depth == T->depth && !T->causal, PHK_E_ARG,
-              "maskgit_backward: transformer table / gradient table mismatch");
-  PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "maskgit_backward: dim must be a multiple of 4");
-  const int64_t dc = context_width(T);
-  for (int l = 0; l < T->depth; ++l)
-    PHK_REQUIRE(!context || !T->layers[l].has_cross || T->layers[l].cross_attn.dim_context == dc, PHK_E_UNSUPPORTED,
-                "maskgit_backward: cross-attention layers of different context widths");
+  const int64_t dc = context_width(&m->transformer);
   // without a context both halves of a pair are the same function of the weights: out = cond, no pair to differentiate
   const bool pair = cfg_pair && context;
   const float sc = pair ? cond_scale : 1.0f;
@@ -2433,6 +2445,26 @@ bool cvivit_shapes_ok(const M* m, int32_t B, int32_t Tp) {
          m->patch_h > 0 && m->patch_w > 0 && m->patch_t > 0 && m->image_h % m->patch_h == 0 && m->image_w % m->patch_w == 0;
 }
 
+// The checks of one side's weight table against its gradient table that every C-ViViT backward makes: the stacks'
+// depths and widths, the temporal stack causal with ALiBi slopes and the spatial one not, no cross-attention layer.
+template <class M>  // phk_cvivit_t or phk_cvivit_dec_t
+int check_cvivit_pair(const char* entry, const M* m, const M* grads) {
+  const phk_transformer_t* TT = &m->temporal;
+  const phk_transformer_t* TS = &m->spatial;
+  PHK_REQUIRE_IN(entry, grads->temporal.layers && grads->spatial.layers && grads->temporal.depth == TT->depth &&
+                 grads->spatial.depth == TS->depth, PHK_E_ARG, "weight table / gradient table mismatch");
+  PHK_REQUIRE_IN(entry, TT->causal && TT->alibi_slopes && !TS->causal, PHK_E_ARG,
+                 "the temporal stack is causal with ALiBi slopes, the spatial one is not");
+  PHK_REQUIRE_IN(entry, TT->dim == m->dim && TS->dim == m->dim && TT->heads == m->heads && TS->heads == m->heads &&
+                 TT->dim_head == m->dim_head && TS->dim_head == m->dim_head, PHK_E_ARG,
+                 "transformer widths differ from the model's");
+  PHK_REQUIRE_IN(entry, m->dim % 4 == 0, PHK_E_UNSUPPORTED, "dim must be a multiple of 4");
+  const phk_transformer_t* stacks[2] = {TT, TS};
+  for (const phk_transformer_t* T : stacks)
+    for (int l = 0; l < T->depth; ++l) PHK_REQUIRE_IN(entry, !T->layers[l].has_cross, PHK_E_ARG, "cross-attention layer");
+  return 0;
+}
+
 }  // namespace
 }  // namespace phk
 
@@ -2452,21 +2484,10 @@ extern "C" int phk_cvivit_decode_backward(const phk_cvivit_dec_t* m, const phk_c
   const int64_t need = phk_cvivit_decode_backward_workspace_bytes(m, B, Tp, prec);
   PHK_REQUIRE(need > 0, PHK_E_ARG, "cvivit_decode_backward: bad model table or shape");
   PHK_REQUIRE(workspace_bytes >= need, PHK_E_WORKSPACE, "cvivit_decode_backward: workspace too small");
-  const phk_transformer_t* TT = &m->temporal;
-  const phk_transformer_t* TS = &m->spatial;
-  PHK_REQUIRE(grads->temporal.layers && grads->spatial.layers && grads->temporal.depth == TT->depth &&
-              grads->spatial.depth == TS->depth, PHK_E_ARG, "cvivit_decode_backward: weight table / gradient table mismatch");
-  PHK_REQUIRE(TT->causal && TT->alibi_slopes && !TS->causal, PHK_E_ARG,
-              "cvivit_decode_backward: the temporal stack is causal with ALiBi slopes, the spatial one is not");
-  PHK_REQUIRE(TT->dim == m->dim && TS->dim == m->dim && TT->heads == m->heads && TS->heads == m->heads &&
-              TT->dim_head == m->dim_head && TS->dim_head == m->dim_head, PHK_E_ARG,
-              "cvivit_decode_backward: transformer widths differ from the model's");
-  PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "cvivit_decode_backward: dim must be a multiple of 4");
-  for (int l = 0; l < TT->depth; ++l) PHK_REQUIRE(!TT->layers[l].has_cross, PHK_E_ARG, "cvivit_decode_backward: cross-attention layer");
-  for (int l = 0; l < TS->depth; ++l) PHK_REQUIRE(!TS->layers[l].has_cross, PHK_E_ARG, "cvivit_decode_backward: cross-attention layer");
+  PHK_TRY(check_cvivit_pair("cvivit_decode_backward", m, grads));
   PHK_REQUIRE(!ids || (m->codebook_bits > 0 && m->vq_out_w && m->vq_out_b && grads->vq_out_w && grads->vq_out_b), PHK_E_ARG,
               "cvivit_decode_backward: ids need LFQ's project_out and its gradient");
-  const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(TT), stack_inner(TS)));
+  const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(&m->temporal), stack_inner(&m->spatial)));
   Arena ar{(char*)workspace, workspace_bytes, 0};
   CvShared S;
   PHK_TRY(cv_shared_init(ar, g, m->spatial_bias, prec, s, S));
@@ -2534,24 +2555,12 @@ extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* 
               enc->channels == dec->channels && enc->image_h == dec->image_h && enc->image_w == dec->image_w &&
               enc->patch_h == dec->patch_h && enc->patch_w == dec->patch_w && enc->patch_t == dec->patch_t &&
               enc->codebook_bits == dec->codebook_bits, PHK_E_ARG, "cvivit_backward: encoder and decoder tables differ in shape");
-  const phk_transformer_t* ES = &enc->spatial;
-  const phk_transformer_t* ET = &enc->temporal;
   PHK_REQUIRE(enc->vq_w && enc->vq_b && enc_grads->vq_w && enc_grads->vq_b && dec->vq_out_w && dec->vq_out_b &&
               dec_grads->vq_out_w && dec_grads->vq_out_b, PHK_E_ARG, "cvivit_backward: LFQ's projections and their gradients");
-  PHK_REQUIRE(enc_grads->spatial.layers && enc_grads->temporal.layers && enc_grads->spatial.depth == ES->depth &&
-              enc_grads->temporal.depth == ET->depth && dec_grads->spatial.layers && dec_grads->temporal.layers &&
-              dec_grads->spatial.depth == dec->spatial.depth && dec_grads->temporal.depth == dec->temporal.depth, PHK_E_ARG,
-              "cvivit_backward: weight table / gradient table mismatch");
-  const phk_transformer_t* stacks[4] = {ES, ET, &dec->spatial, &dec->temporal};
-  for (int k = 0; k < 4; ++k) {
-    const phk_transformer_t* T = stacks[k];
-    PHK_REQUIRE(T->dim == dec->dim && T->heads == dec->heads && T->dim_head == dec->dim_head, PHK_E_ARG,
-                "cvivit_backward: transformer widths differ from the model's");
-    PHK_REQUIRE((k % 2 == 1) == (T->causal != 0) && (!T->causal || T->alibi_slopes), PHK_E_ARG,
-                "cvivit_backward: the temporal stacks are causal with ALiBi slopes, the spatial ones are not");
-    for (int l = 0; l < T->depth; ++l) PHK_REQUIRE(!T->layers[l].has_cross, PHK_E_ARG, "cvivit_backward: cross-attention layer");
-  }
-  PHK_REQUIRE(dec->dim % 4 == 0, PHK_E_UNSUPPORTED, "cvivit_backward: dim must be a multiple of 4");
+  PHK_TRY(check_cvivit_pair("cvivit_backward", enc, enc_grads));
+  PHK_TRY(check_cvivit_pair("cvivit_backward", dec, dec_grads));
+  const phk_transformer_t* ES = &enc->spatial;
+  const phk_transformer_t* ET = &enc->temporal;
   const int Tp = 1 + (F - 1) / dec->patch_t;
   const int64_t inner = imax(imax(stack_inner(&dec->temporal), stack_inner(&dec->spatial)), imax(stack_inner(ET), stack_inner(ES)));
   const CvGeom g = cv_geom(dec, B, Tp, inner);
@@ -2668,22 +2677,11 @@ extern "C" int phk_cvivit_encode_backward(const phk_cvivit_t* m, const phk_cvivi
   const int64_t need = phk_cvivit_encode_backward_workspace_bytes(m, B, Tp, prec);
   PHK_REQUIRE(need > 0, PHK_E_ARG, "cvivit_encode_backward: bad model table or shape");
   PHK_REQUIRE(workspace_bytes >= need, PHK_E_WORKSPACE, "cvivit_encode_backward: workspace too small");
-  const phk_transformer_t* TS = &m->spatial;
-  const phk_transformer_t* TT = &m->temporal;
-  PHK_REQUIRE(grads->temporal.layers && grads->spatial.layers && grads->temporal.depth == TT->depth &&
-              grads->spatial.depth == TS->depth, PHK_E_ARG, "cvivit_encode_backward: weight table / gradient table mismatch");
+  PHK_TRY(check_cvivit_pair("cvivit_encode_backward", m, grads));
   const phk_cpb_t& gc = grads->spatial_bias;
   PHK_REQUIRE(gc.w0 && gc.b0 && gc.w1 && gc.b1 && gc.w2 && gc.b2, PHK_E_ARG,
               "cvivit_encode_backward: the gradient table has no position-bias MLP");
-  PHK_REQUIRE(TT->causal && TT->alibi_slopes && !TS->causal, PHK_E_ARG,
-              "cvivit_encode_backward: the temporal stack is causal with ALiBi slopes, the spatial one is not");
-  PHK_REQUIRE(TT->dim == m->dim && TS->dim == m->dim && TT->heads == m->heads && TS->heads == m->heads &&
-              TT->dim_head == m->dim_head && TS->dim_head == m->dim_head, PHK_E_ARG,
-              "cvivit_encode_backward: transformer widths differ from the model's");
-  PHK_REQUIRE(m->dim % 4 == 0, PHK_E_UNSUPPORTED, "cvivit_encode_backward: dim must be a multiple of 4");
-  for (int l = 0; l < TT->depth; ++l) PHK_REQUIRE(!TT->layers[l].has_cross, PHK_E_ARG, "cvivit_encode_backward: cross-attention layer");
-  for (int l = 0; l < TS->depth; ++l) PHK_REQUIRE(!TS->layers[l].has_cross, PHK_E_ARG, "cvivit_encode_backward: cross-attention layer");
-  const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(TS), stack_inner(TT)));
+  const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(&m->spatial), stack_inner(&m->temporal)));
   Arena ar{(char*)workspace, workspace_bytes, 0};
   CvShared S;
   PHK_TRY(cv_shared_init(ar, g, m->spatial_bias, prec, s, S));

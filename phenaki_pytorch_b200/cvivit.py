@@ -20,7 +20,8 @@ from torch import nn
 from . import _lib as L
 from . import sharding
 from .modules import (ContinuousPositionBias, GradKeep, Keep, Transformer, Workspace, _NoParams, cpb_grad_table,
-                      cpb_table, transformer_grad_table, transformer_table, weights_signature)
+                      cpb_table, recompute_in_backward, train_precision, transformer_grad_table, transformer_table,
+                      weights_signature)
 
 
 def _pair(v):
@@ -194,17 +195,21 @@ class CViViT(nn.Module):
         self.load_state_dict(torch.load(str(path)))
 
     # ---- libphk plumbing ---------------------------------------------------------------------
+    def _geometry(self, t):
+        """Fills the header a phk_cvivit_t and a phk_cvivit_dec_t share (widths, image and patch sizes); returns ``t``."""
+        t.dim, t.heads, t.dim_head, t.channels = self.dim, self.heads, self.dim_head, self.channels
+        t.image_h, t.image_w = self.image_size
+        t.patch_h, t.patch_w = self.patch_size
+        t.patch_t = self.temporal_patch_size
+        return t
+
     def _table(self):
         sig = (weights_signature(self), self.precision)
         if self._tables is None or sig != self._sig:
             keep = Keep()
             h16 = self.precision == L.PREC_BF16
             mode = self.precision  # which tensor-core weight copies the table carries (none in parity mode)
-            t = L.CvivitT()
-            t.dim, t.heads, t.dim_head, t.channels = self.dim, self.heads, self.dim_head, self.channels
-            t.image_h, t.image_w = self.image_size
-            t.patch_h, t.patch_w = self.patch_size
-            t.patch_t = self.temporal_patch_size
+            t = self._geometry(L.CvivitT())
             t.codebook_bits = self.vq.codebook_dim if self.lookup_free_quantization else 0
             f, r = self.to_patch_emb_first_frame, self.to_patch_emb
             t.pf_ln1_g, t.pf_ln1_b, t.pf_w, t.pf_b = keep.t(f[1].weight), keep.t(f[1].bias), keep.t(f[2].weight), keep.t(f[2].bias)
@@ -231,11 +236,7 @@ class CViViT(nn.Module):
         if self._dec_tables is None or sig != self._dec_sig:
             keep = Keep()
             mode = self.precision
-            t = L.CvivitDecT()
-            t.dim, t.heads, t.dim_head, t.channels = self.dim, self.heads, self.dim_head, self.channels
-            t.image_h, t.image_w = self.image_size
-            t.patch_h, t.patch_w = self.patch_size
-            t.patch_t = self.temporal_patch_size
+            t = self._geometry(L.CvivitDecT())
             if self.lookup_free_quantization:
                 t.codebook_bits = self.vq.codebook_dim
                 t.vq_out_w, t.vq_out_b = keep.t(self.vq.project_out.weight), keep.t(self.vq.project_out.bias)
@@ -286,7 +287,7 @@ class CViViT(nn.Module):
             if ids is None:
                 ids = self._ids_buf[key] = torch.empty((b, tp, hh, ww), dtype=torch.int64, device=video.device)
             nbytes = lib.phk_cvivit_workspace_bytes(C.byref(table), b, f, self.precision)
-            ws = self._ws.get(nbytes, video.device)
+            ws = self._ws.get_for("phk_cvivit_workspace_bytes", nbytes, video.device)
             bias = self._spatial_bias(table, video.device)
             tap_ptrs = [None] * 4
             if taps is not None:
@@ -336,7 +337,7 @@ class CViViT(nn.Module):
                         dev_ids = torch.empty((depth, b, tp, hh, ww), dtype=torch.int64, device=device)
                         host = [torch.empty((b, tp, hh, ww), dtype=torch.int64).pin_memory() for _ in range(depth)]
                         nbytes = lib.phk_cvivit_workspace_bytes(C.byref(table), b, f, self.precision)
-                        ws = self._ws.get(nbytes, device)
+                        ws = self._ws.get_for("phk_cvivit_workspace_bytes", nbytes, device)
                     assert tuple(video.shape) == shape, "all batches of one stream must have the same shape"
                     if len(inflight) == depth:
                         yield retire().clone()
@@ -426,8 +427,10 @@ class CViViT(nn.Module):
                    list(self.spatial_rel_pos_bias.parameters())])
 
     def _recon_loss(self, video, mask):
-        """(loss, recon): the masked MSE of decode(encode(video)) against video, differentiable through
-        ``_ReconLossFn`` when grad mode is on and ``video`` or a parameter requires grad."""
+        """(loss, recon): the masked MSE of decode(encode(video)) against video, differentiable with respect to
+        ``video`` and the parameters by ``recompute_in_backward`` through phk_cvivit_backward.  The backward decodes from
+        the forward's ids, so it differentiates the function whose loss was returned even where a recomputed projection
+        would flip a sign; LFQ's straight-through estimator makes d x independent of the signs."""
         video = L.require_cuda(video, "video", torch.float32)
         b, c, f, *image_dims = video.shape
         assert tuple(image_dims) == self.image_size and c == self.channels
@@ -447,11 +450,16 @@ class CViViT(nn.Module):
             self.calculate_video_token_mask(video, mask)  # for its assertion only, as the reference (LFQ takes no mask)
             mask = mask.to(torch.uint8).contiguous()
         params = self._encoder_params() + self._decoder_params(True)
-        spec = dict(net=self, mask=mask, params=params, n_enc=len(self._encoder_params()), precision=self.precision,
-                    straight_through=self.vq.training, sig=weights_signature(self), sync=bool(self.sync_gradients))
-        if torch.is_grad_enabled() and (video.requires_grad or any(p.requires_grad for p in params)):
-            return _ReconLossFn.apply(spec, video, *params)
-        return self._recon_forward(video.detach(), mask)[1:]
+        call = dict(params=params, n_enc=len(self._encoder_params()), precision=self.precision,
+                    straight_through=self.vq.training, sync=bool(self.sync_gradients))
+
+        def run():
+            ids, loss, recon = self._recon_forward(video.detach(), mask)
+            return (loss, recon), (video, ids, recon, mask)
+
+        return recompute_in_backward("CViViT.forward (the reconstruction loss)", self, run,
+                                     lambda saved, g, needs: self._recon_backward(call, saved, *g, needs[0]), [video],
+                                     params)
 
     def _recon_forward(self, video, mask):
         """(ids, loss, recon) of the inference path: phk_cvivit_encode, phk_cvivit_decode from the ids, the loss."""
@@ -470,11 +478,7 @@ class CViViT(nn.Module):
         """The phk_cvivit_t-shaped table addressing the encoder side's gradient buffers in ``gk``: both stacks, plus
         to_patch_emb* and LFQ's project_in for the reconstruction loss (``recon``; the position-bias MLP's gradient then
         goes through the decoder's table), or the position-bias MLP for ``encode`` (no quantiser: cosine-sim modules too)."""
-        t = L.CvivitT()
-        t.dim, t.heads, t.dim_head, t.channels = self.dim, self.heads, self.dim_head, self.channels
-        t.image_h, t.image_w = self.image_size
-        t.patch_h, t.patch_w = self.patch_size
-        t.patch_t = self.temporal_patch_size
+        t = self._geometry(L.CvivitT())
         if recon:
             t.codebook_bits = self.vq.codebook_dim
             f, r = self.to_patch_emb_first_frame, self.to_patch_emb
@@ -491,18 +495,15 @@ class CViViT(nn.Module):
         t.temporal = transformer_grad_table(self.enc_temporal_transformer, gk, False)
         return t
 
-    def _recon_backward(self, spec, video, ids, recon, dloss, drecon, want_video_grad):
-        """phk_cvivit_backward for one ``_ReconLossFn`` call: ([gradient or None per parameter of spec["params"]],
-        d video or None)."""
-        if weights_signature(self) != spec["sig"]:
-            raise RuntimeError("a parameter of this module was modified or replaced between the forward and the backward: "
-                               "the backward recomputes the forward from the current weights, so it would differentiate "
-                               "another function")
+    def _recon_backward(self, call, saved, dloss, drecon, want_video_grad):
+        """phk_cvivit_backward for one ``_recon_loss`` call: ([d video or None], [gradient or None per parameter of
+        call["params"]])."""
+        video, ids, recon, mask = saved
         lib = L.lib()
         dev = video.device
         b, _, f = video.shape[:3]
-        prec = L.PREC_BF16 if spec["precision"] == L.PREC_BF16 else L.PREC_F32  # split-bf16 is an inference mode
-        straight = spec["straight_through"]
+        prec = train_precision(call["precision"])
+        straight = call["straight_through"]
         with torch.cuda.device(dev):
             enc, dec = self._table(), self._dec_table()
             groups = self._recon_gradient_groups()
@@ -514,11 +515,9 @@ class CViViT(nn.Module):
             drecon = None if drecon is None else drecon.to(dev, torch.float32).reshape(recon.shape).contiguous()
             dvideo = torch.empty_like(video) if want_video_grad else None
             nbytes = lib.phk_cvivit_backward_workspace_bytes(C.byref(enc), C.byref(dec), b, f, prec)
-            if nbytes < 0:
-                raise L.PhkError("phk_cvivit_backward_workspace_bytes: unsupported configuration")
-            ws = self._ws.get(nbytes, dev)
+            ws = self._ws.get_for("phk_cvivit_backward_workspace_bytes", nbytes, dev)
             plan = None
-            if spec["sync"]:
+            if call["sync"]:
                 n_groups = lib.phk_cvivit_backward_progress_groups(C.byref(enc), C.byref(dec))
                 assert n_groups == len(groups), f"phk_cvivit_backward records {n_groups} events, not {len(groups)}"
                 plan = sharding.overlap_plan(self, gk.flat, n_groups, dev)
@@ -527,18 +526,18 @@ class CViViT(nn.Module):
                 L.check(lib.phk_train_set_progress_events(plan["handles"], len(plan["events"])),
                         "phk_train_set_progress_events")
             L.check(lib.phk_cvivit_backward(C.byref(enc), C.byref(egt), C.byref(dec), C.byref(dgt), L.ptr(video),
-                                            L.ptr(recon), L.ptr(ids), L.ptr(spec["mask"]), b, f, L.ptr(dloss),
+                                            L.ptr(recon), L.ptr(ids), L.ptr(mask), b, f, L.ptr(dloss),
                                             L.ptr(drecon), L.ptr(dvideo), int(straight), L.ptr(ws), ws.numel(), prec,
                                             L.stream_ptr()),
                     "phk_cvivit_backward")
             if plan is not None:
                 torch.cuda.current_stream().wait_event(sharding.launch_overlapped_all_reduce(gk.flat, plan, spans))
-            elif spec["sync"]:
+            elif call["sync"]:
                 sharding.all_reduce_mean_(gk.flat)
-        grads = [gk.grad_of(p) for p in spec["params"]]
+        grads = [gk.grad_of(p) for p in call["params"]]
         if not straight:  # eval mode: q is a constant, nothing reaches the encoder
-            grads[:spec["n_enc"]] = [None] * spec["n_enc"]
-        return grads, dvideo
+            grads[:call["n_enc"]] = [None] * call["n_enc"]
+        return [dvideo], grads
 
     def _decode(self, ids, tokens, b, tp, device, taps=None):
         lib = L.lib()
@@ -548,7 +547,7 @@ class CViViT(nn.Module):
             f = 1 + (tp - 1) * self.temporal_patch_size
             video = torch.empty((b, self.channels, f, *self.image_size), dtype=torch.float32, device=device)
             nbytes = lib.phk_cvivit_decode_workspace_bytes(C.byref(table), b, tp, self.precision)
-            ws = self._ws.get(nbytes, device)
+            ws = self._ws.get_for("phk_cvivit_decode_workspace_bytes", nbytes, device)
             bias = self._spatial_bias(enc, device)
             tap_ptrs = [None] * 3
             if taps is not None:
@@ -572,11 +571,7 @@ class CViViT(nn.Module):
 
     def _dec_grad_table(self, gk, with_project_out):
         """The phk_cvivit_dec_t-shaped table addressing the decoder side's gradient buffers in ``gk``."""
-        t = L.CvivitDecT()
-        t.dim, t.heads, t.dim_head, t.channels = self.dim, self.heads, self.dim_head, self.channels
-        t.image_h, t.image_w = self.image_size
-        t.patch_h, t.patch_w = self.patch_size
-        t.patch_t = self.temporal_patch_size
+        t = self._geometry(L.CvivitDecT())
         if with_project_out:
             t.codebook_bits = self.vq.codebook_dim
             t.vq_out_w, t.vq_out_b = gk.g(self.vq.project_out.weight), gk.g(self.vq.project_out.bias)
@@ -589,43 +584,39 @@ class CViViT(nn.Module):
         return t
 
     def _differentiable_decode(self, ids, tokens, b, tp, device, taps=None):
-        """``_decode`` exactly as it runs under ``torch.no_grad`` and, when autograd wants a gradient of it (grad mode on,
-        and a decoder-side parameter or ``tokens`` requires grad), connected to phk_cvivit_decode_backward through
-        ``_DecodeFn``."""
+        """``_decode`` exactly as it runs under ``torch.no_grad``, made differentiable with respect to ``tokens`` and the
+        decoder-side parameters by ``recompute_in_backward`` through phk_cvivit_decode_backward."""
+        call = dict(params=self._decoder_params(ids is not None), b=b, tp=tp, precision=self.precision)
+
         def run():
-            return self._decode(ids, None if tokens is None else tokens.detach(), b, tp, device, taps)
+            video = self._decode(ids, None if tokens is None else tokens.detach(), b, tp, device, taps)
+            return video, (ids, tokens)
 
-        params = self._decoder_params(ids is not None)
-        if not torch.is_grad_enabled() or not (any(p.requires_grad for p in params)
-                                               or (tokens is not None and tokens.requires_grad)):
-            return run()
-        spec = dict(net=self, params=params, b=b, tp=tp, precision=self.precision, sig=weights_signature(self))
-        return _DecodeFn.apply(run, spec, ids, tokens, *params)
+        return recompute_in_backward("CViViT.decode", self, run,
+                                     lambda saved, g, needs: self._decode_backward(call, saved, g[0], needs[0]),
+                                     [tokens], call["params"])
 
-    def _decode_backward(self, spec, dvideo, ids, tokens, want_tokens_grad):
-        """phk_cvivit_decode_backward for one ``_differentiable_decode`` call: ([gradient or None per parameter of
-        spec["params"]], d tokens or None)."""
-        if weights_signature(self) != spec["sig"]:
-            raise RuntimeError("a parameter of this module was modified or replaced between the decode and the backward: "
-                               "the backward recomputes the decode from the current weights, so it would differentiate "
-                               "another function")
+    def _decode_backward(self, call, saved, dvideo, want_tokens_grad):
+        """phk_cvivit_decode_backward for one ``_differentiable_decode`` call: ([d tokens or None], [gradient or None per
+        parameter of call["params"]])."""
+        ids, tokens = saved
         lib = L.lib()
         dvideo = L.require_cuda(dvideo.to(torch.float32), "upstream gradient")
         dev = dvideo.device
-        b, tp = spec["b"], spec["tp"]
-        prec = L.PREC_BF16 if spec["precision"] == L.PREC_BF16 else L.PREC_F32  # split-bf16 is an inference mode
+        b, tp = call["b"], call["tp"]
+        prec = train_precision(call["precision"])
         with torch.cuda.device(dev):
             table = self._dec_table()
-            gk = GradKeep(spec["params"])
+            gk = GradKeep(call["params"])
             gtable = self._dec_grad_table(gk, ids is not None)
             dtokens = torch.empty_like(tokens) if tokens is not None and want_tokens_grad else None
             nbytes = lib.phk_cvivit_decode_backward_workspace_bytes(C.byref(table), b, tp, prec)
-            ws = self._ws.get(nbytes, dev)
+            ws = self._ws.get_for("phk_cvivit_decode_backward_workspace_bytes", nbytes, dev)
             L.check(lib.phk_cvivit_decode_backward(C.byref(table), C.byref(gtable), L.ptr(ids), L.ptr(tokens), b, tp,
                                                    L.ptr(dvideo), L.ptr(dtokens), L.ptr(ws), ws.numel(), prec,
                                                    L.stream_ptr()),
                     "phk_cvivit_decode_backward")
-        return [gk.grad_of(p) for p in spec["params"]], dtokens
+        return [dtokens], [gk.grad_of(p) for p in call["params"]]
 
     def decode_from_codebook_indices(self, indices, taps=None):
         """ids (b, n) or (b, t, h, w) int64 CUDA -> video (b, c, f, H, W) fp32 (cvivit.py:437-443): LFQ
@@ -670,47 +661,41 @@ class CViViT(nn.Module):
             table = self._table()
             out = torch.empty_like(tokens)
             nbytes = lib.phk_cvivit_encode_tokens_workspace_bytes(C.byref(table), b, tp, self.precision)
-            if nbytes < 0:
-                raise L.PhkError("phk_cvivit_encode_tokens_workspace_bytes: unsupported configuration")
-            ws = self._ws.get(nbytes, dev)
+            ws = self._ws.get_for("phk_cvivit_encode_tokens_workspace_bytes", nbytes, dev)
             bias = self._spatial_bias(table, dev)
             L.check(lib.phk_cvivit_encode_tokens(C.byref(table), L.ptr(tokens), b, tp, L.ptr(out), L.ptr(ws), ws.numel(),
                                                  self.precision, L.ptr(bias), L.stream_ptr()),
                     "phk_cvivit_encode_tokens")
         return out
 
-    def _encode_backward(self, spec, dout, tokens, want_tokens_grad):
-        """phk_cvivit_encode_backward for one ``encode`` call: ([gradient or None per parameter of spec["params"]],
-        d tokens or None)."""
-        if weights_signature(self) != spec["sig"]:
-            raise RuntimeError("a parameter of this module was modified or replaced between the encode and the backward: "
-                               "the backward recomputes the encode from the current weights, so it would differentiate "
-                               "another function")
+    def _encode_backward(self, call, saved, dout, want_tokens_grad):
+        """phk_cvivit_encode_backward for one ``encode`` call: ([d tokens or None], [gradient or None per parameter of
+        call["params"]])."""
+        tokens, = saved
         lib = L.lib()
         dout = L.require_cuda(dout.to(torch.float32), "upstream gradient")
         dev = dout.device
-        b, tp = spec["b"], spec["tp"]
-        prec = L.PREC_BF16 if spec["precision"] == L.PREC_BF16 else L.PREC_F32  # split-bf16 is an inference mode
+        b, tp = call["b"], call["tp"]
+        prec = train_precision(call["precision"])
         with torch.cuda.device(dev):
             table = self._table()
-            gk = GradKeep(spec["params"])
+            gk = GradKeep(call["params"])
             gtable = self._enc_grad_table(gk, False)
             dtokens = torch.empty_like(tokens) if want_tokens_grad else None
             nbytes = lib.phk_cvivit_encode_backward_workspace_bytes(C.byref(table), b, tp, prec)
-            if nbytes < 0:
-                raise L.PhkError("phk_cvivit_encode_backward_workspace_bytes: unsupported configuration")
-            ws = self._ws.get(nbytes, dev)
+            ws = self._ws.get_for("phk_cvivit_encode_backward_workspace_bytes", nbytes, dev)
             L.check(lib.phk_cvivit_encode_backward(C.byref(table), C.byref(gtable), L.ptr(tokens), b, tp, L.ptr(dout),
                                                    L.ptr(dtokens), L.ptr(ws), ws.numel(), prec, L.stream_ptr()),
                     "phk_cvivit_encode_backward")
-        return [gk.grad_of(p) for p in spec["params"]], dtokens
+        return [dtokens], [gk.grad_of(p) for p in call["params"]]
 
     def encode(self, tokens):
         """tokens (b, t, h, w, dim) fp32 CUDA, (h, w) = patch_height_width -> a new (b, t, h, w, dim) fp32 tensor: the
         encoder's spatial and temporal transformers (cvivit.py:449-474), the temporal one's norm_out included.  The
         quantiser is not involved.  Differentiable: with grad mode on and ``tokens`` or an encoder-stack / position-bias
         parameter requiring grad, ``f(out).backward()`` fills their gradients through phk_cvivit_encode_backward, which
-        recomputes both stacks with saved activations.  No dropout is applied (DESIGN.md section 8)."""
+        recomputes both stacks with saved activations (``recompute_in_backward``).  No dropout is applied (DESIGN.md
+        section 8)."""
         assert tokens.ndim == 5, f"tokens must be (b, t, h, w, dim), got {tuple(tokens.shape)}"
         b, t, h, w, d = tokens.shape
         assert (h, w) == tuple(self.patch_height_width), \
@@ -718,84 +703,7 @@ class CViViT(nn.Module):
         assert d == self.dim, f"token width {d} is not the module's dim {self.dim}"
         assert b > 0 and t > 0, "empty batch or no latent frames"
         tokens = L.require_cuda(tokens, "tokens", torch.float32)
-
-        def run():
-            return self._encode_tokens(tokens.detach())
-
-        params = self._encode_params()
-        if not torch.is_grad_enabled() or not (tokens.requires_grad or any(p.requires_grad for p in params)):
-            return run()
-        spec = dict(net=self, params=params, b=b, tp=t, precision=self.precision, sig=weights_signature(self))
-        return _EncodeFn.apply(run, spec, tokens, *params)
-
-
-class _DecodeFn(torch.autograd.Function):
-    """Makes the C-ViViT decode differentiable.  The forward runs the library's decode unchanged (same launches, same
-    values) and keeps only its inputs; the backward recomputes it with saved activations inside
-    phk_cvivit_decode_backward, as activation checkpointing does.  The decode applies no dropout (DESIGN.md section 8),
-    so the backward applies none either: it differentiates the function the forward returned."""
-
-    @staticmethod
-    def forward(ctx, run, spec, ids, tokens, *params):
-        ctx.spec = spec
-        ctx.save_for_backward(ids, None if tokens is None else tokens.detach())
-        return run()
-
-    @staticmethod
-    def backward(ctx, dvideo):
-        if torch.is_grad_enabled():
-            raise RuntimeError("CViViT.decode does not support create_graph=True: its backward is hand-written CUDA and "
-                               "builds no graph of its own")
-        ids, tokens = ctx.saved_tensors
-        spec = ctx.spec
-        grads, dtokens = spec["net"]._decode_backward(spec, dvideo, ids, tokens, ctx.needs_input_grad[3])
-        return (None, None, None, dtokens, *grads)
-
-
-class _ReconLossFn(torch.autograd.Function):
-    """Makes the C-ViViT reconstruction loss differentiable.  The forward runs the inference path unchanged (encode to
-    ids, decode from them, the loss kernel) and keeps the video, the ids, the reconstruction and the mask; the backward
-    recomputes the decoder and, in training mode, the encoder with saved activations inside phk_cvivit_backward.  It
-    decodes from the forward's ids, so it differentiates the function whose loss was returned even where a recomputed
-    projection would flip a sign; LFQ's straight-through estimator makes d x independent of the signs."""
-
-    @staticmethod
-    def forward(ctx, spec, video, *params):
-        ctx.set_materialize_grads(False)
-        ids, loss, recon = spec["net"]._recon_forward(video.detach(), spec["mask"])
-        ctx.spec = spec
-        ctx.save_for_backward(video.detach(), ids, recon)
-        return loss, recon
-
-    @staticmethod
-    def backward(ctx, dloss, drecon):
-        if torch.is_grad_enabled():
-            raise RuntimeError("the C-ViViT reconstruction loss does not support create_graph=True: its backward is "
-                               "hand-written CUDA and builds no graph of its own")
-        video, ids, recon = ctx.saved_tensors
-        spec = ctx.spec
-        grads, dvideo = spec["net"]._recon_backward(spec, video, ids, recon, dloss, drecon, ctx.needs_input_grad[1])
-        return (None, dvideo, *grads)
-
-
-class _EncodeFn(torch.autograd.Function):
-    """Makes ``CViViT.encode(tokens)`` differentiable.  The forward runs the library's encoder stacks unchanged (same
-    launches, same values) and keeps only the detached tokens; the backward recomputes both stacks with saved
-    activations inside phk_cvivit_encode_backward.  No dropout either way: it differentiates the function the forward
-    returned."""
-
-    @staticmethod
-    def forward(ctx, run, spec, tokens, *params):
-        ctx.spec = spec
-        ctx.save_for_backward(tokens.detach())
-        return run()
-
-    @staticmethod
-    def backward(ctx, dout):
-        if torch.is_grad_enabled():
-            raise RuntimeError("CViViT.encode does not support create_graph=True: its backward is hand-written CUDA and "
-                               "builds no graph of its own")
-        tokens, = ctx.saved_tensors
-        spec = ctx.spec
-        grads, dtokens = spec["net"]._encode_backward(spec, dout, tokens, ctx.needs_input_grad[2])
-        return (None, None, dtokens, *grads)
+        call = dict(params=self._encode_params(), b=b, tp=t, precision=self.precision)
+        return recompute_in_backward("CViViT.encode", self, lambda: (self._encode_tokens(tokens.detach()), (tokens,)),
+                                     lambda saved, g, needs: self._encode_backward(call, saved, g[0], needs[0]),
+                                     [tokens], call["params"])

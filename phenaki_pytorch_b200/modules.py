@@ -379,3 +379,67 @@ class Workspace:
         if self.buf is None or self.buf.numel() < nbytes or self.buf.device != device:
             self.buf = torch.empty(int(nbytes), dtype=torch.uint8, device=device)
         return self.buf
+
+    def get_for(self, query, nbytes, device):
+        """``get`` for the byte count ``nbytes`` that the library's ``query`` (a ``phk_*_workspace_bytes``) returned; a
+        negative count means the library does not support the call's tables or shapes, which raises here."""
+        if nbytes < 0:
+            raise L.PhkError(f"{query}: unsupported configuration")
+        return self.get(nbytes, device)
+
+
+def train_precision(p):
+    """The precision mode a training step or backward runs in for a module in mode ``p``: split-bf16 is an inference
+    mode, so it trains in fp32."""
+    return L.PREC_BF16 if p == L.PREC_BF16 else L.PREC_F32
+
+
+def refuse_create_graph(entry):
+    """The hand-written backwards build no graph of their own, so they cannot be differentiated again."""
+    if torch.is_grad_enabled():
+        raise RuntimeError(f"{entry} does not support create_graph=True: its backward is hand-written CUDA and builds "
+                           "no graph of its own")
+
+
+def recompute_in_backward(entry, owner, run, backward, inputs, params):
+    """Makes a library entry point differentiable by recomputing it in the backward, as activation checkpointing does.
+
+    ``run()`` -> (outputs, saved) runs the inference path unchanged (same launches, same values).  Without grad mode, or
+    when nothing in ``inputs`` (tensors or None) or ``params`` requires grad, its outputs are returned as they are.
+    Otherwise they are connected to autograd: the forward keeps only ``saved`` (detached), and the backward calls
+    ``backward(saved, grad_outputs, needs_input_grad)`` -> (a gradient or None per input, per parameter), a library
+    entry point that recomputes the forward with saved activations from the current weights.  A weight modified or
+    replaced in between would make it differentiate another function, so ``weights_signature(owner)`` is taken here and
+    the backward refuses when it has changed; ``create_graph=True`` is refused too.  Only outputs that received a
+    gradient get one (None for the others).  ``entry`` names the call in these refusals.  The entry points apply no
+    dropout (DESIGN.md section 8), so neither does the recomputation: it differentiates the function the forward
+    returned."""
+    if not torch.is_grad_enabled() or not (any(t is not None and t.requires_grad for t in inputs)
+                                           or any(p.requires_grad for p in params)):
+        return run()[0]
+    call = dict(entry=entry, owner=owner, backward=backward, sig=weights_signature(owner), n=len(inputs))
+    return _RecomputeInBackward.apply(run, call, *inputs, *params)
+
+
+class _RecomputeInBackward(torch.autograd.Function):
+    """The autograd node of ``recompute_in_backward``; ``run`` is not kept, only what it saved."""
+
+    @staticmethod
+    def forward(ctx, run, call, *inputs_and_params):
+        ctx.set_materialize_grads(False)
+        ctx.call = call
+        out, saved = run()
+        ctx.save_for_backward(*(None if t is None else t.detach() for t in saved))
+        return out
+
+    @staticmethod
+    def backward(ctx, *grad_outputs):
+        call = ctx.call
+        refuse_create_graph(call["entry"])
+        if weights_signature(call["owner"]) != call["sig"]:
+            raise RuntimeError(f"{call['entry']}: a parameter of this module was modified or replaced between the forward "
+                               "and the backward: the backward recomputes the forward from the current weights, so it "
+                               "would differentiate another function")
+        n = call["n"]
+        input_grads, param_grads = call["backward"](ctx.saved_tensors, grad_outputs, ctx.needs_input_grad[2:2 + n])
+        return (None, None, *input_grads, *param_grads)

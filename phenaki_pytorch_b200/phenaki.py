@@ -21,7 +21,8 @@ from . import sharding
 from .cvivit import CViViT
 
 from .modules import (ContinuousPositionBias, GradKeep, Keep, Transformer, Workspace, _NoParams, cpb_grad_table,
-                      cpb_table, transformer_grad_table, transformer_table, weights_signature)
+                      cpb_table, recompute_in_backward, refuse_create_graph, train_precision, transformer_grad_table,
+                      transformer_table, weights_signature)
 
 
 def _noise_seed(dev):
@@ -158,7 +159,7 @@ class _TokenTransformer(nn.Module):
             width = table.dim if embeds_only else table.num_tokens
             out = torch.empty((reps * b, n, width), dtype=torch.float32, device=dev)
             nbytes = lib.phk_maskgit_workspace_bytes(C.byref(table), b, n, ctx_len, int(cfg_pair), self.precision)
-            ws = self._ws.get(nbytes, dev)
+            ws = self._ws.get_for("phk_maskgit_workspace_bytes", nbytes, dev)
             bias = self._pos_bias(table, patch_shape, dev)
             if text_mask is not None:
                 text_mask = L.require_cuda(text_mask.to(torch.uint8), "text mask")
@@ -183,7 +184,7 @@ class _TokenTransformer(nn.Module):
         with torch.cuda.device(dev):
             table = self._table()
             nbytes = lib.phk_maskgit_sample_workspace_bytes(C.byref(table), b, n, ctx_len)
-            ws = self._ws.get(nbytes, dev)
+            ws = self._ws.get_for("phk_maskgit_sample_workspace_bytes", nbytes, dev)
             bias = self._pos_bias(table, patch_shape, dev)
             if text_mask is not None:
                 text_mask = L.require_cuda(text_mask.to(torch.uint8), "text mask")
@@ -260,27 +261,15 @@ class _TokenTransformer(nn.Module):
         assert _prod(patch_shape) == n, "video patch shape must cover the token sequence"
         dev = ids_in.device
         with torch.cuda.device(dev):
-            table = self._table()
+            table, keep, context, text_mask, video_mask = self._call_tables(b, head, context, text_mask, video_mask)
             assert n <= table.max_seq_len, \
                 f"the video token sequence length you are passing in ({n}) is greater than the `max_seq_len` ({table.max_seq_len})"
-            keep = Keep()
-            if head is not None:  # same body, another head: a shallow copy of the table with the head members swapped
-                table = L.MaskgitT.from_buffer_copy(table)
-                table.head_w, table.head_b, table.head_w_h = keep.t(head.weight), keep.t(head.bias), None
-            has_cross = context is not None and self.transformer.layers[0][2] is not None
+            has_cross = context is not None
             ctx_len = 0
             if has_cross:
-                context = L.require_cuda(context, "text embeds", torch.float32)
                 assert context.shape[0] == b and context.shape[-1] == self.transformer.layers[0][2].dim_context, \
                     "text embedding dimension is not correct"
                 ctx_len = context.shape[1]
-                if text_mask is None:
-                    text_mask = torch.ones((b, ctx_len), device=dev, dtype=torch.bool)
-                text_mask = L.require_cuda(text_mask.to(torch.uint8), "text mask")
-            else:
-                context = text_mask = None
-            if video_mask is not None:
-                video_mask = L.require_cuda(video_mask.to(torch.uint8), "video mask")
             if bce:
                 labels = L.require_cuda(labels.reshape(b, n).float(), "critic labels", torch.float32)
                 targets = token_mask = None
@@ -295,9 +284,9 @@ class _TokenTransformer(nn.Module):
             if keep_logits and not bce:
                 logits = torch.empty((b, n, table.num_tokens), dtype=torch.float32, device=dev)
             loss = torch.zeros((), dtype=torch.float32, device=dev)
-            prec = L.PREC_BF16 if self.precision == L.PREC_BF16 else L.PREC_F32  # (split-bf16 is an inference mode)
+            prec = train_precision(self.precision)
             nbytes = lib.phk_maskgit_train_workspace_bytes(C.byref(table), b, n, ctx_len, int(bce), prec)
-            ws = self._ws.get(nbytes, dev)
+            ws = self._ws.get_for("phk_maskgit_train_workspace_bytes", nbytes, dev)
             pt, ph, pw = (int(v) for v in patch_shape)
             dropout = None
             if dropout_on:  # reserve exactly the counters the step's masks use (the C side owns the layout)
@@ -345,61 +334,67 @@ class _TokenTransformer(nn.Module):
         groups = self._gradient_groups(gk, owner)
         return None if groups is None else dict(plan, groups=groups)
 
+    def _call_tables(self, b, head, context, text_mask, video_mask):
+        """(weight table, its Keep, context, text mask, video mask) as phk_maskgit_train_step and phk_maskgit_backward
+        take them.  ``head``: an nn.Linear(dim, 1) that replaces the network's own head (SelfCritic.to_pred) in a shallow
+        copy of the table.  The context and text mask are dropped when the network has no cross-attention; an absent
+        text mask is all true."""
+        table = self._table()
+        keep = Keep()
+        if head is not None:
+            table = L.MaskgitT.from_buffer_copy(table)
+            table.head_w, table.head_b, table.head_w_h = keep.t(head.weight), keep.t(head.bias), None
+        if context is None or self.transformer.layers[0][2] is None:
+            context = text_mask = None
+        else:
+            context = L.require_cuda(context, "text embeds", torch.float32)
+            if text_mask is None:
+                text_mask = torch.ones((b, context.shape[1]), device=context.device, dtype=torch.bool)
+            text_mask = L.require_cuda(text_mask.to(torch.uint8), "text mask")
+        if video_mask is not None:
+            video_mask = L.require_cuda(video_mask.to(torch.uint8), "video mask")
+        return table, keep, context, text_mask, video_mask
+
     def _differentiable(self, run, owner, ids, patch_shape, *, context, text_mask, video_mask, cond_scale, head_kind,
                         head=None):
-        """Returns ``run()`` -- the forward exactly as it runs under ``torch.no_grad`` -- and, when autograd wants a
-        gradient of it (grad mode on, and a parameter of ``owner`` or ``context`` requires grad), connects the result to
-        the hand-written backward (phk_maskgit_backward) through ``_ForwardBackwardFn``.
+        """``run()`` -- the forward exactly as it runs under ``torch.no_grad`` -- made differentiable with respect to the
+        parameters of ``owner`` and ``context`` by ``recompute_in_backward`` through phk_maskgit_backward.
         ids (b, n), patch_shape, context (the text embeddings, or None when the network ignores them), text_mask (after
         the cond_drop_prob draw), video_mask, cond_scale (!= 1: the CFG pair) and head_kind (_lib.HEAD_*) describe
         the call; ``head``: an nn.Linear(dim, 1) that replaces the network's own head (SelfCritic.to_pred)."""
-        params = list(owner.parameters())
-        if not torch.is_grad_enabled() or not (any(p.requires_grad for p in params)
-                                               or (context is not None and context.requires_grad)):
-            return run()
-        spec = dict(net=self, owner=owner, head=head, patch_shape=tuple(int(v) for v in patch_shape),
-                    cond_scale=float(cond_scale), head_kind=head_kind, sig=weights_signature(owner))
-        return _ForwardBackwardFn.apply(run, spec, ids, text_mask if context is not None else None, video_mask,
-                                        context, *params)
+        call = dict(owner=owner, head=head, patch_shape=tuple(int(v) for v in patch_shape), cond_scale=float(cond_scale),
+                    head_kind=head_kind)
+        saved = (ids, text_mask if context is not None else None, video_mask, context)
+        entry = f"{type(owner).__name__}.{'forward' if cond_scale == 1 else 'forward_with_cond_scale'}"
+        return recompute_in_backward(entry, owner, lambda: (run(), saved),
+                                     lambda s, g, needs: self._backward_from(call, s, g[0], needs[0]),
+                                     [context], list(owner.parameters()))
 
-    def _backward_from(self, spec, upstream, ids, text_mask, video_mask, context, want_context_grad):
-        """phk_maskgit_backward for one ``_differentiable`` call: ([gradient or None per parameter of the owner],
-        d context or None).  The gradients are copies: the flat bucket they were accumulated in is free again on
-        return."""
+    def _backward_from(self, call, saved, upstream, want_context_grad):
+        """phk_maskgit_backward for one ``_differentiable`` call: ([d context or None], [gradient or None per parameter of
+        the owner]).  The gradients are copies: the flat bucket they were accumulated in is free again on return."""
         lib = L.lib()
-        owner, head, head_kind = spec["owner"], spec["head"], spec["head_kind"]
-        if weights_signature(owner) != spec["sig"]:
-            raise RuntimeError("a parameter of this module was modified or replaced between the forward and the backward: "
-                               "the backward recomputes the forward from the current weights, so it would differentiate "
-                               "another function")
+        owner, head, head_kind = call["owner"], call["head"], call["head_kind"]
+        ids, text_mask, video_mask, context = saved
         ids = L.require_cuda(ids, "token ids", torch.int64)
         b, n = ids.shape
         dev = ids.device
         with torch.cuda.device(dev):
-            table = self._table()
-            keep = Keep()
-            if head is not None:  # same body, another head (as in train_step)
-                table = L.MaskgitT.from_buffer_copy(table)
-                table.head_w, table.head_b, table.head_w_h = keep.t(head.weight), keep.t(head.bias), None
+            table, keep, context, text_mask, video_mask = self._call_tables(b, head, context, text_mask, video_mask)
             has_cross = context is not None
             ctx_len = context.shape[1] if has_cross else 0
-            if has_cross:
-                context = L.require_cuda(context.detach(), "text embeds", torch.float32)
-                text_mask = L.require_cuda(text_mask.to(torch.uint8), "text mask")
-            if video_mask is not None:
-                video_mask = L.require_cuda(video_mask.to(torch.uint8), "video mask")
             upstream = L.require_cuda(upstream.to(torch.float32), "upstream gradient")
-            cfg = spec["cond_scale"] != 1
-            prec = L.PREC_BF16 if self.precision == L.PREC_BF16 else L.PREC_F32  # split-bf16 is an inference mode
-            pt, ph, pw = spec["patch_shape"]
+            cfg = call["cond_scale"] != 1
+            prec = train_precision(self.precision)
+            pt, ph, pw = call["patch_shape"]
             gtable, gk = self._grad_table(has_cross, owner=owner, head=head)
             try:
                 nbytes = lib.phk_maskgit_backward_workspace_bytes(C.byref(table), b, n, ctx_len, int(cfg), head_kind, prec)
-                ws = self._ws.get(nbytes, dev)
+                ws = self._ws.get_for("phk_maskgit_backward_workspace_bytes", nbytes, dev)
                 d_context = torch.zeros_like(context) if has_cross and want_context_grad else None
                 L.check(lib.phk_maskgit_backward(C.byref(table), C.byref(gtable), L.ptr(ids), b, n, pt, ph, pw,
                                                  L.ptr(context), ctx_len, L.ptr(text_mask), L.ptr(video_mask), int(cfg),
-                                                 spec["cond_scale"], head_kind, L.ptr(upstream), L.ptr(d_context),
+                                                 call["cond_scale"], head_kind, L.ptr(upstream), L.ptr(d_context),
                                                  L.ptr(ws), ws.numel(), prec, L.stream_ptr()),
                         "phk_maskgit_backward")
                 # the embeddings head leaves the network's own head out of the graph, as the reference's autograd does
@@ -410,7 +405,7 @@ class _TokenTransformer(nn.Module):
                     grads.append(None if g is None or p in unused else g.clone())
             finally:
                 gk.busy = False
-        return grads, d_context
+        return [d_context], grads
 
     def _check_ids(self, x):
         """nn.Embedding raises on an id outside the table (phenaki_pytorch.py:194); the kernels only clamp.  One device
@@ -464,7 +459,7 @@ class MaskGit(_TokenTransformer):
     def forward(self, x, cond_drop_prob=0.0, text_mask=None, video_mask=None, video_patch_shape=None,
                 return_embeds=False, context=None, **kwargs):
         """phenaki_pytorch.py:163-213: logits (b, n, V), or the embeddings (b, n, dim) with ``return_embeds``.
-        Differentiable with respect to the parameters and ``context`` (``_ForwardBackwardFn``: the backward recomputes
+        Differentiable with respect to the parameters and ``context`` (``recompute_in_backward``: the backward recomputes
         the forward with saved activations, so it costs one training forward plus the backward).  Training-mode
         dropout is not applied, here or in the backward (DESIGN.md section 8)."""
         assert x.ndim in {2, 4}, "video token ids must be of shape (batch, seq) or (batch, frame, height, width)"
@@ -645,9 +640,8 @@ class _TrainStepFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, gout):
-        if ctx.needs_input_grad[3] and torch.is_grad_enabled():
-            raise RuntimeError("Phenaki.forward does not support create_graph=True with text embeddings that require grad: "
-                               "the training step's backward is hand-written CUDA and builds no graph of its own")
+        if ctx.needs_input_grad[3]:
+            refuse_create_graph("Phenaki.forward with text embeddings that require grad")
         if ctx.sync:  # data parallel: average the one flat gradient bucket over the ranks (DDP's all-reduce)
             reduced = getattr(ctx.keep, "reduced", None)
             if reduced is not None:  # already launched slice by slice on the side stream, overlapped with the backward
@@ -659,32 +653,6 @@ class _TrainStepFn(torch.autograd.Function):
         out = (None, None, None, d_context, *[None if g is None else g * gout for g in ctx.grads])  # copies: the bucket is free again
         ctx.keep.busy = False
         return out
-
-
-class _ForwardBackwardFn(torch.autograd.Function):
-    """Makes the MaskGit / TokenCritic / SelfCritic forwards differentiable.  The forward runs the library's inference
-    forward unchanged (same launches, same values) and keeps only the call's inputs.  The backward recomputes the forward
-    with saved activations inside phk_maskgit_backward, as activation checkpointing does, and runs the hand-written
-    backward from the upstream gradient: a backward costs one training forward plus the backward of the training step.
-    Training-mode dropout is not applied by these forwards (DESIGN.md section 8), so the backward applies none either:
-    it differentiates the function the forward returned."""
-
-    @staticmethod
-    def forward(ctx, run, spec, ids, text_mask, video_mask, context, *params):
-        ctx.spec = spec
-        ctx.save_for_backward(ids, text_mask, video_mask, None if context is None else context.detach())
-        return run()
-
-    @staticmethod
-    def backward(ctx, gout):
-        if torch.is_grad_enabled():
-            raise RuntimeError("MaskGit / TokenCritic / SelfCritic forwards do not support create_graph=True: their "
-                               "backward is hand-written CUDA and builds no graph of its own")
-        ids, text_mask, video_mask, context = ctx.saved_tensors
-        spec = ctx.spec
-        grads, d_context = spec["net"]._backward_from(spec, gout, ids, text_mask, video_mask, context,
-                                                      ctx.needs_input_grad[5])
-        return (None, None, None, None, None, d_context, *grads)
 
 
 def get_mask_subset_with_prob(mask, prob, u=None):
@@ -953,7 +921,7 @@ class Phenaki(nn.Module):
                 head_w, head_b = L.ptr(keep[0]), L.ptr(keep[1])
             cref = C.byref(ctable) if ctable is not None else None
             nbytes = lib.phk_maskgit_demask_iteration_workspace_bytes(C.byref(table), cref, b, plen + n, ctx_len)
-            ws = mg._ws.get(nbytes, dev)
+            ws = mg._ws.get_for("phk_maskgit_demask_iteration_workspace_bytes", nbytes, dev)
             bias = mg._pos_bias(table, patch_shape, dev)
             pt, ph, pw = (int(v) for v in patch_shape)
             inp = bufs["inp"] if plen else bufs["ids"]
