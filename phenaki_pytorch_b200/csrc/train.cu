@@ -302,21 +302,31 @@ __global__ void __launch_bounds__(256) cast_transpose_bf16_kernel(const float* _
 struct TcScratch { __nv_bfloat16* a; __nv_bfloat16* b; int64_t elems; };  // two operand buffers of `elems` bf16 each
 inline int64_t pad8(int64_t v) { return (v + 7) / 8 * 8; }
 
-int cast_to(const float* src, int64_t rows, int64_t cols, bool transpose, __nv_bfloat16* dst, int64_t cap, int64_t* ld,
-            cudaStream_t st) {
+// src [rows, cols] (transpose: its transpose) as bf16 with the leading dimension padded to 8 elements
+int cast_check(int64_t rows, int64_t cols, bool transpose, int64_t cap, int64_t* ld) {
   PHK_REQUIRE(rows > 0 && cols > 0 && cols < (1LL << 31), PHK_E_ARG, "train: bad operand shape");
+  *ld = pad8(transpose ? rows : cols);
+  PHK_REQUIRE((transpose ? cols : rows) * *ld <= cap, PHK_E_WORKSPACE, "train: tensor-core operand scratch too small");
+  PHK_REQUIRE(!transpose || (rows + 31) / 32 <= 65535, PHK_E_UNSUPPORTED, "train: operand too tall for the transposing cast");
+  return 0;
+}
+int cast_to(const float* src, int64_t rows, int64_t cols, bool transpose, __nv_bfloat16* dst, int64_t ld, cudaStream_t st) {
   if (!transpose) {
-    *ld = pad8(cols);
-    PHK_REQUIRE(rows * *ld <= cap, PHK_E_WORKSPACE, "train: tensor-core operand scratch too small");
-    PHK_KERNEL_LAUNCH(cast_bf16_kernel, dim3(ew_grid_fwd(rows * cols)), dim3(256), (size_t)(0), st, src, rows, (int)cols, dst, *ld);
+    PHK_KERNEL_LAUNCH(cast_bf16_kernel, dim3(ew_grid_fwd(rows * cols)), dim3(256), (size_t)(0), st, src, rows, (int)cols, dst, ld);
   } else {
-    *ld = pad8(rows);
-    PHK_REQUIRE(cols * *ld <= cap, PHK_E_WORKSPACE, "train: tensor-core operand scratch too small");
-    PHK_REQUIRE((rows + 31) / 32 <= 65535, PHK_E_UNSUPPORTED, "train: operand too tall for the transposing cast");
-    PHK_KERNEL_LAUNCH(cast_transpose_bf16_kernel, dim3((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32)), dim3(256), (size_t)(0), st, src, rows, (int)cols, dst, *ld);
+    PHK_KERNEL_LAUNCH(cast_transpose_bf16_kernel, dim3((unsigned)((cols + 31) / 32), (unsigned)((rows + 31) / 32)), dim3(256), (size_t)(0), st, src, rows, (int)cols, dst, ld);
   }
   PHK_LAUNCH_CHECK();
   return 0;
+}
+// both operands of one product into tc.a / tc.b: both are checked before either cast launches, so that a refused call
+// leaves no work behind
+int cast_operands(const TcScratch& tc, const float* a, int64_t ar, int64_t ac, bool at, int64_t* lda, const float* b,
+                  int64_t br, int64_t bc, bool bt, int64_t* ldb, cudaStream_t st) {
+  PHK_TRY(cast_check(ar, ac, at, tc.elems, lda));
+  PHK_TRY(cast_check(br, bc, bt, tc.elems, ldb));
+  PHK_TRY(cast_to(a, ar, ac, at, tc.a, *lda, st));
+  return cast_to(b, br, bc, bt, tc.b, *ldb, st);
 }
 
 // Y[M,N] = X[M,K].W[N,K]^T (+bias) (+residual: `residual` must be Y itself, i.e. Y already holds the residual)
@@ -325,8 +335,7 @@ int linear_fwd(int prec, const TcScratch& tc, const float* X, const float* W, fl
   if (prec != PHK_PREC_BF16)
     return phk_gemm_f32(X, K, W, K, Y, N, M, (int32_t)N, (int32_t)K, bias, residual, 0, 0, 0, s);
   int64_t lda = 0, ldw = 0;
-  PHK_TRY(cast_to(X, M, K, false, tc.a, tc.elems, &lda, to_stream(s)));
-  PHK_TRY(cast_to(W, N, K, false, tc.b, tc.elems, &ldw, to_stream(s)));
+  PHK_TRY(cast_operands(tc, X, M, K, false, &lda, W, N, K, false, &ldw, to_stream(s)));
   if (residual && residual != Y) PHK_CUDA(cudaMemcpyAsync(Y, residual, M * N * 4, cudaMemcpyDeviceToDevice, to_stream(s)));
   return phk_gemm_bf16(tc.a, lda, tc.b, ldw, Y, N, M, (int32_t)N, (int32_t)K, bias, residual ? Y : nullptr, 0, 0, 0, 0, s);
 }
@@ -335,8 +344,7 @@ int dgrad_p(int prec, const TcScratch& tc, const float* dY, const float* W, floa
             int accumulate, phk_stream_t s) {
   if (prec != PHK_PREC_BF16) return dgrad(dY, W, dX, M, N, K, accumulate, to_stream(s));
   int64_t lda = 0, ldw = 0;
-  PHK_TRY(cast_to(dY, M, N, false, tc.a, tc.elems, &lda, to_stream(s)));
-  PHK_TRY(cast_to(W, N, K, true, tc.b, tc.elems, &ldw, to_stream(s)));  // W^T [K, N]
+  PHK_TRY(cast_operands(tc, dY, M, N, false, &lda, W, N, K, true, &ldw, to_stream(s)));  // dY [M, N], W^T [K, N]
   return phk_gemm_bf16(tc.a, lda, tc.b, ldw, dX, K, M, (int32_t)K, (int32_t)N, nullptr, accumulate ? dX : nullptr, 0, 0, 0, 0, s);
 }
 // dW[N,K] += dY[M,N]^T . X[M,K]
@@ -344,8 +352,7 @@ int wgrad_p(int prec, const TcScratch& tc, const float* dY, const float* X, floa
             phk_stream_t s) {
   if (prec != PHK_PREC_BF16) return wgrad(dY, X, dW, M, N, K, to_stream(s));
   int64_t lda = 0, ldw = 0;
-  PHK_TRY(cast_to(dY, M, N, true, tc.a, tc.elems, &lda, to_stream(s)));  // dY^T [N, M]
-  PHK_TRY(cast_to(X, M, K, true, tc.b, tc.elems, &ldw, to_stream(s)));   // X^T  [K, M]
+  PHK_TRY(cast_operands(tc, dY, M, N, true, &lda, X, M, K, true, &ldw, to_stream(s)));  // dY^T [N, M], X^T [K, M]
   return phk_gemm_bf16(tc.a, lda, tc.b, ldw, dW, K, N, (int32_t)K, (int32_t)M, nullptr, dW, 0, 0, 0, 0, s);
 }
 
@@ -757,10 +764,27 @@ __global__ void attn_bwd_dbias_kernel(const float* __restrict__ dS, float* __res
   }
 }
 
-struct AttnBwdBufs { float *qh, *kh, *vv, *P, *dS; };
+// The attention backward's scratch, per (sequence, head): qh [n, dh], kh and vv [nkt, dh], P and dS [n, nkt], then the
+// batched-product outputs preQ = dS.kh [n, dh], preK = dS^T.qh and preV = P^T.dO [nkt, dh].  attention_forward_dropout
+// uses the first four.
+struct AttnBwdBufs { float *qh, *kh, *vv, *P, *dS, *preQ, *preK, *preV; };
+
+AttnBwdBufs attn_bwd_bufs(float* scratch, const AttnBwdGeom& g) {
+  const int64_t bh = (int64_t)g.b * g.H, nkt = g.nnull + g.m;
+  AttnBwdBufs B;
+  B.qh = scratch;
+  B.kh = B.qh + bh * g.n * g.dh;
+  B.vv = B.kh + bh * nkt * g.dh;
+  B.P = B.vv + bh * nkt * g.dh;
+  B.dS = B.P + bh * g.n * nkt;
+  B.preQ = B.dS + bh * g.n * nkt;
+  B.preK = B.preQ + bh * g.n * g.dh;
+  B.preV = B.preK + bh * nkt * g.dh;
+  return B;
+}
 
 int64_t attn_bwd_scratch_floats(int b, int H, int n, int nkt, int dh) {
-  // qh, kh, vv, P, dS + the batched-product outputs dS.kh [n, dh], dS^T.qh and P^T.dO [nkt, dh]
+  // everything attn_bwd_bufs carves: 2 [n, dh] + 4 [nkt, dh] + 2 [n, nkt] per (sequence, head)
   return (int64_t)b * H * (2 * (int64_t)n * dh + 4 * (int64_t)nkt * dh + 2 * (int64_t)n * nkt) + 64;
 }
 
@@ -772,12 +796,7 @@ int attention_backward(const float* q, const float* kv, const phk_attn_t& A, con
   PHK_REQUIRE(g.nnull == 0 || (A.null_kv && G.null_kv), PHK_E_ARG, "train: null_kv (gradient) missing");
   const int nkt = g.nnull + g.m;
   const int64_t bh = (int64_t)g.b * g.H;
-  AttnBwdBufs B;
-  B.qh = scratch;
-  B.kh = B.qh + bh * g.n * g.dh;
-  B.vv = B.kh + bh * nkt * g.dh;
-  B.P = B.vv + bh * nkt * g.dh;
-  B.dS = B.P + bh * g.n * nkt;
+  const AttnBwdBufs B = attn_bwd_bufs(scratch, g);
   const int64_t prep_warps = bh * (g.n + nkt);
   PHK_KERNEL_LAUNCH(attn_bwd_prep_kernel, dim3((unsigned)((prep_warps + 7) / 8)), dim3(256), (size_t)(0), st, q, kv, A.null_kv, A.q_scale, A.k_scale, B.qh, B.kh,
                                                                         B.vv, g);
@@ -796,9 +815,9 @@ int attention_backward(const float* q, const float* kv, const phk_attn_t& A, con
   // kernels walk a column of dS / P with a stride of nkt floats: 1.5 ms per layer at n = 576), loops for short ones
   float* preQ = nullptr; float* preK = nullptr; float* preV = nullptr;
   if ((int64_t)g.n * nkt >= 64 * 64) {
-    preQ = B.dS + bh * g.n * nkt;
-    preK = preQ + bh * g.n * g.dh;
-    preV = preK + bh * nkt * g.dh;
+    preQ = B.preQ;
+    preK = B.preK;
+    preV = B.preV;
     const GemmBatch bq{(int)bh, 1, (int64_t)g.n * nkt, 0, (int64_t)nkt * g.dh, 0, (int64_t)g.n * g.dh, 0};
     PHK_TRY(sgemm_batched(B.dS, nkt, 1, B.kh, g.dh, 1, preQ, g.dh, g.n, g.dh, nkt, 0, bq, st, bf16_products));  // dS . kh
     const GemmBatch bk{(int)bh, 1, (int64_t)g.n * nkt, 0, (int64_t)g.n * g.dh, 0, (int64_t)nkt * g.dh, 0};
@@ -830,10 +849,8 @@ int attention_forward_dropout(const float* q, const float* kv, const phk_attn_t&
   PHK_REQUIRE(g.nnull == 0 || A.null_kv, PHK_E_ARG, "train: null_kv missing");
   const int nkt = g.nnull + g.m;
   const int64_t bh = (int64_t)g.b * g.H;
-  float* qh = scratch;
-  float* kh = qh + bh * g.n * g.dh;
-  float* vv = kh + bh * nkt * g.dh;
-  float* P = vv + bh * nkt * g.dh;
+  const AttnBwdBufs B = attn_bwd_bufs(scratch, g);
+  float *qh = B.qh, *kh = B.kh, *vv = B.vv, *P = B.P;
   const int64_t prep_warps = bh * (g.n + nkt);
   PHK_KERNEL_LAUNCH(attn_bwd_prep_kernel, dim3((unsigned)((prep_warps + 7) / 8)), dim3(256), (size_t)(0), st, q, kv, A.null_kv, A.q_scale, A.k_scale, qh, kh, vv, g);
   PHK_LAUNCH_CHECK();

@@ -31,20 +31,24 @@ def _for_emulator(text):
                   r"\1* \2 = reinterpret_cast<\1*>(::emu::S.dyn_smem);", text)
 
 
-def build_emu():
+def build_emu(extra_source=None, lib_path=EMU_LIB):
+    """extra_source: (path, text) of code appended to train.cu's translation unit (test-only wrappers around its
+    internal functions), built into lib_path instead of the shared EMU_LIB."""
     kernel_paths = [os.path.join(CSRC, f) for f in KERNEL_SOURCES]
     deps = SOURCES + kernel_paths + [os.path.join(EMU_DIR, "cuda_emu.h"), os.path.join(ROOT, "include", "phk.h"),
-                                     os.path.abspath(__file__)]
-    if not os.path.exists(EMU_LIB) or any(os.path.getmtime(d) > os.path.getmtime(EMU_LIB) for d in deps):
-        build = os.path.dirname(EMU_LIB)
+                                     os.path.abspath(__file__)] + ([extra_source[0]] if extra_source else [])
+    if not os.path.exists(lib_path) or any(os.path.getmtime(d) > os.path.getmtime(lib_path) for d in deps):
+        build = os.path.dirname(lib_path)
         os.makedirs(build, exist_ok=True)
         rewritten = []
         for path in kernel_paths:
             out = os.path.join(build, f"{os.path.basename(path)}.{os.getpid()}.emu.cpp")
             with open(path) as f, open(out, "w") as g:
                 g.write(_for_emulator(f.read()))
+                if extra_source and os.path.basename(path) == "train.cu":
+                    g.write("\n" + _for_emulator(extra_source[1]))
             rewritten.append(out)
-        tmp = EMU_LIB + f".{os.getpid()}.tmp"
+        tmp = lib_path + f".{os.getpid()}.tmp"
         try:
             san = ["-fsanitize=address", "-fno-omit-frame-pointer", "-g"] if ASAN else []
             subprocess.check_call(["g++", "-O1", "-std=c++17", "-fPIC", "-shared", "-ffp-contract=off", "-U_FORTIFY_SOURCE",
@@ -52,8 +56,8 @@ def build_emu():
         finally:
             for r in rewritten:
                 os.remove(r)
-        os.replace(tmp, EMU_LIB)
-    lib = ctypes.CDLL(EMU_LIB)
+        os.replace(tmp, lib_path)
+    lib = ctypes.CDLL(lib_path)
     for name, argtypes in L.PROTOTYPES.items():
         if not hasattr(lib, name):
             continue  # tensor-core / TMA entry points are not part of the emulated build

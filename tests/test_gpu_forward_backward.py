@@ -6,6 +6,11 @@ every gradient tensor, and d(text_embeds), within 1e-4 of its largest entry (max
 norm); the analytically zero position-bias bias within 1e-6 of the largest gradient; the set of gradients left None is
 the reference's.  bf16 mode is held to the training step's bf16 closeness bars.  The forward itself is unchanged: the
 same values and the same kernel sequence with grad enabled as under no_grad."""
+import json
+import os
+import subprocess
+import sys
+
 import pytest
 import torch
 from torch.profiler import ProfilerActivity, profile
@@ -69,18 +74,31 @@ def test_forward_values_are_unchanged_and_no_grad_builds_no_graph(lib, modules, 
     FG.check_forward_unchanged(lib, DEV, _sync, modules(name), name)
 
 
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
 def _device_ops(fn):
+    """Names of the device ops fn runs, in start order, bracketed by two marker fills: a capture counts only when it
+    begins and ends with a marker, i.e. when the profiler kept every record of the session."""
+    marker = torch.zeros(1, device=DEV)
     _sync()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        marker.fill_(1.0)
         fn()
+        marker.fill_(2.0)
         _sync()
     ops = [e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-    return [e.name for e in sorted(ops, key=lambda e: e.time_range.start)]
+    names = [e.name for e in sorted(ops, key=lambda e: e.time_range.start)]
+    assert len(names) >= 2 and "FillFunctor" in names[0] and "FillFunctor" in names[-1], \
+        f"incomplete profiler capture: {len(names)} ops, {names[:2]} ... {names[-2:]}"
+    return names[1:-1]
 
 
-@pytest.mark.parametrize("name", ["ragged_logits_cfg", "prod_critic", "ragged_self_critic_cfg"])
-def test_forward_kernel_sequence_is_the_same_with_grad_enabled(lib, modules, name):
-    module = modules(name)
+def kernel_sequences(name):
+    """(device ops of the no_grad forward, device ops of the forward with grad enabled) in bf16 mode, after a warm-up
+    of both (position-bias cache, workspace).  Run in a fresh process: late in a long test process the profiler drops
+    the first records of a session (a capture once began at the forward's first device-to-host copy)."""
+    module = T.build_module(FG.ALL_CASES[name]["base"]).to(DEV).train()
     FG.set_precision(module, L.PREC_BF16)
 
     def plain():
@@ -90,8 +108,22 @@ def test_forward_kernel_sequence_is_the_same_with_grad_enabled(lib, modules, nam
     def graphed():
         FG.product_out(name, module, DEV)
 
-    plain(), graphed()  # warm-up: position-bias cache, workspace
-    a, b = _device_ops(plain), _device_ops(graphed)
+    plain(), graphed()
+    return _device_ops(plain), _device_ops(graphed)
+
+
+def _child(fn, *args):
+    code = (f"import json, sys; sys.path.insert(0, {ROOT!r}); from tests import test_gpu_forward_backward as T; "
+            f"print(json.dumps(T.{fn}(*{args!r})))")
+    flags = ["-s"] if sys.flags.no_user_site else []
+    run = subprocess.run([sys.executable, *flags, "-c", code], cwd=ROOT, capture_output=True, text=True, timeout=900)
+    assert run.returncode == 0, run.stderr[-4000:]
+    return json.loads(run.stdout.strip().splitlines()[-1])
+
+
+@pytest.mark.parametrize("name", ["ragged_logits_cfg", "prod_critic", "ragged_self_critic_cfg"])
+def test_forward_kernel_sequence_is_the_same_with_grad_enabled(name):
+    a, b = _child("kernel_sequences", name)
     assert a and a == b, f"{name}: no_grad forward ran {len(a)} device ops, the graphed forward {len(b)}"
 
 
