@@ -700,6 +700,17 @@ int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_t* grads, c
  * transformer layer depth-1-k, events[depth + 1] embeddings + position-bias MLP (= all).  If the next such call is
  * phk_cvivit_backward instead, it records them in its own group order (see there).  One-shot; NULL clears. */
 int phk_train_set_progress_events(void** events, int32_t count);
+/* Deterministic mode of the calling thread (what torch.use_deterministic_algorithms(True) asks for); returns the previous
+ * mode.  It is read by phk_maskgit_train_step, phk_maskgit_backward, phk_cvivit_decode_backward,
+ * phk_cvivit_encode_backward and phk_cvivit_backward, and by their *_workspace_bytes queries, at each call.
+ *   0 (default)  the gradient reductions across CTAs use float atomics: two calls can differ in the last bits.
+ *   1            every reduction adds its partial sums in an order fixed by the call's shapes (and, for the token
+ *                embedding, its ids), so every gradient the call writes or accumulates is bit-identical across calls with
+ *                the same inputs, shapes, precision mode and device type.  The partial sums live in the workspace: the
+ *                queries return more in this mode, and a call made in it needs the size the query returned in it.
+ * Progress events keep their meaning: a group's partial sums are added before its event is recorded.  Across ranks, the
+ * sum of the local gradients is left to the collective. */
+int32_t phk_train_set_deterministic(int32_t on);
 
 /* Backward of a MaskGit / TokenCritic / SelfCritic forward from a gradient the caller supplies: what
  * `out = module(ids, ...); out.backward(upstream)` computes for the parameters (and the text embeddings) under torch

@@ -127,6 +127,7 @@ PROTOTYPES = {
     "phk_attention_small_bf16": [vp, vp, vp, vp, C.POINTER(AttnGeomT), vp],
     "phk_attention_mid_bf16": [vp, i64, vp, i64, vp, vp, i32, i32, i32, vp],
     "phk_train_set_progress_events": [vp, i32],
+    "phk_train_set_deterministic": [i32],
     "phk_split3": [vp, i64, vp, i64, i32, i32, vp],
     "phk_cross_kv_pack": [vp, vp, vp, i32, vp, i32, i32, i32, i32, vp, vp, vp],
     "phk_gemm_bf16_qnorm": [vp, i64, vp, i64, vp, i64, i32, i32, vp, f32, vp],
@@ -234,6 +235,14 @@ def check(rc, what=""):
     if rc == -2:
         raise AssertionError(f"{what}: {msg}")
     raise PhkError(f"{what}: {msg} (code {rc})")
+
+
+def sync_deterministic():
+    """Sets the library's deterministic mode (phk_train_set_deterministic) of the calling thread to
+    ``torch.are_deterministic_algorithms_enabled()``.  The mode is per thread and autograd runs a backward on a thread of
+    its own, so each backward calls this right before its workspace query and its library call.  ``warn_only=True``
+    counts as on: the library has no nondeterministic path left to warn about."""
+    lib().phk_train_set_deterministic(int(torch.are_deterministic_algorithms_enabled()))
 
 
 def stream_ptr():

@@ -31,6 +31,71 @@ constexpr float kLnEps = 1e-5f;
 constexpr float kL2Eps = 1e-12f;
 
 // ------------------------------------------------------------------------------------------------------------------
+// Deterministic mode (include/phk.h, phk_train_set_deterministic; DESIGN.md section 7.6).  Every reduction that the
+// default path finishes with float atomics -- split-K wgrad, bias column sums, LayerNorm gamma / beta, q_scale / k_scale,
+// null_kv, the PEG weights, the embeddings and the position-bias table -- then writes per-CTA partial sums to fixed slots
+// of a scratch region and adds the slots into the gradient in slot order, or gathers its terms in index order.  Every
+// summation order is a function of the call's shapes (and, for the token embedding, of the ids) alone.
+// The entry point carves the region from the call's workspace and publishes it in t_det for the duration of the call;
+// t_det.p == NULL is the default path.  The reductions run one after another on the call's stream, so each one uses
+// the region from its start.
+// ------------------------------------------------------------------------------------------------------------------
+thread_local int32_t t_det_mode = 0;             // phk_train_set_deterministic: read by the backward entry points
+struct DetScratch { float* p; int64_t floats; };
+thread_local DetScratch t_det{nullptr, 0};        // the current call's region (NULL: default path)
+
+// Clears t_det when the entry point that published it returns, whichever way it returns.
+struct DetScope {
+  DetScope() = default;
+  DetScope(const DetScope&) = delete;
+  ~DetScope() { t_det = DetScratch{nullptr, 0}; }
+};
+
+constexpr int kDetRows = 256;  // rows per partial sum of colsum_fixed
+inline int64_t det_blocks(int64_t rows) { return (rows + kDetRows - 1) / kDetRows; }
+
+// Fixed-order column sums of x [rows, cols] (leading dimension ld).  CTA (cx, gy) takes 32 columns of the rows
+// [gy * per, (gy + 1) * per): warp w adds rows w, w + 8, ... in order, then the 8 warps are added in order.
+// to_out == 0: the sum is written to out[gy * cols + c]; to_out == 1: it is added to out[c] (gridDim.y == 1).
+__global__ void __launch_bounds__(256) colsum_fixed_kernel(const float* __restrict__ x, int64_t rows, int64_t cols,
+                                                           int64_t ld, int64_t per, float* __restrict__ out, int to_out) {
+  __shared__ float red[8][33];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int64_t c = (int64_t)blockIdx.x * 32 + lane;
+  const int64_t r0 = (int64_t)blockIdx.y * per, r1 = r0 + per < rows ? r0 + per : rows;
+  float a = 0.f;
+  if (c < cols)
+    for (int64_t r = r0 + w; r < r1; r += 8) a += x[r * ld + c];
+  red[w][lane] = a;
+  __syncthreads();
+  if (w == 0 && c < cols) {
+    float s = red[0][lane];
+    for (int k = 1; k < 8; ++k) s += red[k][lane];
+    if (to_out) out[c] += s;
+    else out[(int64_t)blockIdx.y * cols + c] = s;
+  }
+}
+// out[c] += sum_r slots[r, c] for a [nslots, cols] block of partial sums, in one fixed order
+int add_slots(const float* slots, int64_t nslots, int64_t cols, float* out, cudaStream_t st) {
+  PHK_KERNEL_LAUNCH(colsum_fixed_kernel, dim3((unsigned)((cols + 31) / 32), 1), dim3(256), (size_t)(0), st, slots, nslots, cols, cols, nslots, out, 1);
+  PHK_LAUNCH_CHECK();
+  return 0;
+}
+// Floats of scratch colsum_fixed uses for `rows` rows of `cols` columns
+inline int64_t colsum_fixed_floats(int64_t rows, int64_t cols) { return det_blocks(rows) * cols; }
+// out[c] += sum_r x[r, c] in a fixed order: partial sums of kDetRows-row blocks into `scratch` (cap floats), then
+// those partials in block order
+int colsum_fixed(const float* x, int64_t rows, int64_t cols, int64_t ld, float* out, float* scratch, int64_t cap,
+                 cudaStream_t st) {
+  const int64_t G = det_blocks(rows);
+  PHK_REQUIRE(scratch && G * cols <= cap, PHK_E_WORKSPACE, "train: deterministic reduction scratch too small");
+  PHK_REQUIRE(G <= 65535 && (cols + 31) / 32 < (1LL << 31), PHK_E_UNSUPPORTED, "train: column sum too large");
+  PHK_KERNEL_LAUNCH(colsum_fixed_kernel, dim3((unsigned)((cols + 31) / 32), (unsigned)G), dim3(256), (size_t)(0), st, x, rows, cols, ld, (int64_t)kDetRows, scratch, 0);
+  PHK_LAUNCH_CHECK();
+  return add_slots(scratch, G, cols, out, st);
+}
+
+// ------------------------------------------------------------------------------------------------------------------
 // Generic strided fp32 GEMM for the backward products:  C[m, n] (+)= sum_k A(m,k) * B(k,n)
 //   A(m,k) = A[m*sam + k*sak],  B(k,n) = B[k*sbk + n*sbn],  C row-major with leading dimension ldc.
 //   dgrad  dX[M,K'] = dY[M,N'] . W[N',K']   : sam=N', sak=1, sbk=K', sbn=1
@@ -231,10 +296,20 @@ int wgrad(const float* dY, const float* X, float* dW, int64_t M, int64_t N, int6
   if (N * K <= 4 * GB * GB && M >= 1024) {
     const int64_t chunk = 256;
     const int parts = (int)((M + chunk - 1) / chunk);
+    if (t_det.p) {  // deterministic mode: slice z writes its [N, K] product to slot z, the slots are added in order
+      PHK_REQUIRE(parts * N * K <= t_det.floats, PHK_E_WORKSPACE, "train: deterministic reduction scratch too small");
+      const GemmBatch gb{parts, 1, chunk * N, 0, chunk * K, 0, N * K, 0, (int)M};
+      PHK_TRY(sgemm_batched(dY, 1, N, X, K, 1, t_det.p, K, N, K, chunk, 0, gb, st));
+      return add_slots(t_det.p, parts, N * K, dW, st);
+    }
     const GemmBatch gb{parts, 1, chunk * N, 0, chunk * K, 0, 0, 0, (int)M};
     return sgemm_batched(dY, 1, N, X, K, 1, dW, K, N, K, chunk, 2, gb, st);
   }
   return sgemm(dY, 1, N, X, K, 1, dW, K, N, K, M, 1, st);
+}
+// Deterministic-mode scratch of wgrad: the split-K slots (0 when the product is not split)
+int64_t wgrad_det_floats(int64_t M, int64_t N, int64_t K) {
+  return (N * K <= 4 * GB * GB && M >= 1024) ? (M + 255) / 256 * N * K : 0;
 }
 inline unsigned ew_grid_fwd(int64_t total) {
   const int64_t b = (total + 255) / 256;
@@ -253,6 +328,7 @@ __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x
   if (r1 > r0) atomicAdd(out + c, a);
 }
 int colsum(const float* x, int64_t rows, int cols, int64_t ld, float* out, cudaStream_t st) {
+  if (t_det.p) return colsum_fixed(x, rows, cols, ld, out, t_det.p, t_det.floats, st);
   int chunks = (int)((rows + 63) / 64);
   if (chunks > 64) chunks = 64;
   if (chunks < 1) chunks = 1;
@@ -414,11 +490,51 @@ __global__ void __launch_bounds__(256) ln_bwd_dgb_kernel(const float* __restrict
   }
 }
 
+// Deterministic mode: the column kernel's sums over kDetRows-row blocks, in colsum_fixed_kernel's order, into
+// part_g / part_b [gridDim.y, dim]
+__global__ void __launch_bounds__(256) ln_bwd_dgb_fixed_kernel(const float* __restrict__ x, const float* __restrict__ dy,
+                                                               const float2* __restrict__ stats, int64_t rows, int dim,
+                                                               float* __restrict__ part_g, float* __restrict__ part_b) {
+  __shared__ float rg[8][33], rb[8][33];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  const int c = blockIdx.x * 32 + lane;
+  const int64_t r0 = (int64_t)blockIdx.y * kDetRows, r1 = r0 + kDetRows < rows ? r0 + kDetRows : rows;
+  float ag = 0.f, ab = 0.f;
+  if (c < dim)
+    for (int64_t r = r0 + w; r < r1; r += 8) {
+      const float2 s = stats[r];
+      const float d = dy[r * dim + c];
+      ag += d * (x[r * dim + c] - s.x) * s.y;
+      ab += d;
+    }
+  rg[w][lane] = ag;
+  rb[w][lane] = ab;
+  __syncthreads();
+  if (w == 0 && c < dim) {
+    float sg = rg[0][lane], sb = rb[0][lane];
+    for (int k = 1; k < 8; ++k) { sg += rg[k][lane]; sb += rb[k][lane]; }
+    part_g[(int64_t)blockIdx.y * dim + c] = sg;
+    if (part_b) part_b[(int64_t)blockIdx.y * dim + c] = sb;
+  }
+}
+inline int64_t ln_det_floats(int64_t rows, int64_t dim) { return 2 * det_blocks(rows) * dim; }
+
 // dx (+)= LN_bwd(x; g)(dy); dgamma += ..; dbeta += .. (dbeta NULL: the custom LayerNorm's beta is a buffer)
 int ln_backward(const float* x, const float* g, const float* dy, float* dx, int accumulate, float* dgamma, float* dbeta,
                 float2* stats, int64_t rows, int dim, cudaStream_t st) {
   PHK_KERNEL_LAUNCH(ln_bwd_dx_kernel, dim3((unsigned)((rows + 7) / 8)), dim3(256), (size_t)(0), st, x, g, dy, dx, stats, rows, dim, accumulate);
   PHK_LAUNCH_CHECK();
+  if (t_det.p) {
+    const int64_t G = det_blocks(rows);
+    PHK_REQUIRE(ln_det_floats(rows, dim) <= t_det.floats, PHK_E_WORKSPACE, "train: deterministic reduction scratch too small");
+    PHK_REQUIRE(G <= 65535, PHK_E_UNSUPPORTED, "train: LayerNorm backward too tall");
+    float* pg = t_det.p;
+    float* pb = dbeta ? t_det.p + G * dim : nullptr;
+    PHK_KERNEL_LAUNCH(ln_bwd_dgb_fixed_kernel, dim3((unsigned)((dim + 31) / 32), (unsigned)G), dim3(256), (size_t)(0), st, x, dy, (const float2*)stats, rows, dim, pg, pb);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(add_slots(pg, G, dim, dgamma, st));
+    return dbeta ? add_slots(pb, G, dim, dbeta, st) : 0;
+  }
   int chunks = (int)((rows + 63) / 64);
   if (chunks > 64) chunks = 64;
   PHK_KERNEL_LAUNCH(ln_bwd_dgb_kernel, dim3((unsigned)((dim + 255) / 256), (unsigned)chunks), dim3(256), (size_t)(0), st, x, dy, stats, rows, dim, dgamma,
@@ -636,10 +752,12 @@ constexpr int kDPL = 4;  // dim_head <= 128
 // one warp per (sequence, head, query): dqh = 8 * sum_j dS[i,j] kh[j,:]; 8 warps per CTA share one dq_scale reduction
 // `pre` (optional): dS.kh already computed as a batched register-tiled product [b*H, n, dh] (long sequences: the warp-per-
 // row loop below re-reads the whole key block per query)
-__global__ void __launch_bounds__(256) attn_bwd_dq_kernel(const float* __restrict__ q, const float* __restrict__ kh,
-                                                          const float* __restrict__ dS, const float* __restrict__ q_scale,
-                                                          float* __restrict__ dq, float* __restrict__ dq_scale,
-                                                          const float* __restrict__ pre, AttnBwdGeom g) {
+// scale_part (deterministic mode, else NULL): the CTA's q_scale sum goes to its slot blockIdx.x instead of dq_scale
+__device__ __forceinline__ void attn_bwd_dq_body(const float* __restrict__ q, const float* __restrict__ kh,
+                                                 const float* __restrict__ dS, const float* __restrict__ q_scale,
+                                                 float* __restrict__ dq, float* __restrict__ dq_scale,
+                                                 const float* __restrict__ pre, float* __restrict__ scale_part,
+                                                 const AttnBwdGeom& g) {
   __shared__ float red[8][32 * kDPL];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int nkt = g.nnull + g.m;
@@ -679,18 +797,35 @@ __global__ void __launch_bounds__(256) attn_bwd_dq_kernel(const float* __restric
   if (threadIdx.x < g.dh) {
     float a = 0.f;
     for (int k = 0; k < 8; ++k) a += red[k][threadIdx.x];
-    atomicAdd(dq_scale + threadIdx.x, a);
+    if (scale_part) scale_part[(int64_t)blockIdx.x * g.dh + threadIdx.x] = a;
+    else atomicAdd(dq_scale + threadIdx.x, a);
   }
+}
+__global__ void __launch_bounds__(256) attn_bwd_dq_kernel(const float* __restrict__ q, const float* __restrict__ kh,
+                                                          const float* __restrict__ dS, const float* __restrict__ q_scale,
+                                                          float* __restrict__ dq, float* __restrict__ dq_scale,
+                                                          const float* __restrict__ pre, AttnBwdGeom g) {
+  attn_bwd_dq_body(q, kh, dS, q_scale, dq, dq_scale, pre, nullptr, g);
+}
+__global__ void __launch_bounds__(256) attn_bwd_dq_fixed_kernel(const float* __restrict__ q, const float* __restrict__ kh,
+                                                                const float* __restrict__ dS,
+                                                                const float* __restrict__ q_scale, float* __restrict__ dq,
+                                                                const float* __restrict__ pre,
+                                                                float* __restrict__ scale_part, AttnBwdGeom g) {
+  attn_bwd_dq_body(q, kh, dS, q_scale, dq, nullptr, pre, scale_part, g);
 }
 
 // one warp per (sequence, head, key j in [0, nkt)): dkh = 8 * sum_i dS[i,j] qh[i,:], dvv = sum_i P[i,j] dO[i,:]
-__global__ void __launch_bounds__(256) attn_bwd_dkv_kernel(const float* __restrict__ kv, const float* __restrict__ null_kv,
-                                                           const float* __restrict__ qh, const float* __restrict__ dO,
-                                                           const float* __restrict__ P, const float* __restrict__ dS,
-                                                           const float* __restrict__ k_scale, float* __restrict__ dkv,
-                                                           float* __restrict__ dnull_kv, float* __restrict__ dk_scale,
-                                                           const float* __restrict__ preK, const float* __restrict__ preV,
-                                                           AttnBwdGeom g) {
+// scale_part / null_part (deterministic mode, else NULL): the CTA's k_scale sum goes to its slot blockIdx.x, and the
+// null keys / values of sequence bi to slot bi, instead of dk_scale / dnull_kv
+__device__ __forceinline__ void attn_bwd_dkv_body(const float* __restrict__ kv, const float* __restrict__ null_kv,
+                                                  const float* __restrict__ qh, const float* __restrict__ dO,
+                                                  const float* __restrict__ P, const float* __restrict__ dS,
+                                                  const float* __restrict__ k_scale, float* __restrict__ dkv,
+                                                  float* __restrict__ dnull_kv, float* __restrict__ dk_scale,
+                                                  const float* __restrict__ preK, const float* __restrict__ preV,
+                                                  const AttnBwdGeom& g, float* __restrict__ scale_part,
+                                                  float* __restrict__ null_part) {
   __shared__ float red[8][32 * kDPL];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int nkt = g.nnull + g.m;
@@ -729,11 +864,18 @@ __global__ void __launch_bounds__(256) attn_bwd_dkv_kernel(const float* __restri
     float draw[kDPL];
     l2norm_scale_bwd<kDPL>(raw, k_scale, ak, g.dh, lane, draw, dsc);
     if (j < g.nnull) {  // the null keys / values are parameters shared by every sequence: accumulate over the batch
-      float* nk = dnull_kv + ((int64_t)h * 2 * g.nnull + 2 * j) * g.dh;
+      const int64_t nidx = ((int64_t)h * 2 * g.nnull + 2 * j) * g.dh;
+      if (null_part) {  // deterministic mode: sequence bi's terms to slot bi
+        float* nk = null_part + (int64_t)bi * g.H * 2 * g.nnull * g.dh + nidx;
 #pragma unroll
-      for (int c = 0; c < kDPL; ++c) {
-        const int d = lane + 32 * c;
-        if (d < g.dh) { atomicAdd(nk + d, draw[c]); atomicAdd(nk + g.dh + d, av[c]); }
+        for (int c = 0; c < kDPL; ++c) { const int d = lane + 32 * c; if (d < g.dh) { nk[d] = draw[c]; nk[g.dh + d] = av[c]; } }
+      } else {
+        float* nk = dnull_kv + nidx;
+#pragma unroll
+        for (int c = 0; c < kDPL; ++c) {
+          const int d = lane + 32 * c;
+          if (d < g.dh) { atomicAdd(nk + d, draw[c]); atomicAdd(nk + g.dh + d, av[c]); }
+        }
       }
     } else {
       float* out = dkv + ((int64_t)bi * g.m + (j - g.nnull)) * 2 * I + (int64_t)h * g.dh;
@@ -747,8 +889,29 @@ __global__ void __launch_bounds__(256) attn_bwd_dkv_kernel(const float* __restri
   if (threadIdx.x < g.dh) {
     float a = 0.f;
     for (int k = 0; k < 8; ++k) a += red[k][threadIdx.x];
-    atomicAdd(dk_scale + threadIdx.x, a);
+    if (scale_part) scale_part[(int64_t)blockIdx.x * g.dh + threadIdx.x] = a;
+    else atomicAdd(dk_scale + threadIdx.x, a);
   }
+}
+__global__ void __launch_bounds__(256) attn_bwd_dkv_kernel(const float* __restrict__ kv, const float* __restrict__ null_kv,
+                                                           const float* __restrict__ qh, const float* __restrict__ dO,
+                                                           const float* __restrict__ P, const float* __restrict__ dS,
+                                                           const float* __restrict__ k_scale, float* __restrict__ dkv,
+                                                           float* __restrict__ dnull_kv, float* __restrict__ dk_scale,
+                                                           const float* __restrict__ preK, const float* __restrict__ preV,
+                                                           AttnBwdGeom g) {
+  attn_bwd_dkv_body(kv, null_kv, qh, dO, P, dS, k_scale, dkv, dnull_kv, dk_scale, preK, preV, g, nullptr, nullptr);
+}
+__global__ void __launch_bounds__(256) attn_bwd_dkv_fixed_kernel(const float* __restrict__ kv,
+                                                                 const float* __restrict__ null_kv,
+                                                                 const float* __restrict__ qh, const float* __restrict__ dO,
+                                                                 const float* __restrict__ P, const float* __restrict__ dS,
+                                                                 const float* __restrict__ k_scale, float* __restrict__ dkv,
+                                                                 const float* __restrict__ preK,
+                                                                 const float* __restrict__ preV, AttnBwdGeom g,
+                                                                 float* __restrict__ scale_part,
+                                                                 float* __restrict__ null_part) {
+  attn_bwd_dkv_body(kv, null_kv, qh, dO, P, dS, k_scale, dkv, nullptr, nullptr, preK, preV, g, scale_part, null_part);
 }
 
 // dbias[h, i, j] += sum_b dS[b, h, i, nnull + j]   (self-attention position bias, shared by batch and layers)
@@ -781,6 +944,15 @@ AttnBwdBufs attn_bwd_bufs(float* scratch, const AttnBwdGeom& g) {
   B.preK = B.preQ + bh * g.n * g.dh;
   B.preV = B.preK + bh * nkt * g.dh;
   return B;
+}
+
+// Deterministic-mode scratch of attention_backward: the larger of the dq kernel's slots and the dkv kernel's (k_scale and
+// null_kv), each followed by colsum_fixed's partials over its CTA slots
+int64_t attn_bwd_det_floats(const AttnBwdGeom& g) {
+  const int64_t bh = (int64_t)g.b * g.H, nq = (bh * g.n + 7) / 8, nk = (bh * (g.nnull + g.m) + 7) / 8;
+  const int64_t fq = nq * g.dh + colsum_fixed_floats(nq, g.dh);
+  const int64_t fk = nk * g.dh + (int64_t)g.b * g.H * 2 * g.nnull * g.dh + colsum_fixed_floats(nk, g.dh);
+  return fq > fk ? fq : fk;
 }
 
 int64_t attn_bwd_scratch_floats(int b, int H, int n, int nkt, int dh) {
@@ -826,11 +998,31 @@ int attention_backward(const float* q, const float* kv, const phk_attn_t& A, con
                        (int64_t)g.H * nkt * g.dh, (int64_t)nkt * g.dh};
     PHK_TRY(sgemm_batched(B.P, 1, nkt, dO, I, 1, preV, g.dh, nkt, g.dh, g.n, 0, bv, st, bf16_products));     // P^T . dO
   }
-  PHK_KERNEL_LAUNCH(attn_bwd_dq_kernel, dim3((unsigned)((bh * g.n + 7) / 8)), dim3(256), (size_t)(0), st, q, B.kh, B.dS, A.q_scale, dq, (float*)G.q_scale, (const float*)preQ, g);
-  PHK_LAUNCH_CHECK();
-  PHK_KERNEL_LAUNCH(attn_bwd_dkv_kernel, dim3((unsigned)((bh * nkt + 7) / 8)), dim3(256), (size_t)(0), st, kv, A.null_kv, B.qh, dO, B.P, B.dS, A.k_scale, dkv,
-                                                                     (float*)G.null_kv, (float*)G.k_scale, (const float*)preK, (const float*)preV, g);
-  PHK_LAUNCH_CHECK();
+  const int64_t nq = (bh * g.n + 7) / 8, nk = (bh * nkt + 7) / 8;  // CTAs of the dq and dkv kernels
+  if (t_det.p) {
+    // deterministic mode: each CTA's q_scale / k_scale sum and each sequence's null_kv terms go to their own slots, which
+    // are then added in order (the dq slots are dead before the dkv kernel reuses the region)
+    PHK_REQUIRE(attn_bwd_det_floats(g) <= t_det.floats, PHK_E_WORKSPACE, "train: deterministic reduction scratch too small");
+    float* qs = t_det.p;
+    PHK_KERNEL_LAUNCH(attn_bwd_dq_fixed_kernel, dim3((unsigned)nq), dim3(256), (size_t)(0), st, q, B.kh, B.dS, A.q_scale, dq, (const float*)preQ, qs, g);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(colsum_fixed(qs, nq, g.dh, g.dh, (float*)G.q_scale, qs + nq * g.dh, t_det.floats - nq * g.dh, st));
+    float* ks = t_det.p;
+    float* ns = g.nnull ? ks + nk * g.dh : nullptr;
+    const int64_t nnf = (int64_t)g.H * 2 * g.nnull * g.dh;  // null_kv floats
+    PHK_KERNEL_LAUNCH(attn_bwd_dkv_fixed_kernel, dim3((unsigned)nk), dim3(256), (size_t)(0), st, kv, A.null_kv, B.qh, dO, B.P, B.dS, A.k_scale, dkv,
+                      (const float*)preK, (const float*)preV, g, ks, ns);
+    PHK_LAUNCH_CHECK();
+    if (ns) PHK_TRY(add_slots(ns, g.b, nnf, (float*)G.null_kv, st));
+    const int64_t used = nk * g.dh + (ns ? g.b * nnf : 0);
+    PHK_TRY(colsum_fixed(ks, nk, g.dh, g.dh, (float*)G.k_scale, t_det.p + used, t_det.floats - used, st));
+  } else {
+    PHK_KERNEL_LAUNCH(attn_bwd_dq_kernel, dim3((unsigned)nq), dim3(256), (size_t)(0), st, q, B.kh, B.dS, A.q_scale, dq, (float*)G.q_scale, (const float*)preQ, g);
+    PHK_LAUNCH_CHECK();
+    PHK_KERNEL_LAUNCH(attn_bwd_dkv_kernel, dim3((unsigned)nk), dim3(256), (size_t)(0), st, kv, A.null_kv, B.qh, dO, B.P, B.dS, A.k_scale, dkv,
+                      (float*)G.null_kv, (float*)G.k_scale, (const float*)preK, (const float*)preV, g);
+    PHK_LAUNCH_CHECK();
+  }
   if (dbias) {
     const int64_t total = (int64_t)g.H * g.n * g.m;
     PHK_KERNEL_LAUNCH(attn_bwd_dbias_kernel, dim3((unsigned)((total + 255) / 256 < 4096 ? (total + 255) / 256 : 4096)), dim3(256), (size_t)(0), st, B.dS, dbias, g);
@@ -876,9 +1068,10 @@ int attention_forward_dropout(const float* q, const float* kv, const phk_attn_t&
 // registers (threads over channels, coalesced rows) and leaves as ONE atomic per (channel, tap, chunk) -- the per-position
 // atomics this replaces (27 * D per position onto 27 * D addresses) took 0.5 ms per layer at 2304 positions.
 constexpr int PEG_DW_CHUNKS = 16, PEG_DW_MAXJ = 8;  // D <= 128 * 8
-__global__ void __launch_bounds__(128) peg_bwd_dw_kernel(const float* __restrict__ x, const float* __restrict__ dy,
-                                                         float* __restrict__ dw, int64_t P, int T, int H, int W, int D,
-                                                         int pad_t0) {
+// part (deterministic mode, else NULL): the chunk's sums go to its slot [blockIdx.y][D][27] instead of dw
+__device__ __forceinline__ void peg_bwd_dw_body(const float* __restrict__ x, const float* __restrict__ dy,
+                                                float* __restrict__ dw, int64_t P, int T, int H, int W, int D, int pad_t0,
+                                                float* __restrict__ part) {
   const int tap = blockIdx.x;
   const int kt = tap / 9, kh = (tap / 3) % 3, kw = tap % 3;
   const int HW = H * W;
@@ -905,9 +1098,23 @@ __global__ void __launch_bounds__(128) peg_bwd_dw_kernel(const float* __restrict
 #pragma unroll
   for (int j = 0; j < PEG_DW_MAXJ; ++j) {
     const int d = threadIdx.x + 128 * j;
-    if (d < D && p1 > p0) atomicAdd(dw + (int64_t)d * 27 + tap, acc[j]);  // dsconv.weight[d, 0, kt, kh, kw]
+    if (d >= D) continue;
+    if (part) part[(int64_t)blockIdx.y * 27 * D + (int64_t)d * 27 + tap] = p1 > p0 ? acc[j] : 0.f;
+    else if (p1 > p0) atomicAdd(dw + (int64_t)d * 27 + tap, acc[j]);  // dsconv.weight[d, 0, kt, kh, kw]
   }
 }
+__global__ void __launch_bounds__(128) peg_bwd_dw_kernel(const float* __restrict__ x, const float* __restrict__ dy,
+                                                         float* __restrict__ dw, int64_t P, int T, int H, int W, int D,
+                                                         int pad_t0) {
+  peg_bwd_dw_body(x, dy, dw, P, T, H, W, D, pad_t0, nullptr);
+}
+__global__ void __launch_bounds__(128) peg_bwd_dw_fixed_kernel(const float* __restrict__ x, const float* __restrict__ dy,
+                                                               int64_t P, int T, int H, int W, int D, int pad_t0,
+                                                               float* __restrict__ part) {
+  peg_bwd_dw_body(x, dy, nullptr, P, T, H, W, D, pad_t0, part);
+}
+
+inline int64_t peg_det_floats(int64_t D) { return PEG_DW_CHUNKS * 27 * D; }
 
 __global__ void __launch_bounds__(128) peg_bwd_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                       const float* __restrict__ dy, float* __restrict__ dx,
@@ -955,6 +1162,75 @@ __global__ void embed_bwd_kernel(const int64_t* __restrict__ ids, const float* _
   }
 }
 
+// Deterministic mode, token embedding: the rows of one id are summed in row order by one CTA, the one of the id's first
+// row (the leader).  CTA r first looks for an earlier row with its id and leaves if there is one; the leader then walks
+// the rows after it in tiles of blockDim.x, lists the tile's matching rows in order (a prefix sum over the tile) and adds
+// their dx rows, columns over threads, into four accumulators taken in turn (a0 gets the entry, then the four rotate).
+__device__ __forceinline__ int64_t embed_row_id(const int64_t* ids, int64_t r, int vocab_rows) {
+  const int64_t id = ids[r];
+  return id < 0 ? 0 : (id >= vocab_rows ? vocab_rows - 1 : id);
+}
+__global__ void __launch_bounds__(128) embed_tok_fixed_kernel(const int64_t* __restrict__ ids, const float* __restrict__ dx,
+                                                              float* __restrict__ dtok, int64_t rows, int dim, float alpha,
+                                                              int vocab_rows) {
+  __shared__ int found;
+  __shared__ int scan[128];
+  __shared__ int64_t list[128];
+  const int t = threadIdx.x;
+  const int64_t r = blockIdx.x;
+  const int64_t id = embed_row_id(ids, r, vocab_rows);
+  if (t == 0) found = 0;
+  __syncthreads();
+  for (int64_t q = t; q < r; q += blockDim.x)
+    if (embed_row_id(ids, q, vocab_rows) == id) { found = 1; break; }
+  __syncthreads();
+  if (found) return;  // uniform over the CTA
+  for (int c0 = 0; c0 < dim; c0 += 128 * 4) {
+    float a0[4], a1[4], a2[4], a3[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) a0[j] = a1[j] = a2[j] = a3[j] = 0.f;
+    for (int64_t base = r; base < rows; base += blockDim.x) {
+      const int64_t q = base + t;
+      const int hit = q < rows && embed_row_id(ids, q, vocab_rows) == id;
+      scan[t] = hit;
+      __syncthreads();
+      for (int off = 1; off < 128; off <<= 1) {  // inclusive prefix sum over the tile
+        const int v = t >= off ? scan[t - off] : 0;
+        __syncthreads();
+        scan[t] += v;
+        __syncthreads();
+      }
+      if (hit) list[scan[t] - 1] = q;
+      const int cnt = scan[127];
+      __syncthreads();
+      for (int e = 0; e < cnt; ++e) {
+        const float* xr = dx + list[e] * dim;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int c = c0 + t + 128 * j;
+          const float v = a0[j] + (c < dim ? alpha * xr[c] : 0.f);
+          a0[j] = a1[j]; a1[j] = a2[j]; a2[j] = a3[j]; a3[j] = v;
+        }
+      }
+      __syncthreads();  // list and scan are rewritten by the next tile
+    }
+    for (int j = 0; j < 4; ++j) {
+      const int c = c0 + t + 128 * j;
+      if (c < dim) dtok[id * dim + c] += (a0[j] + a1[j]) + (a2[j] + a3[j]);
+    }
+  }
+}
+// Deterministic mode, position embedding: dpos[p, c] += sum over the sequences b, in order, of alpha dx[b n + p, c]
+__global__ void embed_pos_fixed_kernel(const float* __restrict__ dx, float* __restrict__ dpos, int64_t rows, int n, int dim,
+                                       float alpha) {
+  const int64_t total = (int64_t)n * dim, nb = rows / n;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    float a = 0.f;
+    for (int64_t b = 0; b < nb; ++b) a += alpha * dx[b * total + i];
+    dpos[i] += a;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // ContinuousPositionBias backward (attention.py:257-275): bias[h,i,j] = table[u(i,j), h], table = MLP(in[u]).
 // The MLP runs over the U distinct coordinate deltas; its backward is three dgrad/wgrad pairs on [U, .] matrices.
@@ -999,6 +1275,29 @@ __global__ void cpb_dtable_kernel(const float* __restrict__ dbias, float* __rest
   }
 }
 
+// Deterministic mode: dtable[u, h] = sum of dbias[h, i, j] over the (i, j) pairs with delta u, in increasing i (a gather:
+// the pairs of u are i = j + delta with both inside the grid)
+__global__ void cpb_dtable_fixed_kernel(const float* __restrict__ dbias, float* __restrict__ dtable, int heads, int d0,
+                                        int d1, int d2) {
+  const int n = d0 * d1 * d2;
+  const int64_t total = (int64_t)n * n;
+  const int s1 = 2 * d1 - 1, s2 = 2 * d2 - 1;
+  const int64_t U = (int64_t)(2 * d0 - 1) * s1 * s2;
+  for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < U * heads; idx += (int64_t)gridDim.x * blockDim.x) {
+    const int h = (int)(idx % heads);
+    const int u = (int)(idx / heads);
+    const int e0 = u / (s1 * s2) - (d0 - 1), e1 = (u / s2) % s1 - (d1 - 1), e2 = u % s2 - (d2 - 1);  // i - j per axis
+    float a = 0.f;
+    for (int i0 = e0 > 0 ? e0 : 0; i0 < d0 && i0 - e0 < d0; ++i0)
+      for (int i1 = e1 > 0 ? e1 : 0; i1 < d1 && i1 - e1 < d1; ++i1)
+        for (int i2 = e2 > 0 ? e2 : 0; i2 < d2 && i2 - e2 < d2; ++i2) {
+          const int64_t i = ((int64_t)i0 * d1 + i1) * d2 + i2, j = ((int64_t)(i0 - e0) * d1 + (i1 - e1)) * d2 + (i2 - e2);
+          a += dbias[(int64_t)h * total + i * n + j];
+        }
+    dtable[idx] = a;
+  }
+}
+
 inline unsigned ew_grid(int64_t total) {
   const int64_t b = (total + 255) / 256;
   return (unsigned)(b < 1 ? 1 : (b > kNumSMs * 16 ? kNumSMs * 16 : b));
@@ -1029,10 +1328,15 @@ int cpb_backward(const phk_cpb_t& c, const phk_cpb_t& G, const float* dbias, int
   PHK_KERNEL_LAUNCH(bias_lrelu_kernel, dim3(ew_grid(U * hid)), dim3(256), (size_t)(0), st, a2, c.b1, U, hid);
   PHK_LAUNCH_CHECK();
   // dtable[u, h] = sum over the (i, j) pairs with delta u
-  PHK_CUDA(cudaMemsetAsync(dtable, 0, U * H * sizeof(float), st));
-  const int64_t nn = (int64_t)d0 * d1 * d2 * d0 * d1 * d2;
-  PHK_KERNEL_LAUNCH(cpb_dtable_kernel, dim3(ew_grid(nn)), dim3(256), (size_t)(0), st, dbias, dtable, H, d0, d1, d2);
-  PHK_LAUNCH_CHECK();
+  if (t_det.p) {
+    PHK_KERNEL_LAUNCH(cpb_dtable_fixed_kernel, dim3(ew_grid(U * H)), dim3(256), (size_t)(0), st, dbias, dtable, H, d0, d1, d2);
+    PHK_LAUNCH_CHECK();
+  } else {
+    PHK_CUDA(cudaMemsetAsync(dtable, 0, U * H * sizeof(float), st));
+    const int64_t nn = (int64_t)d0 * d1 * d2 * d0 * d1 * d2;
+    PHK_KERNEL_LAUNCH(cpb_dtable_kernel, dim3(ew_grid(nn)), dim3(256), (size_t)(0), st, dbias, dtable, H, d0, d1, d2);
+    PHK_LAUNCH_CHECK();
+  }
   // last layer: table = a2 W2^T + b2
   PHK_TRY(wgrad(dtable, a2, (float*)G.w2, U, H, hid, st));
   PHK_TRY(colsum(dtable, U, H, H, (float*)G.b2, st));
@@ -1219,6 +1523,12 @@ extern "C" int phk_train_set_progress_events(void** events, int32_t count) {
   g_progress_events = events;
   g_progress_count = events ? count : 0;
   return 0;
+}
+// See include/phk.h: the deterministic mode of this thread's next backward calls and workspace queries
+extern "C" int32_t phk_train_set_deterministic(int32_t on) {
+  const int32_t prev = t_det_mode;
+  t_det_mode = on ? 1 : 0;
+  return prev;
 }
 static inline int progress_mark(void** ev, int n, int idx, cudaStream_t st) {
   if (ev && idx < n && ev[idx]) PHK_CUDA(cudaEventRecord(reinterpret_cast<cudaEvent_t>(ev[idx]), st));
@@ -1474,8 +1784,15 @@ int layer_backward(const LayerCall& c, int l, const LayerSave& Sv, float** dx, f
   // PEG: x1 = x0 + conv(x0) + b
   PHK_TRY(colsum(d, R, D, D, (float*)Gy.peg.b, st));
   PHK_REQUIRE(D <= 128 * PEG_DW_MAXJ, PHK_E_UNSUPPORTED, "train: PEG backward needs dim <= 1024");
-  PHK_KERNEL_LAUNCH(peg_bwd_dw_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, Sv.x0, d, (float*)Gy.peg.w, R, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal ? 2 : 1);
-  PHK_LAUNCH_CHECK();
+  if (t_det.p) {  // deterministic mode: one [D, 27] slot per chunk of positions, added in order
+    PHK_REQUIRE(peg_det_floats(D) <= t_det.floats, PHK_E_WORKSPACE, "train: deterministic reduction scratch too small");
+    PHK_KERNEL_LAUNCH(peg_bwd_dw_fixed_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, Sv.x0, (const float*)d, R, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal ? 2 : 1, t_det.p);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(add_slots(t_det.p, PEG_DW_CHUNKS, 27 * (int64_t)D, (float*)Gy.peg.w, st));
+  } else {
+    PHK_KERNEL_LAUNCH(peg_bwd_dw_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, Sv.x0, d, (float*)Gy.peg.w, R, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal ? 2 : 1);
+    PHK_LAUNCH_CHECK();
+  }
   PHK_KERNEL_LAUNCH(peg_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, Sv.x0, Ly.peg.w, d, *dx_alt, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal ? 2 : 1);
   PHK_LAUNCH_CHECK();
   *dx = *dx_alt;
@@ -1603,15 +1920,81 @@ int step_backward(Step& S, float* d_context, void** prog, int nprog) {
     PHK_TRY(progress_mark(prog, nprog, 1 + (T->depth - 1 - l), st));
   }
   // ---------------------------------------------------------------- embeddings, position-bias MLP
-  PHK_KERNEL_LAUNCH(embed_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, S.ids, dx, (float*)grads->token_emb, (float*)grads->pos_emb, n, D,
-                                               m->is_critic ? 1.0f : m->shrink_alpha, m->num_tokens + 1);
-  PHK_LAUNCH_CHECK();
+  const float alpha = m->is_critic ? 1.0f : m->shrink_alpha;
+  if (t_det.p) {
+    PHK_KERNEL_LAUNCH(embed_tok_fixed_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, S.ids, (const float*)dx, (float*)grads->token_emb, R, D, alpha, m->num_tokens + 1);
+    PHK_LAUNCH_CHECK();
+    PHK_KERNEL_LAUNCH(embed_pos_fixed_kernel, dim3(ew_grid((int64_t)n * D)), dim3(256), (size_t)(0), st, (const float*)dx, (float*)grads->pos_emb, R, n, D, alpha);
+    PHK_LAUNCH_CHECK();
+  } else {
+    PHK_KERNEL_LAUNCH(embed_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, S.ids, dx, (float*)grads->token_emb, (float*)grads->pos_emb, n, D,
+                                                 alpha, m->num_tokens + 1);
+    PHK_LAUNCH_CHECK();
+  }
   if (m->has_bias) {
     float* csc = ar.f(cpb_bwd_scratch_floats(m->pos_bias, pt, ph, pw));
     PHK_REQUIRE(csc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (position-bias backward)");
     PHK_TRY(cpb_backward(m->pos_bias, grads->pos_bias, S.dbias, pt, ph, pw, csc, st));
   }
   PHK_TRY(progress_mark(prog, nprog, T->depth + 1, st));
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------------------------------
+// Deterministic-mode scratch (t_det): the largest region any one reduction of the call uses, from the same per-site
+// functions the reductions check against.  DetNeed keeps the maximum.
+// ------------------------------------------------------------------------------------------------------------------
+struct DetNeed {
+  int64_t f = 0;
+  void add(int64_t v) { f = v > f ? v : f; }
+  void colsum(int64_t rows, int64_t cols) { add(colsum_fixed_floats(rows, cols)); }
+  void ln(int64_t rows, int64_t dim) { add(ln_det_floats(rows, dim)); }
+  void wgrad(int64_t M, int64_t N, int64_t K) { add(wgrad_det_floats(M, N, K)); }
+};
+
+// Every layer of T over b sequences of n rows (L > 0: cross-attention to L context tokens), and its norm_out
+void det_need_stack(DetNeed& d, const phk_transformer_t* T, int b, int n, int L) {
+  const int64_t R = (int64_t)b * n, CR = (int64_t)b * L, D = T->dim, I = (int64_t)T->heads * T->dim_head;
+  d.ln(R, D);
+  for (int l = 0; l < T->depth; ++l) {
+    const phk_layer_t& Ly = T->layers[l];
+    const int64_t inner = Ly.ff.inner;
+    d.wgrad(R, D, inner); d.wgrad(R, 2 * inner, D); d.wgrad(R, D, I); d.wgrad(R, I, D); d.wgrad(R, 2 * I, D);
+    d.add(attn_bwd_det_floats(AttnBwdGeom{b, T->heads, n, n, 0, T->dim_head}));
+    if (Ly.has_peg) { d.colsum(R, D); d.add(peg_det_floats(D)); }
+    if (Ly.has_cross && L > 0) {
+      const int64_t dc = Ly.cross_attn.dim_context;
+      d.ln(CR, dc); d.wgrad(CR, 2 * I, dc);
+      d.add(attn_bwd_det_floats(AttnBwdGeom{b, T->heads, n, L, Ly.cross_attn.num_null_kv, T->dim_head}));
+    }
+  }
+}
+
+// cpb_backward over U coordinate deltas
+void det_need_cpb(DetNeed& d, const phk_cpb_t& c, int64_t U) {
+  d.wgrad(U, c.heads, c.hidden); d.wgrad(U, c.hidden, c.hidden); d.wgrad(U, c.hidden, c.num_dims);
+  d.colsum(U, c.heads > c.hidden ? c.heads : c.hidden);
+}
+
+// stages 2 and 3 of a MaskGit differentiation of b sequences (head rows R = b n at most)
+int64_t step_det_floats(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L) {
+  DetNeed d;
+  const int64_t R = (int64_t)b * n;
+  det_need_stack(d, &m->transformer, b, n, L);
+  d.colsum(R, m->num_tokens); d.wgrad(R, m->num_tokens, m->dim); d.wgrad(R, 1, m->dim);
+  if (m->has_bias) det_need_cpb(d, m->pos_bias, 8 * (int64_t)n);  // U <= 8 n (step_workspace_bytes)
+  return d.f;
+}
+
+// Bytes the deterministic mode adds to a workspace (0 in the default mode): the region and its alignment
+int64_t det_bytes(int64_t floats) { return t_det_mode ? (floats > 0 ? floats : 1) * 4 + 256 : 0; }
+
+// Carves the deterministic-mode region from the front of `ar` and publishes it for the call (nothing in the default mode)
+int det_begin(Arena& ar, int64_t floats, const char* msg) {
+  if (!t_det_mode) return 0;
+  float* p = ar.f(floats > 0 ? floats : 1);
+  PHK_REQUIRE(p, PHK_E_WORKSPACE, msg);
+  t_det = DetScratch{p, floats};
   return 0;
 }
 
@@ -1697,7 +2080,7 @@ extern "C" int64_t phk_maskgit_train_workspace_bytes(const phk_maskgit_t* m, int
   const int64_t R = (int64_t)b * n;
   // (d)logits in place or the differentiated copy; row losses
   const int64_t head = bce_head ? 3 * R : R * (int64_t)m->num_tokens + 2 * R;
-  return step_workspace_bytes(m, b, n, L, head, !bce_head, prec);
+  return step_workspace_bytes(m, b, n, L, head, !bce_head, prec) + det_bytes(step_det_floats(m, b, n, L));
 }
 
 extern "C" int64_t phk_maskgit_train_dropout_counters(const phk_maskgit_t* m, int32_t b, int32_t n, int32_t L) {
@@ -1736,6 +2119,8 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   S.m = m; S.grads = grads; S.ids = ids_in; S.b = b; S.n = n; S.pt = pt; S.ph = ph; S.pw = pw; S.L = L;
   S.context = context; S.text_mask = text_mask; S.video_mask = video_mask; S.prec = prec; S.s = s; S.dropout = dropout;
   S.ar = Arena{(char*)workspace, workspace_bytes, 0};
+  DetScope det_scope;
+  PHK_TRY(det_begin(S.ar, step_det_floats(m, b, n, L), "maskgit_train_step: workspace too small (deterministic mode)"));
   step_init(S);
   const cudaStream_t st = S.st;
   const int D = S.D, V = m->num_tokens;
@@ -1834,7 +2219,7 @@ extern "C" int64_t phk_maskgit_backward_workspace_bytes(const phk_maskgit_t* m, 
   const int64_t Rh = (int64_t)b * n, CRh = (int64_t)b * L, dc = context_width(&m->transformer);
   int64_t head = 64;
   if (pair) head += Rh * m->dim + pair_input_floats(Rh, CRh, dc) + 2 * CRh * dc;  // mixed embeddings; inputs; d context
-  return step_workspace_bytes(m, B, n, L, head, head_kind == PHK_HEAD_LOGITS, prec);
+  return step_workspace_bytes(m, B, n, L, head, head_kind == PHK_HEAD_LOGITS, prec) + det_bytes(step_det_floats(m, B, n, L));
 }
 
 // See include/phk.h.
@@ -1864,6 +2249,8 @@ extern "C" int phk_maskgit_backward(const phk_maskgit_t* m, const phk_maskgit_t*
   S.context = context; S.text_mask = text_mask; S.video_mask = video_mask; S.prec = prec; S.s = s;
   S.ar = Arena{(char*)workspace, workspace_bytes, 0};
   Arena& ar = S.ar;
+  DetScope det_scope;
+  PHK_TRY(det_begin(ar, step_det_floats(m, S.b, n, L), "maskgit_backward: workspace too small (deterministic mode)"));
   float* ctx_grad = d_context;  // where stage 3 accumulates d/d(context): both halves of a pair, summed below
   if (pair) {  // the 2b-sequence inputs of the forward's pair (phk_maskgit_forward, cfg_pair = 1)
     int64_t* ids2 = reinterpret_cast<int64_t*>(ar.f(2 * Rh * 2));
@@ -2482,13 +2869,47 @@ int check_cvivit_pair(const char* entry, const M* m, const M* grads) {
   return 0;
 }
 
+// Deterministic-mode scratch (see step_det_floats) of the C-ViViT backward phases
+void det_need_cv_stacks(DetNeed& d, const phk_transformer_t* TT, const phk_transformer_t* TS, const CvGeom& g) {
+  det_need_stack(d, TT, g.B * g.hw, g.Tp, 0);
+  det_need_stack(d, TS, g.B * g.Tp, g.hw, 0);
+}
+void det_need_cv_cpb(DetNeed& d, const phk_cpb_t& c, const CvGeom& g) {
+  det_need_cpb(d, c, (int64_t)(2 * g.hh - 1) * (2 * g.ww - 1));
+}
+int64_t cv_decode_det_floats(const phk_cvivit_dec_t* m, const CvGeom& g) {
+  DetNeed d;
+  det_need_cv_stacks(d, &m->temporal, &m->spatial, g);
+  d.wgrad(g.rows1, g.K1, g.D); d.colsum(g.rows1, g.K1); d.wgrad(g.rows2, g.K2, g.D); d.colsum(g.rows2, g.K2);  // to_pixels*
+  d.wgrad(g.R, g.D, m->codebook_bits); d.colsum(g.R, g.D);                                                    // project_out
+  det_need_cv_cpb(d, m->spatial_bias, g);
+  return d.f;
+}
+int64_t cv_encode_det_floats(const phk_cvivit_t* m, const CvGeom& g) {
+  DetNeed d;
+  det_need_cv_stacks(d, &m->temporal, &m->spatial, g);
+  det_need_cv_cpb(d, m->spatial_bias, g);
+  return d.f;
+}
+int64_t cv_backward_det_floats(const phk_cvivit_t* enc, const phk_cvivit_dec_t* dec, const CvGeom& g) {
+  DetNeed d;
+  d.add(cv_decode_det_floats(dec, g));
+  d.add(cv_encode_det_floats(enc, g));
+  d.wgrad(g.R, enc->codebook_bits, g.D); d.colsum(g.R, enc->codebook_bits);  // project_in
+  const int64_t rows[2] = {g.rows1, g.rows2}, K[2] = {g.K1, g.K2};
+  for (int e = 0; e < 2; ++e) {  // to_patch_emb*: LN -> Linear -> LN
+    d.ln(rows[e], g.D); d.wgrad(rows[e], g.D, K[e]); d.colsum(rows[e], g.D); d.ln(rows[e], K[e]);
+  }
+  return d.f;
+}
+
 }  // namespace
 }  // namespace phk
 
 extern "C" int64_t phk_cvivit_decode_backward_workspace_bytes(const phk_cvivit_dec_t* m, int32_t B, int32_t Tp, int32_t prec) {
   if (!cvivit_shapes_ok(m, B, Tp)) return -1;
   const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(&m->temporal), stack_inner(&m->spatial)));
-  return cv_shared_bytes(g, m->spatial_bias, prec) + dec_phase_floats(m, g) * 4;
+  return cv_shared_bytes(g, m->spatial_bias, prec) + dec_phase_floats(m, g) * 4 + det_bytes(cv_decode_det_floats(m, g));
 }
 
 // See include/phk.h.
@@ -2506,6 +2927,8 @@ extern "C" int phk_cvivit_decode_backward(const phk_cvivit_dec_t* m, const phk_c
               "cvivit_decode_backward: ids need LFQ's project_out and its gradient");
   const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(&m->temporal), stack_inner(&m->spatial)));
   Arena ar{(char*)workspace, workspace_bytes, 0};
+  DetScope det_scope;
+  PHK_TRY(det_begin(ar, cv_decode_det_floats(m, g), "cvivit_decode_backward: workspace too small (deterministic mode)"));
   CvShared S;
   PHK_TRY(cv_shared_init(ar, g, m->spatial_bias, prec, s, S));
   return decode_backward_phase(m, grads, ids, tokens, g, dvideo, dtokens, nullptr, S, ar, true, prec, s, nullptr);
@@ -2539,7 +2962,8 @@ extern "C" int64_t phk_cvivit_backward_workspace_bytes(const phk_cvivit_t* enc, 
   const CvGeom g = cv_geom(dec, B, Tp, inner);
   const int64_t video = (int64_t)B * g.C * F * dec->image_h * dec->image_w;
   const int64_t own = g.R * enc->codebook_bits + video + 256 * 4 / 4;            // d q, d recon
-  return cv_shared_bytes(g, dec->spatial_bias, prec) + (own + imax(dec_phase_floats(dec, g), enc_phase_floats(enc, g, true))) * 4;
+  return cv_shared_bytes(g, dec->spatial_bias, prec) + (own + imax(dec_phase_floats(dec, g), enc_phase_floats(enc, g, true))) * 4 +
+         det_bytes(cv_backward_det_floats(enc, dec, g));
 }
 
 // See include/phk.h: to_pixels*, the decoder's spatial and temporal layers, project_out, the encoder's temporal and
@@ -2586,6 +3010,8 @@ extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* 
   const int64_t nvideo = (int64_t)B * C * F * H * W;
   const cudaStream_t st = to_stream(s);
   Arena ar{(char*)workspace, workspace_bytes, 0};
+  DetScope det_scope;
+  PHK_TRY(det_begin(ar, cv_backward_det_floats(enc, dec, g), "cvivit_backward: workspace too small (deterministic mode)"));
   CvShared S;
   PHK_TRY(cv_shared_init(ar, g, dec->spatial_bias, prec, s, S));
   float* dq = ar.f(R * bits);
@@ -2682,7 +3108,7 @@ extern "C" int phk_cvivit_backward(const phk_cvivit_t* enc, const phk_cvivit_t* 
 extern "C" int64_t phk_cvivit_encode_backward_workspace_bytes(const phk_cvivit_t* m, int32_t B, int32_t Tp, int32_t prec) {
   if (!cvivit_shapes_ok(m, B, Tp)) return -1;
   const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(&m->spatial), stack_inner(&m->temporal)));
-  return cv_shared_bytes(g, m->spatial_bias, prec) + enc_stacks_floats(m, g) * 4;
+  return cv_shared_bytes(g, m->spatial_bias, prec) + enc_stacks_floats(m, g) * 4 + det_bytes(cv_encode_det_floats(m, g));
 }
 
 // See include/phk.h.
@@ -2700,6 +3126,8 @@ extern "C" int phk_cvivit_encode_backward(const phk_cvivit_t* m, const phk_cvivi
               "cvivit_encode_backward: the gradient table has no position-bias MLP");
   const CvGeom g = cv_geom(m, B, Tp, imax(stack_inner(&m->spatial), stack_inner(&m->temporal)));
   Arena ar{(char*)workspace, workspace_bytes, 0};
+  DetScope det_scope;
+  PHK_TRY(det_begin(ar, cv_encode_det_floats(m, g), "cvivit_encode_backward: workspace too small (deterministic mode)"));
   CvShared S;
   PHK_TRY(cv_shared_init(ar, g, m->spatial_bias, prec, s, S));
   return encode_backward_phase(m, grads, tokens, g, dout, nullptr, dtokens, nullptr, S, ar, true, prec, s, nullptr);

@@ -514,6 +514,7 @@ class CViViT(nn.Module):
                      else dloss.to(dev, torch.float32).contiguous())
             drecon = None if drecon is None else drecon.to(dev, torch.float32).reshape(recon.shape).contiguous()
             dvideo = torch.empty_like(video) if want_video_grad else None
+            L.sync_deterministic()  # on the thread autograd runs this backward on
             nbytes = lib.phk_cvivit_backward_workspace_bytes(C.byref(enc), C.byref(dec), b, f, prec)
             ws = self._ws.get_for("phk_cvivit_backward_workspace_bytes", nbytes, dev)
             plan = None
@@ -610,6 +611,7 @@ class CViViT(nn.Module):
             gk = GradKeep(call["params"])
             gtable = self._dec_grad_table(gk, ids is not None)
             dtokens = torch.empty_like(tokens) if tokens is not None and want_tokens_grad else None
+            L.sync_deterministic()  # on the thread autograd runs this backward on
             nbytes = lib.phk_cvivit_decode_backward_workspace_bytes(C.byref(table), b, tp, prec)
             ws = self._ws.get_for("phk_cvivit_decode_backward_workspace_bytes", nbytes, dev)
             L.check(lib.phk_cvivit_decode_backward(C.byref(table), C.byref(gtable), L.ptr(ids), L.ptr(tokens), b, tp,
@@ -682,6 +684,7 @@ class CViViT(nn.Module):
             gk = GradKeep(call["params"])
             gtable = self._enc_grad_table(gk, False)
             dtokens = torch.empty_like(tokens) if want_tokens_grad else None
+            L.sync_deterministic()  # on the thread autograd runs this backward on
             nbytes = lib.phk_cvivit_encode_backward_workspace_bytes(C.byref(table), b, tp, prec)
             ws = self._ws.get_for("phk_cvivit_encode_backward_workspace_bytes", nbytes, dev)
             L.check(lib.phk_cvivit_encode_backward(C.byref(table), C.byref(gtable), L.ptr(tokens), b, tp, L.ptr(dout),

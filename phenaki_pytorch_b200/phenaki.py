@@ -285,6 +285,7 @@ class _TokenTransformer(nn.Module):
                 logits = torch.empty((b, n, table.num_tokens), dtype=torch.float32, device=dev)
             loss = torch.zeros((), dtype=torch.float32, device=dev)
             prec = train_precision(self.precision)
+            L.sync_deterministic()  # read here: Phenaki.forward runs the whole step inside the forward
             nbytes = lib.phk_maskgit_train_workspace_bytes(C.byref(table), b, n, ctx_len, int(bce), prec)
             ws = self._ws.get_for("phk_maskgit_train_workspace_bytes", nbytes, dev)
             pt, ph, pw = (int(v) for v in patch_shape)
@@ -389,6 +390,7 @@ class _TokenTransformer(nn.Module):
             pt, ph, pw = call["patch_shape"]
             gtable, gk = self._grad_table(has_cross, owner=owner, head=head)
             try:
+                L.sync_deterministic()  # on the thread autograd runs this backward on
                 nbytes = lib.phk_maskgit_backward_workspace_bytes(C.byref(table), b, n, ctx_len, int(cfg), head_kind, prec)
                 ws = self._ws.get_for("phk_maskgit_backward_workspace_bytes", nbytes, dev)
                 d_context = torch.zeros_like(context) if has_cross and want_context_grad else None
