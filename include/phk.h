@@ -38,6 +38,10 @@ extern "C" {
 typedef struct CUstream_st* phk_stream_t; /* == cudaStream_t */
 
 enum { PHK_PREC_F32 = 0, PHK_PREC_BF16 = 1, PHK_PREC_BF16X3 = 2 };
+/* Element type of a video the encode reads (video_dtype).  PHK_VIDEO_U8: uint8 frames as decoders produce them; a byte u
+ * stands for the fp32 u / 255 correctly rounded (torchvision ToTensor), and every result equals, bit for bit, that of
+ * the PHK_VIDEO_F32 call on those quotients. */
+enum { PHK_VIDEO_F32 = 0, PHK_VIDEO_U8 = 1 };
 enum {
   PHK_E_ARG = -1,      /* null pointer / non-positive size            */
   PHK_E_SHAPE = -2,    /* shape contract violated (reference asserts) */
@@ -171,6 +175,11 @@ int phk_layernorm(const float* x, const float* gamma, const float* beta, void* o
 int phk_patchify_ln(const float* video, int32_t B, int32_t C, int32_t F, int32_t H, int32_t W,
                     int32_t f0, int32_t nt, int32_t pt, int32_t p1, int32_t p2,
                     const float* ln_g, const float* ln_b, void* out, int32_t out_bf16, phk_stream_t s);
+/* The same for a uint8 video (any alignment): out equals, bit for bit, phk_patchify_ln's on the fp32 video u / 255
+ * (correctly rounded quotients, as PHK_VIDEO_U8 defines them). */
+int phk_patchify_ln_u8(const uint8_t* video, int32_t B, int32_t C, int32_t F, int32_t H, int32_t W,
+                       int32_t f0, int32_t nt, int32_t pt, int32_t p1, int32_t p2,
+                       const float* ln_g, const float* ln_b, void* out, int32_t out_bf16, phk_stream_t s);
 
 /* C[map(m), n] = sum_k A[m,k] * W[n,k] (+bias[n]) (+residual[map(m), n]); nn.Linear semantics.
  * Row map: map(m) = (m / seg_len) * seg_stride + seg_off + m % seg_len (seg_len<=0: identity).
@@ -371,22 +380,22 @@ int phk_cfg_combine(const float* cond, const float* null_out, float cond_scale, 
 /* ------------------------------------------------------------------------------------------ */
 
 /* CViViT.forward(video, return_only_codebook_ids=True) (cvivit.py:518-574).
- * video (B,C,F,H,W) fp32 device; ids (B,T',H',W') int64 device.
+ * video (B,C,F,H,W) device, fp32 or uint8 as video_dtype (PHK_VIDEO_*) says; ids (B,T',H',W') int64 device.
  * spatial_bias: cached phk_cpb_bias(spatial_bias, H', W') output [heads, H'W', H'W'] or NULL
  * (recomputed inside).  taps: optional fp32 device buffers for the parity tests:
  * tap_patch / tap_spatial / tap_temporal [B*T'*H'*W', dim] in (b,t,h,w) row order,
  * tap_proj [rows, bits] = LFQ pre-sign projection.
- * Launch cost: the ~75 launches of one call are a pure function of (table contents, buffers, shape, prec).  With
- * spatial_bias given and no taps, the second call with an identical key is captured into a CUDA graph on a
+ * Launch cost: the ~75 launches of one call are a pure function of (table contents, buffers, video_dtype, shape,
+ * prec).  With spatial_bias given and no taps, the second call with an identical key is captured into a CUDA graph on a
  * library-owned stream and later calls replay it on `s` (one cudaGraphLaunch; calls stay eager while the per-family
  * profiler is on).  The graph only bakes in addresses: new data in the same buffers (video, weights updated in place) is
  * honoured; a table with different pointers or dims is a different key. */
 int64_t phk_cvivit_workspace_bytes(const phk_cvivit_t* m, int32_t B, int32_t F, int32_t prec);
-int phk_cvivit_encode(const phk_cvivit_t* m, const float* video, int32_t B, int32_t F,
+int phk_cvivit_encode(const phk_cvivit_t* m, const void* video, int32_t video_dtype, int32_t B, int32_t F,
                       int64_t* ids, void* workspace, int64_t workspace_bytes, int32_t prec,
                       const float* spatial_bias, float* tap_patch, float* tap_spatial,
                       float* tap_temporal, float* tap_proj, phk_stream_t s);
-/* same through HOST buffers (pinned or pageable): H2D of the video, encode, D2H of the ids,
+/* same through HOST buffers (pinned or pageable), fp32 video: H2D of the video, encode, D2H of the ids,
  * stream synchronise.  dev_video / dev_ids are caller-owned staging buffers. */
 int phk_cvivit_encode_host(const phk_cvivit_t* m, const float* host_video, int32_t B, int32_t F,
                            int64_t* host_ids, void* dev_video, int64_t* dev_ids, void* workspace,
@@ -396,16 +405,16 @@ int phk_cvivit_encode_host(const phk_cvivit_t* m, const float* host_video, int32
 /* Pipelined variant of phk_cvivit_encode_host for a stream of batches (what a tokenisation job over a dataset does):
  * submit() enqueues H2D on the pipe's own copy stream, encode + D2H of the ids on the caller's stream `s`, and
  * returns at once; the copy of batch i+1 overlaps the encode of batch i.  The caller owns `depth` staging slots:
- * dev_video_slots = depth x (B,C,F,H,W) floats, dev_ids_slots = depth x B*T'*H'*W' int64 (slot = ticket % depth), and
- * must keep B, F fixed while tickets are in flight.  host_video should be pinned and must stay untouched until
+ * dev_video_slots = depth x (B,C,F,H,W) elements of video_dtype (PHK_VIDEO_*: 4 or 1 bytes each), dev_ids_slots =
+ * depth x B*T'*H'*W' int64 (slot = ticket % depth), and must keep B, F and video_dtype fixed while tickets are in flight.  host_video should be pinned and must stay untouched until
  * wait(ticket) returns.  wait(ticket) blocks until that
  * batch's host_ids are valid; at most `depth` tickets may be in flight.  Host-side objects only (one stream, 3*depth
  * events); no device memory is allocated. */
 typedef struct phk_encode_pipe phk_encode_pipe_t;
 int phk_encode_pipe_create(phk_encode_pipe_t** pipe, int32_t depth);
 int phk_encode_pipe_destroy(phk_encode_pipe_t* pipe);
-int phk_encode_pipe_submit(phk_encode_pipe_t* pipe, const phk_cvivit_t* m, const float* host_video, int32_t B,
-                           int32_t F, int64_t* host_ids, void* dev_video_slots, int64_t* dev_ids_slots,
+int phk_encode_pipe_submit(phk_encode_pipe_t* pipe, const phk_cvivit_t* m, const void* host_video,
+                           int32_t video_dtype, int32_t B, int32_t F, int64_t* host_ids, void* dev_video_slots, int64_t* dev_ids_slots,
                            void* workspace, int64_t workspace_bytes, int32_t prec, const float* spatial_bias,
                            phk_stream_t s, int64_t* ticket);
 int phk_encode_pipe_wait(phk_encode_pipe_t* pipe, int64_t ticket);

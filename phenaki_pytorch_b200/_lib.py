@@ -9,6 +9,8 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("PHK_LIB") or os.path.join(_HERE, "libphk.so")  # PHK_LIB: an A/B build of the same ABI (tools/ only)
 
 PREC_F32, PREC_BF16, PREC_BF16X3 = 0, 1, 2
+VIDEO_F32, VIDEO_U8 = 0, 1  # PHK_VIDEO_*: a uint8 video means video.float() / 255 (ToTensor's correctly rounded quotient)
+VIDEO_DTYPES = {torch.float32: VIDEO_F32, torch.uint8: VIDEO_U8}
 RECON_LOSS_SCRATCH_BYTES = 2048  # PHK_RECON_LOSS_SCRATCH_BYTES (include/phk.h)
 HEAD_LOGITS, HEAD_EMBEDS, HEAD_SCORE = 0, 1, 2  # phk_maskgit_backward head kinds
 
@@ -116,6 +118,7 @@ PROTOTYPES = {
     "phk_prof_collect": [C.POINTER(C.c_double), C.POINTER(i64), C.POINTER(C.c_double), i32],
     "phk_layernorm": [vp, vp, vp, vp, vp, i64, i32, i32, i64, i64, i64, vp],
     "phk_patchify_ln": [vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp],
+    "phk_patchify_ln_u8": [vp, i32, i32, i32, i32, i32, i32, i32, i32, i32, i32, vp, vp, vp, i32, vp],
     "phk_gemm_f32": [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp, i64, i64, i64, vp],
     "phk_gemm_bf16": [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp, i64, i64, i64, i32, vp],
     "phk_gemm_bf16_x2": [vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp, i64, vp, i64, vp, i64, i64, i32, i32, vp, vp],
@@ -146,11 +149,12 @@ PROTOTYPES = {
     "phk_critic_scores": [vp, vp, vp, vp, vp, f32, f32, f32, vp, i64, i32, i64, i64, i64, vp],
     "phk_cfg_combine": [vp, vp, f32, vp, i64, vp],
     "phk_cvivit_workspace_bytes": [C.POINTER(CvivitT), i32, i32, i32],
-    "phk_cvivit_encode": [C.POINTER(CvivitT), vp, i32, i32, vp, vp, i64, i32, vp, vp, vp, vp, vp, vp],
+    "phk_cvivit_encode": [C.POINTER(CvivitT), vp, i32, i32, i32, vp, vp, i64, i32, vp, vp, vp, vp, vp, vp],
     "phk_cvivit_encode_host": [C.POINTER(CvivitT), vp, i32, i32, vp, vp, vp, vp, i64, i32, vp, vp],
     "phk_encode_pipe_create": [C.POINTER(vp), i32],
     "phk_encode_pipe_destroy": [vp],
-    "phk_encode_pipe_submit": [vp, C.POINTER(CvivitT), vp, i32, i32, vp, vp, vp, vp, i64, i32, vp, vp, C.POINTER(i64)],
+    "phk_encode_pipe_submit": [vp, C.POINTER(CvivitT), vp, i32, i32, i32, vp, vp, vp, vp, i64, i32, vp, vp,
+                               C.POINTER(i64)],
     "phk_encode_pipe_wait": [vp, i64],
     "phk_cvivit_decode_workspace_bytes": [C.POINTER(CvivitDecT), i32, i32, i32],
     "phk_cvivit_decode": [C.POINTER(CvivitDecT), vp, vp, i32, i32, vp, vp, i64, i32, vp, vp, vp, vp, vp],
@@ -254,6 +258,13 @@ def ptr(t):
     if t is None:
         return None
     return C.c_void_p(t.data_ptr())
+
+
+def video_dtype(t, name):
+    """The PHK_VIDEO_* code of a video tensor the encode reads (float32 or uint8); raises before anything is launched."""
+    if t.dtype not in VIDEO_DTYPES:
+        raise PhkError(f"{name} must be torch.float32 or torch.uint8, got {t.dtype}")
+    return VIDEO_DTYPES[t.dtype]
 
 
 def require_cuda(t, name, dtype=None):

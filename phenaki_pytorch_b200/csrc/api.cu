@@ -415,8 +415,8 @@ static int cvivit_encode_stacks(const phk_cvivit_t* m, int B, int Tp, int hh, in
   return transformer_forward(c, tf, out, nullptr, st);
 }
 
-static int cvivit_encode_impl(const phk_cvivit_t* m, const float* video, int32_t B, int32_t F, int64_t* ids,
-                              void* workspace, int64_t workspace_bytes, int32_t prec, const float* spatial_bias,
+static int cvivit_encode_impl(const phk_cvivit_t* m, const void* video, int video_dtype, int32_t B, int32_t F,
+                              int64_t* ids, void* workspace, int64_t workspace_bytes, int32_t prec, const float* spatial_bias,
                               float* tap_patch, float* tap_spatial, float* tap_temporal, float* tap_proj,
                               phk_stream_t s) {
   int Tp, hh, ww; int64_t R;
@@ -449,28 +449,33 @@ static int cvivit_encode_impl(const phk_cvivit_t* m, const float* video, int32_t
 
   // ---- to_patch_emb_first_frame / to_patch_emb (cvivit.py:542-549), rows land in (b,t,h,w) order
   const int C = m->channels, H = m->image_h, W = m->image_w;
+  auto patchify_ln = [&](int f0, int nt, int pt, const float* g, const float* b, void* out, int out_bf16) {
+    if (video_dtype == PHK_VIDEO_U8)
+      return phk_patchify_ln_u8((const uint8_t*)video, B, C, F, H, W, f0, nt, pt, m->patch_h, m->patch_w, g, b, out,
+                                out_bf16, s);
+    return phk_patchify_ln((const float*)video, B, C, F, H, W, f0, nt, pt, m->patch_h, m->patch_w, g, b, out, out_bf16,
+                           s);
+  };
   if (h16 && Tp > 1 && m->pf_w_h && m->pr_w_h) {
     // bf16 mode: both patch embeddings in ONE two-problem GEMM launch (16 + 128 tiles at cfg2: the first-frame
     // product alone occupied 16 SMs for 24 us).  A_rest at A, A_first behind it; outputs share P.
     const int64_t rows1 = (int64_t)B * hw, rows2 = (int64_t)B * (Tp - 1) * hw;
     char* A_first = (char*)A + ((rows2 * K2 * 2 + 255) / 256) * 256;
     PHK_REQUIRE((A_first - (char*)A) + rows1 * K1 * 2 <= R * K2 * 4, PHK_E_WORKSPACE, "cvivit_encode: workspace too small");
-    PHK_TRY(phk_patchify_ln(video, B, C, F, H, W, 0, 1, 1, m->patch_h, m->patch_w, m->pf_ln1_g, m->pf_ln1_b, A_first, 1, s));
-    PHK_TRY(phk_patchify_ln(video, B, C, F, H, W, 1, Tp - 1, m->patch_t, m->patch_h, m->patch_w, m->pr_ln1_g,
-                            m->pr_ln1_b, A, 1, s));
+    PHK_TRY(patchify_ln(0, 1, 1, m->pf_ln1_g, m->pf_ln1_b, A_first, 1));
+    PHK_TRY(patchify_ln(1, Tp - 1, m->patch_t, m->pr_ln1_g, m->pr_ln1_b, A, 1));
     PHK_TRY(phk_gemm_bf16_x2(A_first, K1, m->pf_w_h, K1, P, D, rows1, D, (int)K1, m->pf_b, A, K2, m->pr_w_h, K2,
                              P + rows1 * D, D, rows2, D, (int)K2, m->pr_b, s));
     PHK_TRY(phk_layernorm(P, m->pf_ln2_g, m->pf_ln2_b, x, nullptr, rows1, D, 0, hw, (int64_t)Tp * hw, 0, s));
     PHK_TRY(phk_layernorm(P + rows1 * D, m->pr_ln2_g, m->pr_ln2_b, x, nullptr, rows2, D, 0, (int64_t)(Tp - 1) * hw,
                           (int64_t)Tp * hw, hw, s));
   } else {
-  PHK_TRY(phk_patchify_ln(video, B, C, F, H, W, 0, 1, 1, m->patch_h, m->patch_w, m->pf_ln1_g, m->pf_ln1_b, A, h16, s));
+  PHK_TRY(patchify_ln(0, 1, 1, m->pf_ln1_g, m->pf_ln1_b, A, h16));
   PHK_TRY(linear(lin, A, K1, m->pf_w, m->pf_w_h, K1, P, D, (int64_t)B * hw, D, (int)K1, m->pf_b, nullptr, s));
   PHK_TRY(phk_layernorm(P, m->pf_ln2_g, m->pf_ln2_b, x, nullptr, (int64_t)B * hw, D, 0, hw, (int64_t)Tp * hw, 0, s));
   if (Tp > 1) {
     const int64_t rows = (int64_t)B * (Tp - 1) * hw;
-    PHK_TRY(phk_patchify_ln(video, B, C, F, H, W, 1, Tp - 1, m->patch_t, m->patch_h, m->patch_w, m->pr_ln1_g,
-                            m->pr_ln1_b, A, h16, s));
+    PHK_TRY(patchify_ln(1, Tp - 1, m->patch_t, m->pr_ln1_g, m->pr_ln1_b, A, h16));
     PHK_TRY(linear(lin, A, K2, m->pr_w, m->pr_w_h, K2, P, D, rows, D, (int)K2, m->pr_b, nullptr, s));
     PHK_TRY(phk_layernorm(P, m->pr_ln2_g, m->pr_ln2_b, x, nullptr, rows, D, 0, (int64_t)(Tp - 1) * hw,
                           (int64_t)Tp * hw, hw, s));
@@ -516,10 +521,11 @@ struct EncodeGraphKey {
   uint64_t table_hash;
   const void *video, *ids, *ws, *bias;
   int64_t ws_bytes;
-  int B, F, prec, device;
+  int video_dtype, B, F, prec, device;
   bool operator==(const EncodeGraphKey& o) const {
     return table_hash == o.table_hash && video == o.video && ids == o.ids && ws == o.ws && bias == o.bias &&
-           ws_bytes == o.ws_bytes && B == o.B && F == o.F && prec == o.prec && device == o.device;
+           ws_bytes == o.ws_bytes && video_dtype == o.video_dtype && B == o.B && F == o.F && prec == o.prec &&
+           device == o.device;
   }
 };
 struct EncodeGraphKeyHash {
@@ -527,7 +533,8 @@ struct EncodeGraphKeyHash {
     uint64_t h = k.table_hash;
     const uint64_t v[] = {(uint64_t)(uintptr_t)k.video, (uint64_t)(uintptr_t)k.ids, (uint64_t)(uintptr_t)k.ws,
                           (uint64_t)(uintptr_t)k.bias, (uint64_t)k.ws_bytes,
-                          ((uint64_t)k.B << 40) ^ ((uint64_t)k.F << 20) ^ ((uint64_t)k.prec << 8) ^ (uint64_t)k.device};
+                          ((uint64_t)k.B << 40) ^ ((uint64_t)k.F << 20) ^ ((uint64_t)k.prec << 8) ^ (uint64_t)k.device ^
+                              ((uint64_t)k.video_dtype << 60)};
     for (uint64_t x : v) h = (h ^ x) * 0x100000001b3ull;
     return (size_t)h;
   }
@@ -545,13 +552,15 @@ static uint64_t hash_transformer(const phk_transformer_t& T, uint64_t h) {
   return h;
 }
 
-extern "C" int phk_cvivit_encode(const phk_cvivit_t* m, const float* video, int32_t B, int32_t F, int64_t* ids,
-                                 void* workspace, int64_t workspace_bytes, int32_t prec, const float* spatial_bias,
-                                 float* tap_patch, float* tap_spatial, float* tap_temporal, float* tap_proj,
-                                 phk_stream_t s) {
+extern "C" int phk_cvivit_encode(const phk_cvivit_t* m, const void* video, int32_t video_dtype, int32_t B, int32_t F,
+                                 int64_t* ids, void* workspace, int64_t workspace_bytes, int32_t prec,
+                                 const float* spatial_bias, float* tap_patch, float* tap_spatial, float* tap_temporal,
+                                 float* tap_proj, phk_stream_t s) {
+  PHK_REQUIRE(video_dtype == PHK_VIDEO_F32 || video_dtype == PHK_VIDEO_U8, PHK_E_ARG,
+              "cvivit_encode: video_dtype must be PHK_VIDEO_F32 or PHK_VIDEO_U8");
   const bool taps = tap_patch || tap_spatial || tap_temporal || tap_proj;
   if (!m || taps || !spatial_bias || g_prof_on.load(std::memory_order_relaxed))
-    return cvivit_encode_impl(m, video, B, F, ids, workspace, workspace_bytes, prec, spatial_bias, tap_patch, tap_spatial,
+    return cvivit_encode_impl(m, video, video_dtype, B, F, ids, workspace, workspace_bytes, prec, spatial_bias, tap_patch, tap_spatial,
                               tap_temporal, tap_proj, s);
   static std::unordered_map<EncodeGraphKey, EncodeGraphEntry, EncodeGraphKeyHash> cache;
   static std::mutex mu;
@@ -562,7 +571,7 @@ extern "C" int phk_cvivit_encode(const phk_cvivit_t* m, const float* video, int3
   uint64_t th = fnv(m, sizeof(*m), 0xcbf29ce484222325ull);
   th = hash_transformer(m->spatial, th);
   th = hash_transformer(m->temporal, th);
-  const EncodeGraphKey key{th, video, ids, workspace, spatial_bias, workspace_bytes, B, F, prec, dev};
+  const EncodeGraphKey key{th, video, ids, workspace, spatial_bias, workspace_bytes, video_dtype, B, F, prec, dev};
   std::lock_guard<std::mutex> lk(mu);
   auto it = cache.find(key);
   if (it != cache.end() && it->second.exec) {
@@ -578,7 +587,7 @@ extern "C" int phk_cvivit_encode(const phk_cvivit_t* m, const float* video, int3
       }
       cache.emplace(key, EncodeGraphEntry{nullptr, 0, 1});
     }
-    return cvivit_encode_impl(m, video, B, F, ids, workspace, workspace_bytes, prec, spatial_bias, nullptr, nullptr,
+    return cvivit_encode_impl(m, video, video_dtype, B, F, ids, workspace, workspace_bytes, prec, spatial_bias, nullptr, nullptr,
                               nullptr, nullptr, s);
   }
   // second sighting: capture on the library's stream, instantiate, replay on the caller's stream
@@ -588,7 +597,7 @@ extern "C" int phk_cvivit_encode(const phk_cvivit_t* m, const float* video, int3
   cudaError_t e = cudaStreamBeginCapture(cap, cudaStreamCaptureModeThreadLocal);
   int rc = 0;
   if (e == cudaSuccess) {
-    rc = cvivit_encode_impl(m, video, B, F, ids, workspace, workspace_bytes, prec, spatial_bias, nullptr, nullptr, nullptr,
+    rc = cvivit_encode_impl(m, video, video_dtype, B, F, ids, workspace, workspace_bytes, prec, spatial_bias, nullptr, nullptr, nullptr,
                             nullptr, reinterpret_cast<phk_stream_t>(cap));
     e = cudaStreamEndCapture(cap, &graph);
   }
@@ -600,7 +609,7 @@ extern "C" int phk_cvivit_encode(const phk_cvivit_t* m, const float* video, int3
   if (e != cudaSuccess || rc != 0 || !exec) {
     cudaGetLastError();  // clear the sticky capture error; fall back for good
     broken = true;
-    return cvivit_encode_impl(m, video, B, F, ids, workspace, workspace_bytes, prec, spatial_bias, nullptr, nullptr,
+    return cvivit_encode_impl(m, video, video_dtype, B, F, ids, workspace, workspace_bytes, prec, spatial_bias, nullptr, nullptr,
                               nullptr, nullptr, s);
   }
   it->second.exec = exec;
@@ -620,7 +629,7 @@ extern "C" int phk_cvivit_encode_host(const phk_cvivit_t* m, const float* host_v
   cudaStream_t st = to_stream(s);
   const int64_t vbytes = (int64_t)B * m->channels * F * m->image_h * m->image_w * 4;
   PHK_CUDA(cudaMemcpyAsync(dev_video, host_video, vbytes, cudaMemcpyHostToDevice, st));
-  PHK_TRY(phk_cvivit_encode(m, (const float*)dev_video, B, F, dev_ids, workspace, workspace_bytes, prec, spatial_bias,
+  PHK_TRY(phk_cvivit_encode(m, dev_video, PHK_VIDEO_F32, B, F, dev_ids, workspace, workspace_bytes, prec, spatial_bias,
                             nullptr, nullptr, nullptr, nullptr, s));
   PHK_CUDA(cudaMemcpyAsync(host_ids, dev_ids, R * 8, cudaMemcpyDeviceToHost, st));
   PHK_CUDA(cudaStreamSynchronize(st));
@@ -734,17 +743,19 @@ extern "C" int phk_encode_pipe_destroy(phk_encode_pipe_t* p) {
   return 0;
 }
 
-extern "C" int phk_encode_pipe_submit(phk_encode_pipe_t* p, const phk_cvivit_t* m, const float* host_video, int32_t B,
-                                      int32_t F, int64_t* host_ids, void* dev_video_slots, int64_t* dev_ids_slots,
+extern "C" int phk_encode_pipe_submit(phk_encode_pipe_t* p, const phk_cvivit_t* m, const void* host_video,
+                                      int32_t video_dtype, int32_t B, int32_t F, int64_t* host_ids, void* dev_video_slots, int64_t* dev_ids_slots,
                                       void* workspace, int64_t workspace_bytes, int32_t prec,
                                       const float* spatial_bias, phk_stream_t s, int64_t* ticket) {
   int Tp, hh, ww; int64_t R;
   PHK_REQUIRE(p, PHK_E_ARG, "phk_encode_pipe_submit: null pipe");
   PHK_TRY(cvivit_dims(m, B, F, Tp, hh, ww, R));
   PHK_REQUIRE(host_video && host_ids && dev_video_slots && dev_ids_slots, PHK_E_ARG, "phk_encode_pipe_submit: null pointer");
+  PHK_REQUIRE(video_dtype == PHK_VIDEO_F32 || video_dtype == PHK_VIDEO_U8, PHK_E_ARG,
+              "phk_encode_pipe_submit: video_dtype must be PHK_VIDEO_F32 or PHK_VIDEO_U8");
   cudaStream_t st = to_stream(s);
   const int slot = (int)(p->next % p->depth);
-  const int64_t vbytes = (int64_t)B * m->channels * F * m->image_h * m->image_w * 4;
+  const int64_t vbytes = (int64_t)B * m->channels * F * m->image_h * m->image_w * (video_dtype == PHK_VIDEO_U8 ? 1 : 4);
   char* dv = (char*)dev_video_slots + (int64_t)slot * vbytes;
   int64_t* di = dev_ids_slots + (int64_t)slot * R;
   // the slot's previous occupant must have been consumed before it is overwritten (no-op for a fresh event)
@@ -752,7 +763,7 @@ extern "C" int phk_encode_pipe_submit(phk_encode_pipe_t* p, const phk_cvivit_t* 
   PHK_CUDA(cudaMemcpyAsync(dv, host_video, vbytes, cudaMemcpyHostToDevice, p->copy));
   PHK_CUDA(cudaEventRecord(p->h2d_done[slot], p->copy));
   PHK_CUDA(cudaStreamWaitEvent(st, p->h2d_done[slot], 0));
-  PHK_TRY(phk_cvivit_encode(m, (const float*)dv, B, F, di, workspace, workspace_bytes, prec, spatial_bias, nullptr,
+  PHK_TRY(phk_cvivit_encode(m, dv, video_dtype, B, F, di, workspace, workspace_bytes, prec, spatial_bias, nullptr,
                             nullptr, nullptr, nullptr, s));
   PHK_CUDA(cudaEventRecord(p->slot_free[slot], st));
   PHK_CUDA(cudaMemcpyAsync(host_ids, di, R * 8, cudaMemcpyDeviceToHost, st));

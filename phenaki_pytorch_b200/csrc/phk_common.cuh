@@ -18,6 +18,10 @@ void count_launch(int n = 1);
 // patchify_tma.cu: TMA-gathered patchify + LayerNorm; returns 0 when launched, 1 when the shape is not eligible
 int patchify_ln_tma_launch(const float* video, int B, int C, int F, int H, int W, int f0, int nt, int pt, int p1, int p2,
                            const float* ln_g, const float* ln_b, void* out, int out_bf16, cudaStream_t st);
+// the same for a uint8 video (each byte read as u / 255); 1 also when the bytes do not fit a box (p2 or W not a multiple
+// of 16, base not 16-byte aligned)
+int patchify_ln_tma_u8_launch(const uint8_t* video, int B, int C, int F, int H, int W, int f0, int nt, int pt, int p1,
+                              int p2, const float* ln_g, const float* ln_b, void* out, int out_bf16, cudaStream_t st);
 
 #define PHK_REQUIRE(cond, code, msg) \
   do { if (!(cond)) { ::phk::set_error(msg); return (code); } } while (0)

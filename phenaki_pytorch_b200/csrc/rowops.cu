@@ -95,9 +95,22 @@ __global__ void __launch_bounds__(256) ln_block_kernel(const float* __restrict__
 // pixels are gathered as p2-float contiguous runs (128 B for p2=32) straight from the
 // (B,C,F,H,W) video -- the single HBM-visible read of the encoder -- into shared memory,
 // normalised in place and written as one dense row of the GEMM A operand.
+//
+// The video is fp32 or uint8 (phk_patchify_ln_u8).  A byte u stands for the fp32 u / 255 correctly rounded, the
+// quotient torchvision's ToTensor computes; only the loads convert, the arithmetic is one piece of code for both.
 // ------------------------------------------------------------------------------------------
-template <bool VEC4>
-__global__ void __launch_bounds__(256) patchify_ln_kernel(const float* __restrict__ video, int C, int F, int H,
+__device__ __forceinline__ float video_unit(float v) { return v; }
+__device__ __forceinline__ float video_unit(uint8_t u) { return __fdiv_rn((float)u, 255.f); }  // IEEE division
+// 4 consecutive elements: fp32 as one 16-byte load (aligned), bytes one by one (any alignment)
+__device__ __forceinline__ float4 video_group(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
+__device__ __forceinline__ float4 video_group(const uint8_t* p) {
+  return make_float4(video_unit(__ldg(p)), video_unit(__ldg(p + 1)), video_unit(__ldg(p + 2)), video_unit(__ldg(p + 3)));
+}
+
+// VEC4: the mean sums 4-element groups ((x + y) + (z + w), groups i, i + 256, ... per thread); GROUP_VAR: so does the
+// variance -- the order of patchify_ln_reg_kernel and the TMA kernel, which a uint8 video takes when it cannot use them
+template <typename T, bool VEC4, bool GROUP_VAR>
+__global__ void __launch_bounds__(256) patchify_ln_kernel(const T* __restrict__ video, int C, int F, int H,
                                                           int W, int f0, int nt, int pt, int p1, int p2,
                                                           const float* __restrict__ g, const float* __restrict__ b,
                                                           void* __restrict__ out, int out_bf16) {
@@ -112,7 +125,7 @@ __global__ void __launch_bounds__(256) patchify_ln_kernel(const float* __restric
   const int bi = tok / nt;
   const int K = C * pt * p1 * p2;
   const int64_t plane = (int64_t)H * W;
-  const float* base = video + ((int64_t)bi * C * F + f0 + (int64_t)ti * pt) * plane + (int64_t)hi * p1 * W + wi * p2;
+  const T* base = video + ((int64_t)bi * C * F + f0 + (int64_t)ti * pt) * plane + (int64_t)hi * p1 * W + wi * p2;
   float s = 0.f;
   if (VEC4) {
     const int runs = p2 >> 2;  // float4 per patch row
@@ -122,7 +135,7 @@ __global__ void __launch_bounds__(256) patchify_ln_kernel(const float* __restric
       const int dy = r % p1; r /= p1;
       const int dt = r % pt;
       const int c = r / pt;
-      const float4 v = __ldg(reinterpret_cast<const float4*>(base + ((int64_t)c * F + dt) * plane + (int64_t)dy * W) + dx4);
+      const float4 v = video_group(base + ((int64_t)c * F + dt) * plane + (int64_t)dy * W + dx4 * 4);
       reinterpret_cast<float4*>(srow)[i] = v;
       s += (v.x + v.y) + (v.z + v.w);
     }
@@ -133,14 +146,22 @@ __global__ void __launch_bounds__(256) patchify_ln_kernel(const float* __restric
       const int dy = r % p1; r /= p1;
       const int dt = r % pt;
       const int c = r / pt;
-      const float v = __ldg(base + ((int64_t)c * F + dt) * plane + (int64_t)dy * W + dx);
+      const float v = video_unit(__ldg(base + ((int64_t)c * F + dt) * plane + (int64_t)dy * W + dx));
       srow[i] = v;
       s += v;
     }
   }
   const float mean = block_sum(s, red) / (float)K;
   float q = 0.f;
-  for (int i = threadIdx.x; i < K; i += blockDim.x) { const float d = srow[i] - mean; q += d * d; }
+  if (GROUP_VAR) {
+    for (int i = threadIdx.x; i < (K >> 2); i += blockDim.x) {
+      const float4 t = reinterpret_cast<const float4*>(srow)[i];
+      const float a = t.x - mean, bq = t.y - mean, c = t.z - mean, d = t.w - mean;
+      q += (a * a + bq * bq) + (c * c + d * d);
+    }
+  } else {
+    for (int i = threadIdx.x; i < K; i += blockDim.x) { const float d = srow[i] - mean; q += d * d; }
+  }
   const float rstd = rsqrtf(block_sum(q, red) / (float)K + 1e-5f);
   const int64_t orow = (int64_t)blockIdx.x * K;
   if (VEC4) {
@@ -205,17 +226,25 @@ __global__ void token_embed_kernel(const int64_t* __restrict__ ids, const float*
   }
 }
 
+// 4 consecutive elements of the register kernel: fp32 as one 16-byte load, uint8 as one 4-byte load through the table
+__device__ __forceinline__ float4 reg_group(const float* p, const float*) { return video_group(p); }
+__device__ __forceinline__ float4 reg_group(const uint8_t* p, const float* lut) {
+  const unsigned w = __ldg(reinterpret_cast<const unsigned*>(p));
+  return make_float4(lut[w & 255u], lut[(w >> 8) & 255u], lut[(w >> 16) & 255u], lut[w >> 24]);
+}
+
 // Persistent variant for p2 % 4 == 0 and K <= NJ * 1024: each thread owns the same NJ float4 positions of every token, so
 // its gather offsets are computed once, gamma / beta (2 x 24 KB per token at K = 6144 -- twice the video bytes when
 // every CTA re-reads them from L2) are staged once per CTA in shared memory, and the token itself stays in registers
 // between the two LayerNorm passes.  ~60 registers -> 4 CTAs per SM keep ~96 KB of video loads in flight per SM.
-template <int NJ>
-__global__ void __launch_bounds__(256, 4) patchify_ln_reg_kernel(const float* __restrict__ video, int C, int F, int H,
+// A uint8 video (4-byte aligned) reads 4 bytes per position, converted through a 256-entry table of u / 255.
+template <typename T, int NJ>
+__global__ void __launch_bounds__(256, 4) patchify_ln_reg_kernel(const T* __restrict__ video, int C, int F, int H,
                                                                  int W, int f0, int nt, int pt, int p1, int p2,
                                                                  const float* __restrict__ g, const float* __restrict__ b,
                                                                  void* __restrict__ out, int out_bf16, int tokens) {
   pdl_trigger();
-  extern __shared__ float4 sgb[];  // [K4] gamma, [K4] beta
+  extern __shared__ float4 sgb[];  // [K4] gamma, [K4] beta (uint8 video: then [256] floats u / 255)
   __shared__ float red[32];
   const int hh = H / p1, ww = W / p2;
   const int K = C * pt * p1 * p2, K4 = K >> 2;
@@ -237,6 +266,11 @@ __global__ void __launch_bounds__(256, 4) patchify_ln_reg_kernel(const float* __
       sgb[K4 + i] = __ldg(reinterpret_cast<const float4*>(b) + i);
     }
   }
+  float* lut = reinterpret_cast<float*>(sgb + 2 * K4);
+  if (sizeof(T) == 1) {
+    for (int i = threadIdx.x; i < 256; i += blockDim.x) lut[i] = video_unit((uint8_t)i);
+    __syncthreads();
+  }
   pdl_wait();  // gamma / beta are weights; the video may come from the previous kernel (decode -> encode chains)
   for (int token = blockIdx.x; token < tokens; token += gridDim.x) {
     int tok = token;
@@ -244,13 +278,13 @@ __global__ void __launch_bounds__(256, 4) patchify_ln_reg_kernel(const float* __
     const int hi = tok % hh; tok /= hh;
     const int ti = tok % nt;
     const int bi = tok / nt;
-    const float* base = video + ((int64_t)bi * C * F + f0 + (int64_t)ti * pt) * plane + (int64_t)hi * p1 * W + wi * p2;
+    const T* base = video + ((int64_t)bi * C * F + f0 + (int64_t)ti * pt) * plane + (int64_t)hi * p1 * W + wi * p2;
     float4 v[NJ];
     float s = 0.f;
 #pragma unroll
     for (int j = 0; j < NJ; ++j) {
       v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-      if (off[j] >= 0) v[j] = __ldg(reinterpret_cast<const float4*>(base + off[j]));
+      if (off[j] >= 0) v[j] = reg_group(base + off[j], lut);
     }
 #pragma unroll
     for (int j = 0; j < NJ; ++j) s += (v[j].x + v[j].y) + (v[j].z + v[j].w);
@@ -939,21 +973,85 @@ extern "C" int phk_patchify_ln(const float* video, int32_t B, int32_t C, int32_t
     static unsigned long long configured_mask = 0;
   const bool configured = device_configured(&configured_mask);
     if (!configured) {
-      PHK_CUDA(cudaFuncSetAttribute(patchify_ln_reg_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 49152));
-      PHK_CUDA(cudaFuncSetAttribute(patchify_ln_reg_kernel<6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 49152));
+      PHK_CUDA(cudaFuncSetAttribute(patchify_ln_reg_kernel<float, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 49152));
+      PHK_CUDA(cudaFuncSetAttribute(patchify_ln_reg_kernel<float, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 49152));
       mark_configured(&configured_mask);
     }
-    if (K <= 3 * 1024) PHK_CUDA(launch_pdl(patchify_ln_reg_kernel<3>, dim3(pgrid), dim3(256), gsmem, to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16, (int)grid));
-    else PHK_CUDA(launch_pdl(patchify_ln_reg_kernel<6>, dim3(pgrid), dim3(256), gsmem, to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16, (int)grid));
+    if (K <= 3 * 1024) PHK_CUDA(launch_pdl(patchify_ln_reg_kernel<float, 3>, dim3(pgrid), dim3(256), gsmem, to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16, (int)grid));
+    else PHK_CUDA(launch_pdl(patchify_ln_reg_kernel<float, 6>, dim3(pgrid), dim3(256), gsmem, to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16, (int)grid));
     PHK_LAUNCH_CHECK();
     return 0;
   }
   if (smem > 48 * 1024) {
-    PHK_CUDA(cudaFuncSetAttribute(patchify_ln_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 57344));
-    PHK_CUDA(cudaFuncSetAttribute(patchify_ln_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 57344));
+    PHK_CUDA(cudaFuncSetAttribute(patchify_ln_kernel<float, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 57344));
+    PHK_CUDA(cudaFuncSetAttribute(patchify_ln_kernel<float, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 57344));
   }
-  if (vec) PHK_CUDA(launch_pdl(patchify_ln_kernel<true>, dim3(grid), dim3(256), (size_t)(smem), to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16));
-  else PHK_CUDA(launch_pdl(patchify_ln_kernel<false>, dim3(grid), dim3(256), (size_t)(smem), to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16));
+  if (vec) PHK_CUDA(launch_pdl(patchify_ln_kernel<float, true, false>, dim3(grid), dim3(256), (size_t)(smem), to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16));
+  else PHK_CUDA(launch_pdl(patchify_ln_kernel<float, false, false>, dim3(grid), dim3(256), (size_t)(smem), to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16));
+  PHK_LAUNCH_CHECK();
+  return 0;
+}
+
+// The shapes patchify_ln_tma_kernel takes for an fp32 video (tma_launch in patchify_tma.cu), pointers aside
+static bool patchify_tma_f32_shape(int C, int W, int pt, int p1, int p2) {
+  const int K = C * pt * p1 * p2;
+  return p2 % 4 == 0 && W % 4 == 0 && (K * 4) % 128 == 0 && p1 <= 256 && p2 <= 256 && pt <= 256 && C <= 256 &&
+         (size_t)4 * K * sizeof(float) <= 100 * 1024;
+}
+
+// phk_patchify_ln of the fp32 video u / 255.  Whichever kernel serves the bytes adds in the order phk_patchify_ln uses on
+// a 16-byte-aligned fp32 video of the same shape, so the two agree bit for bit: the TMA kernel and the register kernel
+// share one order (4-element groups), the generic kernel sums the mean in that order and the variance element by
+// element (VEC4), or both element by element.  Where the bytes do not fit a TMA box or the register kernel's 4-byte
+// loads, the generic kernel serves them in the grouped order.
+extern "C" int phk_patchify_ln_u8(const uint8_t* video, int32_t B, int32_t C, int32_t F, int32_t H, int32_t W,
+                                  int32_t f0, int32_t nt, int32_t pt, int32_t p1, int32_t p2, const float* ln_g,
+                                  const float* ln_b, void* out, int32_t out_bf16, phk_stream_t s) {
+  Prof prof_(FAM_PATCHIFY, s, (double)B * C * nt * pt * H * W * 5.0);
+  PHK_REQUIRE(video && ln_g && ln_b && out, PHK_E_ARG, "phk_patchify_ln_u8: null pointer");
+  PHK_REQUIRE(B > 0 && C > 0 && F > 0 && H > 0 && W > 0 && pt > 0 && p1 > 0 && p2 > 0 && nt >= 0, PHK_E_ARG,
+              "phk_patchify_ln_u8: bad size");
+  PHK_REQUIRE(H % p1 == 0 && W % p2 == 0, PHK_E_SHAPE, "image size must be divisible by patch size (cvivit.py:271)");
+  PHK_REQUIRE(f0 >= 0 && f0 + nt * pt <= F, PHK_E_SHAPE, "frame range outside the video");
+  if (nt == 0) return 0;
+  const int K = C * pt * p1 * p2;
+  PHK_REQUIRE(K <= 14336, PHK_E_UNSUPPORTED, "patch feature size > 14336 floats (56 KB smem row)");
+  const unsigned grid = (unsigned)((int64_t)B * nt * (H / p1) * (W / p2));
+  const bool gb16 = ((reinterpret_cast<uintptr_t>(ln_g) | reinterpret_cast<uintptr_t>(ln_b)) & 15) == 0;
+  const bool vec = (p2 % 4 == 0) && (W % 4 == 0) && ((reinterpret_cast<uintptr_t>(out) & 15) == 0);
+  const bool grouped = vec && gb16 && (patchify_tma_f32_shape(C, W, pt, p1, p2) || K <= 6 * 1024);
+#ifndef PHK_CUDA_EMU
+  if (grouped) {  // TMA-gathered bytes (patchify_tma.cu; not part of the CPU executor's build: PHK_CUDA_EMU)
+    const int rc = patchify_ln_tma_u8_launch(video, B, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16,
+                                             to_stream(s));
+    if (rc == 0) { PHK_LAUNCH_CHECK(); return 0; }
+    if (rc != 1) return rc;
+  }
+#endif
+  if (grouped && K <= 6 * 1024 && (reinterpret_cast<uintptr_t>(video) & 3) == 0) {
+    PHK_REQUIRE((int64_t)C * F * H * W < (1LL << 31), PHK_E_UNSUPPORTED, "phk_patchify_ln_u8: one video exceeds 2^31 elements");
+    const unsigned pgrid = grid < 4u * kNumSMs ? grid : 4u * kNumSMs;
+    const size_t gsmem = (size_t)2 * K * sizeof(float) + 256 * sizeof(float);  // gamma, beta, the u / 255 table
+    static unsigned long long configured_mask = 0;
+    if (!device_configured(&configured_mask)) {
+      PHK_CUDA(cudaFuncSetAttribute(patchify_ln_reg_kernel<uint8_t, 3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 50176));
+      PHK_CUDA(cudaFuncSetAttribute(patchify_ln_reg_kernel<uint8_t, 6>, cudaFuncAttributeMaxDynamicSharedMemorySize, 50176));
+      mark_configured(&configured_mask);
+    }
+    if (K <= 3 * 1024) PHK_CUDA(launch_pdl(patchify_ln_reg_kernel<uint8_t, 3>, dim3(pgrid), dim3(256), gsmem, to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16, (int)grid));
+    else PHK_CUDA(launch_pdl(patchify_ln_reg_kernel<uint8_t, 6>, dim3(pgrid), dim3(256), gsmem, to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16, (int)grid));
+    PHK_LAUNCH_CHECK();
+    return 0;
+  }
+  const size_t smem = (size_t)K * sizeof(float);
+  if (smem > 48 * 1024) {
+    PHK_CUDA(cudaFuncSetAttribute(patchify_ln_kernel<uint8_t, true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 57344));
+    PHK_CUDA(cudaFuncSetAttribute(patchify_ln_kernel<uint8_t, true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 57344));
+    PHK_CUDA(cudaFuncSetAttribute(patchify_ln_kernel<uint8_t, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 57344));
+  }
+  if (grouped) PHK_CUDA(launch_pdl(patchify_ln_kernel<uint8_t, true, true>, dim3(grid), dim3(256), smem, to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16));
+  else if (vec) PHK_CUDA(launch_pdl(patchify_ln_kernel<uint8_t, true, false>, dim3(grid), dim3(256), smem, to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16));
+  else PHK_CUDA(launch_pdl(patchify_ln_kernel<uint8_t, false, false>, dim3(grid), dim3(256), smem, to_stream(s), video, C, F, H, W, f0, nt, pt, p1, p2, ln_g, ln_b, out, out_bf16));
   PHK_LAUNCH_CHECK();
   return 0;
 }

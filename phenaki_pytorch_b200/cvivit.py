@@ -268,10 +268,13 @@ class CViViT(nn.Module):
         return self._bias_cache[key]
 
     def encode_ids(self, video, taps=None):
-        """video (b,c,f,H,W) fp32 CUDA -> ids (b,T',H',W') int64.  ``taps``: optional dict that receives the
+        """video (b,c,f,H,W) fp32 or uint8 CUDA -> ids (b,T',H',W') int64.  A uint8 video stands for
+        ``video.float() / 255`` (ToTensor's convention, the quotient correctly rounded) and gives, bit for bit, the ids
+        and activations of that fp32 video, at a quarter of the bytes read.  ``taps``: optional dict that receives the
         intermediate activations (parity tests)."""
         lib = L.lib()
-        video = L.require_cuda(video, "video", torch.float32)
+        dtype = L.video_dtype(video, "video")
+        video = L.require_cuda(video, "video")
         b, c, f, *image_dims = video.shape
         assert tuple(image_dims) == self.image_size
         assert c == self.channels
@@ -298,21 +301,22 @@ class CViViT(nn.Module):
                 if self.lookup_free_quantization:
                     taps["proj"] = torch.empty((rows, self.vq.codebook_dim), dtype=torch.float32, device=video.device)
                 tap_ptrs = [L.ptr(taps.get(k)) for k in ("patch", "spatial", "temporal", "proj")]
-            L.check(lib.phk_cvivit_encode(C.byref(table), L.ptr(video), b, f, L.ptr(ids), L.ptr(ws), ws.numel(),
+            L.check(lib.phk_cvivit_encode(C.byref(table), L.ptr(video), dtype, b, f, L.ptr(ids), L.ptr(ws), ws.numel(),
                                           self.precision, L.ptr(bias), *tap_ptrs, L.stream_ptr()),
                     "phk_cvivit_encode")
             return ids.clone()
 
     def encode_host_iter(self, videos, device=None, depth=2):
-        """Tokenises a stream of HOST batches: `videos` yields (b,c,f,H,W) fp32 CPU tensors of one shape (pinned memory
-        gives the full PCIe rate); yields the (b,T',H',W') int64 ids of each batch as CPU tensors, in order.  The H2D
-        copy of batch i+1 overlaps the encode of batch i (phk_encode_pipe_*); nothing is staged by torch."""
+        """Tokenises a stream of HOST batches: `videos` yields (b,c,f,H,W) fp32 or uint8 CPU tensors of one shape and
+        dtype (pinned memory gives the full PCIe rate; uint8 frames, as ``encode_ids`` reads them, copy a quarter of the
+        bytes); yields the (b,T',H',W') int64 ids of each batch as CPU tensors, in order.  The H2D copy of batch i+1
+        overlaps the encode of batch i (phk_encode_pipe_*); nothing is staged by torch."""
         lib = L.lib()
         device = torch.device(device) if device is not None else next(self.parameters()).device
         assert device.type == "cuda", "this framework has no CPU path"
         pipe = C.c_void_p()
         L.check(lib.phk_encode_pipe_create(C.byref(pipe), depth), "phk_encode_pipe_create")
-        shape, inflight, submitted = None, [], 0
+        shape, dtype, inflight, submitted = None, None, [], 0
         try:
             with torch.cuda.device(device):
                 table = self._table()
@@ -324,28 +328,31 @@ class CViViT(nn.Module):
                     return host_ids
 
                 for video in videos:
-                    if video.is_cuda or video.dtype != torch.float32:
-                        raise L.PhkError("encode_host_iter takes fp32 CPU batches (use forward() for device tensors)")
+                    if video.is_cuda or video.dtype not in L.VIDEO_DTYPES:
+                        raise L.PhkError("encode_host_iter takes fp32 or uint8 CPU batches (use forward() for device "
+                                         "tensors)")
                     video = video.contiguous()
                     if shape is None:
-                        shape = tuple(video.shape)
+                        shape, dtype = tuple(video.shape), video.dtype
                         b, c, f, *image_dims = shape
                         assert tuple(image_dims) == self.image_size and c == self.channels
                         assert (f - 1) % self.temporal_patch_size == 0
                         tp, hh, ww = self.get_video_patch_shape(f)
-                        stage = torch.empty((depth, *shape), dtype=torch.float32, device=device)
+                        stage = torch.empty((depth, *shape), dtype=dtype, device=device)
                         dev_ids = torch.empty((depth, b, tp, hh, ww), dtype=torch.int64, device=device)
                         host = [torch.empty((b, tp, hh, ww), dtype=torch.int64).pin_memory() for _ in range(depth)]
                         nbytes = lib.phk_cvivit_workspace_bytes(C.byref(table), b, f, self.precision)
                         ws = self._ws.get_for("phk_cvivit_workspace_bytes", nbytes, device)
                     assert tuple(video.shape) == shape, "all batches of one stream must have the same shape"
+                    assert video.dtype == dtype, "all batches of one stream must have the same dtype"
                     if len(inflight) == depth:
                         yield retire().clone()
                     ticket = C.c_int64()
                     slot_host = host[submitted % depth]
-                    L.check(lib.phk_encode_pipe_submit(pipe, C.byref(table), L.ptr(video), b, f, L.ptr(slot_host),
-                                                       L.ptr(stage), L.ptr(dev_ids), L.ptr(ws), ws.numel(),
-                                                       self.precision, L.ptr(bias), L.stream_ptr(), C.byref(ticket)),
+                    L.check(lib.phk_encode_pipe_submit(pipe, C.byref(table), L.ptr(video), L.VIDEO_DTYPES[dtype], b, f,
+                                                       L.ptr(slot_host), L.ptr(stage), L.ptr(dev_ids), L.ptr(ws),
+                                                       ws.numel(), self.precision, L.ptr(bias), L.stream_ptr(),
+                                                       C.byref(ticket)),
                             "phk_encode_pipe_submit")
                     assert ticket.value == submitted
                     submitted += 1
