@@ -3,21 +3,21 @@
 // A, W bf16, K-major (row-major [rows, K]); fp32 accumulation in registers.
 //
 // gemm_bf16_kernel<EPI, DUAL> behind phk_gemm_bf16 / phk_gemm_bf16_x2 / _qkv / _qnorm, DUAL = two independent problems
-// in one launch.  Persistent (one CTA per SM, 128 x 128 tiles, static round-robin tile scheduler, m-fastest so
-// concurrent CTAs share the W tile in L2 while the A panel stays L2-resident).  Two bodies:
-// * quadrant (single-problem instances, 640 threads):
+// in one launch.  Persistent (one CTA per SM, 128 x 128 tiles or 64 x 128 units, static round-robin scheduler,
+// m-fastest so concurrent CTAs share the W tile in L2 while the A panel stays L2-resident).  Two bodies:
+// * quadrant (bf16 single-problem instances <1, false> and <3, false>, 640 threads):
 //   warpgroup 0     TMA producer (one thread): cp.async.bulk.tensor.2d (SWIZZLE_128B) stages 128x64 A and W tiles into
 //                   a 4-deep shared-memory ring; out-of-bounds rows / the K tail are zero-filled by the TMA unit.
 //   warpgroups 1..4 each multiplies one 64 x 64 quadrant of the tile (wgmma.m64n64k16, both operands from shared
 //                   memory), writes it into the epilogue's staging layout, and then all sixteen warps run the epilogue
 //                   (four per 32-row group, each a quarter of the columns) while the producer fills the ring for the
 //                   next tile.
-// * ping-pong (two-problem instances and gemm_bf16_geglu_kernel, 384 threads; see gemm_pingpong below): two MMA
-//   warpgroups take whole tiles in turn as m64n128k16 row halves and run the epilogue from the accumulator registers
-//   while the other one runs its main loop.  Measured faster where a CTA gets several tiles, slower where it gets one.
-// Epilogues: 0 fp32 (+bias, +residual, row map) -- through the TMA unit when the row map is the identity: the
-//              residual tile is bulk-loaded into SWIZZLE_128B staging boxes during the main loop and the result tile
-//              bulk-stored from them; otherwise staged in a padded smem tile and written with coalesced rows.  Two
+// * ping-pong (384 threads; see gemm_pingpong below): two MMA warpgroups take whole units in turn as m64n128k16 row
+//   halves and run the epilogue while the other one runs its main loop.  128 x 128 tiles for the two-problem instances
+//   and gemm_bf16_geglu_kernel; 64 x 128 units for the fp32 single-problem instance <0, false> (out-projection, FF2).
+// Epilogues: 0 fp32 (+residual, +bias, row map), (acc + residual) + bias -- single problem: through the TMA unit when
+//              the row map is the identity: the residual tile is bulk-loaded into the warpgroup's SWIZZLE_128B staging
+//              boxes during the main loop and the result bulk-stored from them; otherwise from the registers.  Two
 //              problems: fp32 (+bias) from the registers.
 //            1 bf16 (+bias)
 //            2 GEGLU (attention.py:40-43) on W rows packed [64 value rows | 64 gate rows] per 128-column tile ->
@@ -47,9 +47,9 @@ struct EpiParams {
   void* C; int64_t ldc; int64_t M; int N; int K;
   const float* bias; const float* residual;
   int64_t seg_len, seg_stride, seg_off;
-  int m_tiles, n_tiles;
+  int m_tiles, n_tiles;  // row and column units of the launch (64 or 128 rows, 128 columns)
   // fp32 epilogue through the TMA unit (identity row map, C 16-B aligned, residual == C or none): C as a tensor map
-  // with [128 rows x 32 floats] SWIZZLE_128B boxes; the residual tile is bulk-LOADED into the staging boxes while the
+  // with [64 rows x 32 floats] SWIZZLE_128B boxes; the residual tile is bulk-LOADED into the staging boxes while the
   // main loop runs and the finished tile is bulk-STORED from them, so the epilogue warps issue no global accesses
   int tma_epi;
   // epilogue 3 (self-attention operands, attention.py:146-157): bf16 output; columns [0, norm_cols) are l2-normalised
@@ -63,25 +63,15 @@ struct EpiParams {
 __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, %0;" ::"n"(EPI_WARPS * 32) : "memory"); }
 
 // One warpgroup's 64 x 64 accumulator quadrant (rows rq.., columns cq.. of the tile; warp w of the warpgroup) into the
-// epilogue's staging layout, added onto the residual already staged there when `add` is set.  BOX: the four
-// [128 rows x 128 B] SWIZZLE_128B boxes of the TMA epilogue; otherwise rows of CPAD floats.
-template <bool BOX>
-__device__ __forceinline__ void acc_to_stage(const float (&d)[32], uint8_t* stage, int rq, int cq, int w, int lane,
-                                             bool add) {
+// epilogue's staging rows of CPAD floats.
+__device__ __forceinline__ void acc_to_stage(const float (&d)[32], float* stage, int rq, int cq, int w, int lane) {
   const int r0 = rq + 16 * w + (lane >> 2);
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const int c = cq + 8 * j + 2 * (lane & 3);
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int r = r0 + 8 * h;
-      float2* dst = BOX ? reinterpret_cast<float2*>(stage + (c >> 5) * (GM * 128) + r * 128 +
-                                                    ((((c & 31) >> 2) ^ (r & 7)) << 4) + (c & 3) * 4)
-                        : reinterpret_cast<float2*>(reinterpret_cast<float*>(stage) + r * CPAD + c);
-      float2 v = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
-      if (add) { const float2 o = *dst; v.x += o.x; v.y += o.y; }
-      *dst = v;
-    }
+    for (int h = 0; h < 2; ++h)
+      *reinterpret_cast<float2*>(stage + (r0 + 8 * h) * CPAD + c) = make_float2(d[4 * j + 2 * h], d[4 * j + 2 * h + 1]);
   }
 }
 
@@ -116,37 +106,6 @@ __device__ __forceinline__ float head_scale(float c, float inv, float sc) { retu
 // acc_to_stage.
 // ---------------------------------------------------------------------------------------------------
 
-// Residual prefetch: while the main loop of the tile runs, pull the residual chunk into the staging buffer with
-// coalesced 512-B row loads (the previous chunk's write-out finished at its closing barrier).
-template <int EPI>
-__device__ __forceinline__ bool epi_residual_prefetch(const EpiParams& p, float* cstage, int64_t m0, int n0, int ew,
-                                                      int lane) {
-  const bool res_vec = EPI == 0 && p.residual && (p.ldc % 4 == 0) && (p.N % 4 == 0) &&
-                       ((reinterpret_cast<uintptr_t>(p.residual) & 15) == 0);
-  if (res_vec) {
-    const int col = n0 + lane * 4;
-    const uint32_t seg_len = (uint32_t)p.seg_len;
-#pragma unroll 1
-    for (int rb = 0; rb < GM / EPI_WARPS; rb += 8) {
-      float4 rv[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const int r = (rb + u) * EPI_WARPS + ew;
-        const uint32_t m = (uint32_t)m0 + r;
-        uint32_t orow = m;
-        if (seg_len > 0) { const uint32_t q = m / seg_len; orow = q * (uint32_t)p.seg_stride + (uint32_t)p.seg_off + (m - q * seg_len); }
-        rv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (m < (uint32_t)p.M && col < p.N) rv[u] = *reinterpret_cast<const float4*>(p.residual + (int64_t)orow * p.ldc + col);
-      }
-#pragma unroll
-      for (int u = 0; u < 8; ++u)
-        *reinterpret_cast<float4*>(cstage + ((rb + u) * EPI_WARPS + ew) * CPAD + lane * 4) = rv[u];
-    }
-    epi_bar_sync();  // residual chunk complete before the row-per-thread accumulate
-  }
-  return res_vec;
-}
-
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
   asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
                ::"l"(map), "r"(src), "r"(c0), "r"(c1)
@@ -154,132 +113,17 @@ __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t sr
 }
 __device__ __forceinline__ void tma_store_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void tma_store_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_store_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// fp32 chunk (128 rows x 128 columns) through the TMA unit.  Staging = four [128 rows x 128 B] SWIZZLE_128B boxes (one
-// per 32-column part): thread (row r, part c) owns exactly one 128-byte swizzled row of box c, so its eight 16-byte
-// accesses are conflict-free and need no other thread's data.  Order per chunk:
-//   store thread: wait until the previous chunk's bulk stores have READ the boxes; barrier;
-//   store thread: bulk-load the residual tile (C itself: x = f(x) + x) into the boxes (mbarrier `bar_res`);
-//   all: after the main loop, accumulator quadrants + residual into the boxes (acc_to_stage<true>); barrier;
-//        own swizzled row + bias, back into the boxes; fence.proxy.async; barrier;  store thread: four bulk stores.
-// part 1, BEFORE the accumulator-ready wait (overlaps the main loop)
-__device__ __forceinline__ void epi_tma_begin(const EpiParams& p, uint32_t stage_s, uint32_t bar_res, int m0, int n0,
-                                              int ew, int lane) {
-  const bool store_thread = ew == 0 && lane == 0;
-  if (store_thread) tma_store_wait_read();
-  epi_bar_sync();  // the boxes are free (the previous chunk's bulk stores have read them)
-  if (p.residual && store_thread) {
-    mbar_expect_tx(bar_res, 4 * GM * 128);
-#pragma unroll
-    for (int c = 0; c < 4; ++c) tma_load_2d(&p.tmC, bar_res, stage_s + c * (GM * 128), n0 + 32 * c, m0);
-  }
-}
-// part 2, after the accumulator (+ residual) has been staged in the boxes
-__device__ __forceinline__ void epi_tma_finish(const EpiParams& p, uint8_t* stage, uint32_t stage_s, int m0, int n0,
-                                               int ew, int lg, int part, int lane) {
-  const int r = lg * 32 + lane;
-  float4* box_row = reinterpret_cast<float4*>(stage + part * (GM * 128) + r * 128);
-  const int col0 = n0 + part * 32;
-  const bool bias_vec = p.bias && (col0 + 31 < p.N) && ((reinterpret_cast<uintptr_t>(p.bias) & 15) == 0);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    const int pos = j ^ (r & 7);
-    float4 o = box_row[pos];
-    if (bias_vec) {
-      const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + col0) + j);
-      o.x += bv.x; o.y += bv.y; o.z += bv.z; o.w += bv.w;
-    } else if (p.bias) {
-      const int c = col0 + 4 * j;
-      if (c < p.N) o.x += __ldg(p.bias + c);
-      if (c + 1 < p.N) o.y += __ldg(p.bias + c + 1);
-      if (c + 2 < p.N) o.z += __ldg(p.bias + c + 2);
-      if (c + 3 < p.N) o.w += __ldg(p.bias + c + 3);
-    }
-    box_row[pos] = o;
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA unit
-  epi_bar_sync();  // whole chunk staged
-  if (ew == 0 && lane == 0) {
-#pragma unroll
-    for (int c = 0; c < 4; ++c)
-      if (n0 + 32 * c < p.N) tma_store_2d(&p.tmC, stage_s + c * (GM * 128), n0 + 32 * c, m0);  // OOB rows / columns are clipped
-    tma_store_commit();
-  }
-}
-
-// Writes out one chunk staged as CPAD rows (accumulator + the prefetched residual when res_vec).
+// Writes out one chunk staged as CPAD rows (quadrant body: bf16 epilogues 1 and 3).
 template <int EPI>
-__device__ __forceinline__ void epi_chunk(const EpiParams& p, float* cstage, int64_t m0, int n0, bool res_vec, int ew,
-                                          int lane) {
+__device__ __forceinline__ void epi_chunk(const EpiParams& p, float* cstage, int64_t m0, int n0, int ew, int lane) {
+  static_assert(EPI == 1 || EPI == 3, "the fp32 epilogue runs on the ping-pong body");
   const uint32_t seg_len = (uint32_t)p.seg_len;
   // ---- coalesced write-out: one row per warp instruction ----
   constexpr int RPW = GM / EPI_WARPS;  // rows per warp
   const int ncol0 = n0;
   const int nlim = p.N;
-  if (EPI == 0) {
-    const int col = ncol0 + lane * 4;
-    const bool vec = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) && (col + 3 < nlim);
-    float4 bv = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (p.bias) {
-      if (col < nlim) bv.x = __ldg(p.bias + col);
-      if (col + 1 < nlim) bv.y = __ldg(p.bias + col + 1);
-      if (col + 2 < nlim) bv.z = __ldg(p.bias + col + 2);
-      if (col + 3 < nlim) bv.w = __ldg(p.bias + col + 3);
-    }
-    // fast path (whole chunk uniform): vector rows, residual already folded in (or absent), full M tile
-    const bool fast = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0) && (p.N % 4 == 0) &&
-                      (res_vec || !p.residual) && (m0 + GM <= p.M) && seg_len == 0;
-    if (fast) {
-      if (col < nlim) {
-        float* cbase = reinterpret_cast<float*>(p.C) + (m0 + ew) * p.ldc + col;
-        const float* sbase = cstage + ew * CPAD + lane * 4;
-#pragma unroll 1
-        for (int rb = 0; rb < RPW; rb += 8) {
-          float4 o[8];
-#pragma unroll
-          for (int u = 0; u < 8; ++u) o[u] = *reinterpret_cast<const float4*>(sbase + (rb + u) * EPI_WARPS * CPAD);
-#pragma unroll
-          for (int u = 0; u < 8; ++u) {
-            o[u].x += bv.x; o[u].y += bv.y; o[u].z += bv.z; o[u].w += bv.w;
-            *reinterpret_cast<float4*>(cbase + (int64_t)(rb + u) * EPI_WARPS * p.ldc) = o[u];
-          }
-        }
-      }
-    } else
-    // general path, 8 rows per batch: all residual loads of a batch are issued before the first store (C may
-    // alias the residual -- in-place x = f(x) + x -- so the compiler cannot reorder them itself)
-#pragma unroll 1
-    for (int rb = 0; rb < RPW; rb += 8) {
-      int64_t off[8];
-      float4 rv[8];
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        const int r = (rb + u) * EPI_WARPS + ew;
-        const uint32_t m = (uint32_t)m0 + r;
-        uint32_t orow = m;
-        if (seg_len > 0) { const uint32_t q = m / seg_len; orow = q * (uint32_t)p.seg_stride + (uint32_t)p.seg_off + (m - q * seg_len); }
-        off[u] = (m < (uint32_t)p.M && col < nlim) ? (int64_t)orow * p.ldc + col : -1;
-        rv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (!res_vec && vec && p.residual && off[u] >= 0) rv[u] = *reinterpret_cast<const float4*>(p.residual + off[u]);
-      }
-#pragma unroll
-      for (int u = 0; u < 8; ++u) {
-        if (off[u] < 0) continue;
-        const int r = (rb + u) * EPI_WARPS + ew;
-        float4 o = *reinterpret_cast<const float4*>(cstage + r * CPAD + lane * 4);
-        o.x += bv.x + rv[u].x; o.y += bv.y + rv[u].y; o.z += bv.z + rv[u].z; o.w += bv.w + rv[u].w;
-        float* crow = reinterpret_cast<float*>(p.C) + off[u];
-        if (vec) {
-          *reinterpret_cast<float4*>(crow) = o;
-        } else {  // ragged N / unaligned C: scalar tail
-          const float ov[4] = {o.x, o.y, o.z, o.w};
-          for (int j = 0; j < 4; ++j)
-            if (col + j < nlim) crow[j] = ov[j] + ((p.residual && !res_vec) ? p.residual[off[u] + j] : 0.f);
-        }
-      }
-    }
-  } else if (EPI == 3) {
+  if (EPI == 3) {
     // bf16 attention operands: lane owns columns [4 lane, 4 lane + 4) of the chunk; a head is 64 columns = 16 lanes, so
     // the squared norm of a (row, head) is a 4-step xor-shuffle over the half warp
     const int col = ncol0 + lane * 4;
@@ -338,19 +182,19 @@ __device__ __forceinline__ void epi_chunk(const EpiParams& p, float* cstage, int
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Quadrant body (single-problem instances): 128 x 128 tiles, four MMA / epilogue warpgroups of one 64 x 64 quadrant each
+// Quadrant body (bf16 single-problem instances): 128 x 128 tiles, four MMA / epilogue warpgroups of one 64 x 64 quadrant
+// each
 // ---------------------------------------------------------------------------------------------------
 template <int EPI>
 __device__ __forceinline__ void gemm_quadrant(const CUtensorMap& tmA, const CUtensorMap& tmB, const EpiParams& p) {
+  static_assert(EPI == 1 || EPI == 3, "the fp32 epilogue runs on the ping-pong body");
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B atoms need 1024-B alignment
   uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
   const uint32_t sA = base, sB = base + GSTAGES * STAGE_BYTES;
   float* cstage = reinterpret_cast<float*>(base_ptr + RING_BYTES);
-  const uint32_t bars = base + RING_BYTES + CSTAGE_BYTES;
-  // full[s] @ +8s ; empty[s] @ +8(S+s) ; residual landed @ +16S
-  const uint32_t bar_res = bars + 16 * GSTAGES;
+  const uint32_t bars = base + RING_BYTES + CSTAGE_BYTES;  // full[s] @ +8s ; empty[s] @ +8(S+s)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int num_tiles = p.m_tiles * p.n_tiles;
   // tile schedule: round-robin, m-fastest
@@ -369,7 +213,6 @@ __device__ __forceinline__ void gemm_quadrant(const CUtensorMap& tmA, const CUte
       mbar_init(bars + 8 * s, 1);
       mbar_init(bars + 8 * (GSTAGES + s), EPI_WARPS);  // one arrival per MMA warp
     }
-    mbar_init(bar_res, 1);                               // residual tile landed (TMA epilogue)
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
@@ -396,21 +239,14 @@ __device__ __forceinline__ void gemm_quadrant(const CUtensorMap& tmA, const CUte
   } else {
     // ===================== MMA + epilogue: warps 4..19 =====================
     const int ew = warp - 4;        // 0..15: rows ew, ew+16, ... in the coalesced write-out
-    const int lg = warp & 3;        // 32-row group whose rows this warp drains (one row per lane)
-    const int part = ew >> 2;       // which quarter of the tile's columns this warp drains
     const int wg = ew >> 2;         // MMA warpgroup: quadrant rows 64 (wg & 1).., columns 64 (wg >> 1)..
     const int rq = (wg & 1) * 64, cq = (wg >> 1) * 64;
-    uint32_t res_phase = 0;
     int stage = 0;
     uint32_t phase = 0;
     for (int it = 0; it < my_tiles; ++it) {
       int m0, n0;
       tile_of(it, m0, n0);
-      const bool tma = EPI == 0 && p.tma_epi;
-      bool res_vec = false;
-      if (tma) epi_tma_begin(p, base + RING_BYTES, bar_res, m0, n0, ew, lane);
-      else if (EPI == 0) res_vec = epi_residual_prefetch<EPI>(p, cstage, m0, n0, ew, lane);
-      else epi_bar_sync();  // the previous tile's epilogue has left the staging memory
+      epi_bar_sync();  // the previous tile's epilogue has left the staging memory
       // ---- main loop: this warpgroup's 64 x 64 quadrant ----
       float d[32];
 #pragma unroll
@@ -429,56 +265,77 @@ __device__ __forceinline__ void gemm_quadrant(const CUtensorMap& tmA, const CUte
         if (lane == 0) mbar_arrive(bars + 8 * (GSTAGES + stage));  // this warp's reads of the slot are complete
         if (++stage == GSTAGES) { stage = 0; phase ^= 1; }
       }
-      // ---- accumulator -> staging (onto the residual where one was staged) ----
-      if (tma) {
-        if (p.residual) { mbar_wait(bar_res, res_phase); res_phase ^= 1; }
-        acc_to_stage<true>(d, reinterpret_cast<uint8_t*>(cstage), rq, cq, ew & 3, lane, p.residual != nullptr);
-      } else {
-        acc_to_stage<false>(d, reinterpret_cast<uint8_t*>(cstage), rq, cq, ew & 3, lane, res_vec);
-      }
+      acc_to_stage(d, cstage, rq, cq, ew & 3, lane);
       epi_bar_sync();  // whole tile staged
-      if (tma)
-        epi_tma_finish(p, reinterpret_cast<uint8_t*>(cstage), base + RING_BYTES, m0, n0, ew, lg, part, lane);
-      else
-        epi_chunk<EPI>(p, cstage, m0, n0, res_vec, ew, lane);
+      epi_chunk<EPI>(p, cstage, m0, n0, ew, lane);
     }
-    if (EPI == 0 && ew == 0 && lane == 0) tma_store_wait_read();  // staging read out before the CTA exits (the writes complete with the grid)
   }
   __syncthreads();
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Ping-pong body: the GEGLU products (FF1 of every feed-forward block, 22 column tiles) and the two-problem launches
-// (q + k,v projections, patch embeddings) -- the products where a CTA gets several tiles
+// Ping-pong body: the GEGLU products (FF1 of every feed-forward block, 22 column tiles), the two-problem launches
+// (q + k,v projections, patch embeddings) and the fp32 single-problem products (out-projection and FF2 + residual)
 // ---------------------------------------------------------------------------------------------------
 // Warpgroup 0 is the TMA producer (one thread; the warpgroup gives its registers away to the MMA warpgroups) feeding a
-// GG_STAGES-deep ring in the order the CTA's tiles are consumed.  Warpgroups 1 and 2 take the CTA's tiles in turn: each
-// multiplies a whole 128 x 128 tile as two m64n128k16 row halves that share every W slice (6 KB of operands per 64
+// GG_STAGES-deep ring in the order the CTA's units are consumed.  Warpgroups 1 and 2 take the CTA's units in turn: each
+// multiplies a whole UM x 128 unit as UM / 64 m64n128k16 row halves that share every W slice (6 KB of operands per 64
 // tensor-core clocks instead of 4 KB per 32 for a 64 x 64 quadrant), keeps one k-block of MMAs in flight, and runs the
-// epilogue straight from its accumulator registers while the other warpgroup runs the next tile's main loop.  A
+// epilogue while the other warpgroup runs the next unit's main loop, so only the CTA's last epilogue is exposed.  A
 // named-barrier handshake orders the main loops, so the two warpgroups never interleave their MMAs.  Per output element
 // the k-order (k-blocks of 64 in order, k = 16 steps in order) is that of the quadrant body.
+// UM = 128 for the GEGLU and two-problem products.  UM = 64 for the fp32 single-problem products: at 4608 x 512 the
+// 288 units make 2.2 per CTA (a makespan of 1.5 tile-times) where 144 128-row tiles make 1.1 (two tile-times, the
+// machine 55 % busy).  The price: 24 KB of operands per k-block for half a tile's MMAs (32 KB for a whole 128-row
+// tile), which costs at long K (the single patch embedding, K = 6144, is slower than on 128-row tiles).
 // DUAL: two independent problems (own operands, output, N and K) in ONE launch, tiles of problem 1 first.  The q and
 // k,v projections of a self-attention block read different inputs (LayerNorm(x) vs raw x, attention.py:140-144) and
 // are each a single wave of tiles; together they make 3-4 tiles per CTA.
 constexpr int GG_STAGES = 6;
 constexpr int GG_THREADS = 384;
 constexpr int GG_PRODUCER_REGS = 40, GG_CONSUMER_REGS = 232;  // 128 x 40 + 256 x 232 <= 64 K registers
-constexpr int GG_SMEM_TOTAL = GG_STAGES * 2 * STAGE_BYTES + 128 /*barriers*/ + 1024 /*manual 1024-B alignment*/;
+constexpr int UNIT_M = 64;      // rows of a unit of the fp32 single-problem products
 constexpr int GG_BAR_TURN = 1;  // named barriers 1, 2: main-loop turn of MMA warpgroup 0, 1
+constexpr int GG_BAR_EPI = 3;   // named barriers 3, 4: staging area of MMA warpgroup 0, 1
+// Shared memory of a ping-pong launch: the ring, then one staging area per MMA warpgroup, then the barriers
+template <int UM, class Epilogue>
+constexpr int pingpong_smem() {
+  return GG_STAGES * (UM * GK * 2 + STAGE_BYTES) + 2 * Epilogue::kStageBytes + 128 /*barriers*/ +
+         1024 /*manual 1024-B alignment*/;
+}
 
-// The accumulator of a ping-pong tile: acc[h][4j + 2i + e] = (row 64h + 16w + lane/4 + 8i, column 8j + 2(lane%4) + e).
-typedef float PingPongAcc[2][64];
+// The accumulator of a ping-pong unit: acc[h][4j + 2i + e] = (row 64h + 16w + lane/4 + 8i, column 8j + 2(lane%4) + e).
+template <int UM>
+using PingPongAcc = float[UM / 64][64];
 
-template <bool DUAL, class Epilogue>
+// An MMA warp as its epilogue sees it: warp w of MMA warpgroup wg, and the warpgroup's staging area in shared memory
+// (Epilogue::kStageBytes at `stage`, shared address stage_s) with the mbarrier `bar` of its bulk loads (phase `phase`).
+struct PingPongWarp {
+  int wg, w, lane;
+  uint8_t* stage;
+  uint32_t stage_s, bar, phase;
+};
+
+// Epilogues straight from the accumulator registers: no staging area, nothing to load ahead of the main loop.
+struct RegisterEpilogue {
+  static constexpr int kStageBytes = 0;
+  __device__ __forceinline__ void prefetch(const EpiParams&, int, int, const PingPongWarp&) const {}
+};
+constexpr int GG_SMEM_TOTAL = pingpong_smem<128, RegisterEpilogue>();
+
+template <bool DUAL, int UM, class Epilogue>
 __device__ __forceinline__ void gemm_pingpong(const CUtensorMap& tmA, const CUtensorMap& tmB, const EpiParams& p,
                                               const CUtensorMap& tmA2, const CUtensorMap& tmB2, const EpiParams& p2,
                                               const Epilogue& epilogue) {
+  constexpr int A_BYTES = UM * GK * 2;  // the A box of a unit; the W box is STAGE_BYTES
   pdl_trigger();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;  // SWIZZLE_128B atoms need 1024-B alignment
-  const uint32_t sA = base, sB = base + GG_STAGES * STAGE_BYTES;
-  const uint32_t bars = base + GG_STAGES * 2 * STAGE_BYTES;  // full[s] @ +8s ; empty[s] @ +8(S+s)
+  uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
+  const uint32_t sA = base, sB = base + GG_STAGES * A_BYTES;
+  const uint32_t sC = sB + GG_STAGES * STAGE_BYTES;                // staging areas (1024-B aligned)
+  // full[s] @ +8s ; empty[s] @ +8(S+s) ; staging-area load of MMA warpgroup g landed @ +16S + 8g
+  const uint32_t bars = sC + 2 * Epilogue::kStageBytes;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tiles1 = p.m_tiles * p.n_tiles;
   const int num_tiles = tiles1 + (DUAL ? p2.m_tiles * p2.n_tiles : 0);
@@ -489,7 +346,7 @@ __device__ __forceinline__ void gemm_pingpong(const CUtensorMap& tmA, const CUte
     const bool second = DUAL && tile >= tiles1;
     if (second) tile -= tiles1;
     const int mt = second ? p2.m_tiles : p.m_tiles;
-    m0 = (tile % mt) * GM;
+    m0 = (tile % mt) * UM;
     n0 = (tile / mt) * GN;
     return second;
   };
@@ -505,6 +362,10 @@ __device__ __forceinline__ void gemm_pingpong(const CUtensorMap& tmA, const CUte
     for (int s = 0; s < GG_STAGES; ++s) {
       mbar_init(bars + 8 * s, 1);
       mbar_init(bars + 8 * (GG_STAGES + s), 4);  // one arrival per warp of the consuming MMA warpgroup
+    }
+    if (Epilogue::kStageBytes > 0) {
+      mbar_init(bars + 16 * GG_STAGES, 1);
+      mbar_init(bars + 16 * GG_STAGES + 8, 1);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -526,43 +387,46 @@ __device__ __forceinline__ void gemm_pingpong(const CUtensorMap& tmA, const CUte
         for (int kb = 0; kb < num_kb; ++kb) {
           mbar_wait(bars + 8 * (GG_STAGES + stage), phase ^ 1);  // slot free (passes immediately on the first lap)
           const uint32_t full = bars + 8 * stage;
-          mbar_expect_tx(full, 2 * STAGE_BYTES);
-          tma_load_2d(ma, full, sA + stage * STAGE_BYTES, kb * GK, m0);
+          mbar_expect_tx(full, A_BYTES + STAGE_BYTES);
+          tma_load_2d(ma, full, sA + stage * A_BYTES, kb * GK, m0);
           tma_load_2d(mb, full, sB + stage * STAGE_BYTES, kb * GK, n0);
           if (++stage == GG_STAGES) { stage = 0; phase ^= 1; }
         }
       }
     }
   } else {
-    // ===================== MMA + epilogue: warpgroup wg takes the CTA's tiles wg, wg + 2, ... =====================
+    // ===================== MMA + epilogue: warpgroup wg takes the CTA's units wg, wg + 2, ... =====================
     setmaxnreg_inc<GG_CONSUMER_REGS>();
     const int wg = (warp >> 2) - 1;
     const int w = warp & 3;
+    PingPongWarp pw{wg, w, lane, base_ptr + (sC - base) + wg * Epilogue::kStageBytes, sC + wg * Epilogue::kStageBytes,
+                    bars + 16 * GG_STAGES + 8 * wg, 0};
     int stage = 0;
     uint32_t phase = 0;
     for (int it = 0; it < my_tiles; ++it) {
       int m0, n0;
       const bool second = tile_of(it, m0, n0);
       const int num_kb = kblocks(second);
-      if ((it & 1) != wg) {  // the other warpgroup's tile: skip its k-blocks in the ring
+      if ((it & 1) != wg) {  // the other warpgroup's unit: skip its k-blocks in the ring
         stage += num_kb;
         while (stage >= GG_STAGES) { stage -= GG_STAGES; phase ^= 1; }
         continue;
       }
-      if (it > 0) named_bar_sync(GG_BAR_TURN + wg, 256);  // the other warpgroup has issued tile it - 1
-      PingPongAcc acc;
+      epilogue.prefetch(second ? p2 : p, m0, n0, pw);  // e.g. the residual tile, while this warpgroup waits and runs
+      if (it > 0) named_bar_sync(GG_BAR_TURN + wg, 256);  // the other warpgroup has issued unit it - 1
+      PingPongAcc<UM> acc;
       int prev = 0;
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(bars + 8 * stage, phase);
-        const uint64_t da0 = gmma_desc(sA + stage * STAGE_BYTES);
-        const uint64_t da1 = gmma_desc(sA + stage * STAGE_BYTES + 64 * 128);
+        const uint64_t da = gmma_desc(sA + stage * A_BYTES);
         const uint64_t db = gmma_desc(sB + stage * STAGE_BYTES);
         wgmma_fence();
 #pragma unroll
         for (int k = 0; k < GK / 16; ++k) {  // +32 B per K = 16 inside the 128-B swizzle row => +2 in the address field
           const uint32_t accumulate = (kb > 0 || k > 0) ? 1u : 0u;
-          wgmma_m64n128k16_ss(acc[0], da0 + 2 * k, db + 2 * k, accumulate);
-          wgmma_m64n128k16_ss(acc[1], da1 + 2 * k, db + 2 * k, accumulate);
+#pragma unroll
+          for (int h = 0; h < UM / 64; ++h)  // row half h: +64 rows = +8 KB = +512 in the address field
+            wgmma_m64n128k16_ss(acc[h], da + 512 * h + 2 * k, db + 2 * k, accumulate);
         }
         wgmma_commit();
         wgmma_wait<1>();  // k-block kb - 1 retired: its slot can be refilled while kb runs
@@ -577,17 +441,20 @@ __device__ __forceinline__ void gemm_pingpong(const CUtensorMap& tmA, const CUte
       wgmma_wait<0>();
       __syncwarp();
       if (lane == 0) mbar_arrive(bars + 8 * (GG_STAGES + prev));
-      epilogue(second ? p2 : p, acc, m0, n0, w, lane);
+      epilogue(second ? p2 : p, acc, m0, n0, pw);
     }
+    // the last unit's bulk stores have read the staging area before the CTA exits (the writes complete with the grid)
+    if (Epilogue::kStageBytes > 0 && w == 0 && lane == 0) tma_store_wait_read();
   }
   __syncthreads();
 }
 
 // GEGLU of the [64 value | 64 gate] tile -> bf16 columns n0/2 + 8j + 2(lane%4) + e, j < 8: value column c and gate
 // column c + 64 of a row are held by the same lane (N % 128 == 0, even ldc and 4-byte aligned C: checked on the host)
-struct GegluEpilogue {
-  __device__ __forceinline__ void operator()(const EpiParams& p, const PingPongAcc& acc, int m0, int n0, int w,
-                                             int lane) const {
+struct GegluEpilogue : RegisterEpilogue {
+  __device__ __forceinline__ void operator()(const EpiParams& p, const PingPongAcc<128>& acc, int m0, int n0,
+                                             const PingPongWarp& pw) const {
+    const int w = pw.w, lane = pw.lane;
     __nv_bfloat16* C = reinterpret_cast<__nv_bfloat16*>(p.C);
     const int oc = n0 / 2 + 2 * (lane & 3);
 #pragma unroll
@@ -613,9 +480,10 @@ struct GegluEpilogue {
 // over L ^ 8, L ^ 4, L ^ 2 pairs registers jj ^ 4, jj ^ 2, jj ^ 1 of one lane, and L ^ 1 pairs quad lanes 1 and 3; float
 // addition is commutative, so every level rounds as there.  Columns >= norm_cols (the value half of k,v) are only
 // converted.  bf16 output, no bias, identity row map, N % 128 == 0 and 8-byte aligned C (checked on the host).
-struct QkNormEpilogue {
-  __device__ __forceinline__ void operator()(const EpiParams& p, const PingPongAcc& acc, int m0, int n0, int w,
-                                             int lane) const {
+struct QkNormEpilogue : RegisterEpilogue {
+  __device__ __forceinline__ void operator()(const EpiParams& p, const PingPongAcc<128>& acc, int m0, int n0,
+                                             const PingPongWarp& pw) const {
+    const int w = pw.w, lane = pw.lane;
     const int t = lane & 3;
     const bool norm = n0 < p.norm_cols;  // tiles are 128-aligned and norm_cols % 128 == 0
     float2 sc[8];
@@ -663,12 +531,16 @@ struct QkNormEpilogue {
   }
 };
 
-// Epilogue 0 of the two-problem launch from the accumulator: fp32 acc + bias (one add, as epi_chunk<0>), no residual,
-// identity row map; float2 stores, scalar ones for ragged N or a C that is not 8-byte aligned.
-struct Fp32BiasEpilogue {
-  __device__ __forceinline__ void operator()(const EpiParams& p, const PingPongAcc& acc, int m0, int n0, int w,
-                                             int lane) const {
-    const int c0 = n0 + 2 * (lane & 3);
+// Epilogue 0 from the accumulator: fp32 (acc + residual) + bias with the row map; float2 accesses, scalar ones for
+// ragged N or a C / residual that is not 8-byte aligned.  SINGLE: the single-problem launches that the TMA unit cannot
+// serve (Fp32StagedEpilogue), with residual and row map; otherwise the two-problem launch, which has neither.  C may
+// alias the residual (in-place x = f(x) + x): every element is read and written by the same thread.
+template <bool SINGLE>
+struct Fp32Epilogue : RegisterEpilogue {
+  template <int H>  // row halves of the unit
+  __device__ __forceinline__ void operator()(const EpiParams& p, const float (&acc)[H][64], int m0, int n0,
+                                             const PingPongWarp& pw) const {
+    const int c0 = n0 + 2 * (pw.lane & 3);
     float2 bv[16];
 #pragma unroll
     for (int j = 0; j < 16; ++j) {
@@ -676,47 +548,123 @@ struct Fp32BiasEpilogue {
       bv[j].x = (p.bias && c < p.N) ? __ldg(p.bias + c) : 0.f;
       bv[j].y = (p.bias && c + 1 < p.N) ? __ldg(p.bias + c + 1) : 0.f;
     }
-    const bool vec = (p.ldc % 2 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 7) == 0);
+    const float* res = SINGLE ? p.residual : nullptr;
+    const bool vec = (p.ldc % 2 == 0) && (((reinterpret_cast<uintptr_t>(p.C) | reinterpret_cast<uintptr_t>(res)) & 7) == 0);
+    const uint32_t seg_len = SINGLE ? (uint32_t)p.seg_len : 0u;
 #pragma unroll
-    for (int r = 0; r < 4; ++r) {
-      const uint32_t m = (uint32_t)m0 + 64 * (r >> 1) + 16 * w + (lane >> 2) + 8 * (r & 1);
+    for (int r = 0; r < 2 * H; ++r) {
+      const uint32_t m = (uint32_t)m0 + 64 * (r >> 1) + 16 * pw.w + (pw.lane >> 2) + 8 * (r & 1);
       if (m >= (uint32_t)p.M) continue;
+      uint32_t orow = m;
+      if (seg_len > 0) { const uint32_t q = m / seg_len; orow = q * (uint32_t)p.seg_stride + (uint32_t)p.seg_off + (m - q * seg_len); }
       const float* a = acc[r >> 1] + 2 * (r & 1);
-      float* crow = reinterpret_cast<float*>(p.C) + (int64_t)m * p.ldc + c0;
+      const int64_t off = (int64_t)orow * p.ldc + c0;
+      float* crow = reinterpret_cast<float*>(p.C) + off;
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
-        const float2 o = make_float2(a[4 * j] + bv[j].x, a[4 * j + 1] + bv[j].y);
+        float2 o = make_float2(a[4 * j], a[4 * j + 1]);
         const int c = c0 + 8 * j;
         if (vec && c + 1 < p.N) {
+          if (res) { const float2 rv = *reinterpret_cast<const float2*>(res + off + 8 * j); o.x += rv.x; o.y += rv.y; }
+          o.x += bv[j].x; o.y += bv[j].y;
           *reinterpret_cast<float2*>(crow + 8 * j) = o;
         } else {
-          if (c < p.N) crow[8 * j] = o.x;
-          if (c + 1 < p.N) crow[8 * j + 1] = o.y;
+          if (c < p.N) crow[8 * j] = (res ? o.x + res[off + 8 * j] : o.x) + bv[j].x;
+          if (c + 1 < p.N) crow[8 * j + 1] = (res ? o.y + res[off + 8 * j + 1] : o.y) + bv[j].y;
         }
       }
     }
   }
 };
 
+// Epilogue 0 of the single-problem launch (64-row units): fp32 (acc + residual) + bias through the TMA unit when the
+// row map is the identity, C is 16-byte aligned with ldc % 4 == 0 and the residual is C or absent (p.tma_epi); every
+// other call takes Fp32Epilogue.  The staging area of an MMA warpgroup is four [64 rows x 32 floats = 128 B]
+// SWIZZLE_128B boxes, the unit's 64 x 128 fp32 output.  Per unit:
+//   prefetch (before the warpgroup's turn): the store thread waits until its previous unit's bulk stores have read the
+//     area and bulk-loads the residual tile (C itself) into it -- the load runs under this unit's main loop;
+//   epilogue: wait for the residual (or, without one, for the store thread's all-clear); each thread adds its
+//     accumulator fragment onto the residual in the boxes, then the bias; fence.proxy.async; warpgroup barrier; the
+//     store thread bulk-stores the boxes (the TMA unit clips rows >= M and columns >= N) and moves on.
+struct Fp32StagedEpilogue {
+  static constexpr int kStageBytes = 64 * 128 * 4;
+  static constexpr int kBoxBytes = 64 * 128;
+  __device__ __forceinline__ void prefetch(const EpiParams& p, int m0, int n0, const PingPongWarp& pw) const {
+    if (!p.tma_epi || pw.w != 0 || pw.lane != 0) return;
+    tma_store_wait_read();
+    if (p.residual) {
+      mbar_expect_tx(pw.bar, kStageBytes);
+#pragma unroll
+      for (int c = 0; c < 4; ++c) tma_load_2d(&p.tmC, pw.bar, pw.stage_s + c * kBoxBytes, n0 + 32 * c, m0);
+    }
+  }
+  __device__ __forceinline__ void operator()(const EpiParams& p, const PingPongAcc<64>& acc, int m0, int n0,
+                                             PingPongWarp& pw) const {
+    if (!p.tma_epi) { Fp32Epilogue<true>{}(p, acc, m0, n0, pw); return; }
+    const int t = pw.lane & 3;
+    float2 bv[16];
+    if (p.bias) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = n0 + 8 * j + 2 * t;
+        bv[j].x = c < p.N ? __ldg(p.bias + c) : 0.f;
+        bv[j].y = c + 1 < p.N ? __ldg(p.bias + c + 1) : 0.f;
+      }
+    }
+    if (p.residual) {
+      mbar_wait(pw.bar, pw.phase);
+      pw.phase ^= 1;
+    } else {
+      named_bar_sync(GG_BAR_EPI + pw.wg, 128);  // the store thread has seen the previous bulk stores read the area
+    }
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int r = 16 * pw.w + (pw.lane >> 2) + 8 * i;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int c = 8 * j + 2 * t;  // thread-owned 8-byte pieces: conflict-free per quarter-warp in the 128-B swizzle
+        float2* dst = reinterpret_cast<float2*>(pw.stage + (c >> 5) * kBoxBytes + r * 128 +
+                                                ((((c & 31) >> 2) ^ (r & 7)) << 4) + (c & 3) * 4);
+        float2 v = make_float2(acc[0][4 * j + 2 * i], acc[0][4 * j + 2 * i + 1]);
+        if (p.residual) { const float2 o = *dst; v.x += o.x; v.y += o.y; }
+        if (p.bias) { v.x += bv[j].x; v.y += bv[j].y; }
+        *dst = v;
+      }
+    }
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes -> visible to the TMA unit
+    named_bar_sync(GG_BAR_EPI + pw.wg, 128);                       // whole unit staged
+    if (pw.w == 0 && pw.lane == 0) {
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        if (n0 + 32 * c < p.N) tma_store_2d(&p.tmC, pw.stage_s + c * kBoxBytes, n0 + 32 * c, m0);
+      tma_store_commit();
+    }
+  }
+};
+constexpr int UNIT_SMEM_TOTAL = pingpong_smem<UNIT_M, Fp32StagedEpilogue>();
+static_assert(UNIT_SMEM_TOTAL <= 227 * 1024, "the 64-row ping-pong launch exceeds the 227 KB of shared memory per block");
+
 __global__ void __launch_bounds__(GG_THREADS, 1) gemm_bf16_geglu_kernel(const __grid_constant__ CUtensorMap tmA,
                                                                         const __grid_constant__ CUtensorMap tmB,
                                                                         const __grid_constant__ EpiParams p) {
-  gemm_pingpong<false>(tmA, tmB, p, tmA, tmB, p, GegluEpilogue{});
+  gemm_pingpong<false, 128>(tmA, tmB, p, tmA, tmB, p, GegluEpilogue{});
 }
 
 // ---------------------------------------------------------------------------------------------------
-// gemm_bf16_kernel<EPI, DUAL>: single-problem instances run the quadrant body, two-problem ones (epilogues 0 and 3) the
-// ping-pong body
+// gemm_bf16_kernel<EPI, DUAL>: the fp32 single-problem instance runs the ping-pong body on 64-row units, the bf16 ones
+// the quadrant body, the two-problem ones (epilogues 0 and 3) the ping-pong body on 128-row tiles
 // ---------------------------------------------------------------------------------------------------
 template <int EPI, bool DUAL>
-__global__ void __launch_bounds__(DUAL ? GG_THREADS : GTHREADS, 1) gemm_bf16_kernel(
+__global__ void __launch_bounds__(DUAL || EPI == 0 ? GG_THREADS : GTHREADS, 1) gemm_bf16_kernel(
     const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ EpiParams p,
     const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
     const __grid_constant__ EpiParams p2) {
   if constexpr (DUAL) {
     static_assert(EPI == 0 || EPI == 3, "two-problem launches have the fp32 (+bias) or the q/k,v epilogue");
-    if constexpr (EPI == 3) gemm_pingpong<true>(tmA, tmB, p, tmA2, tmB2, p2, QkNormEpilogue{});
-    else gemm_pingpong<true>(tmA, tmB, p, tmA2, tmB2, p2, Fp32BiasEpilogue{});
+    if constexpr (EPI == 3) gemm_pingpong<true, 128>(tmA, tmB, p, tmA2, tmB2, p2, QkNormEpilogue{});
+    else gemm_pingpong<true, 128>(tmA, tmB, p, tmA2, tmB2, p2, Fp32Epilogue<false>{});
+  } else if constexpr (EPI == 0) {
+    gemm_pingpong<false, UNIT_M>(tmA, tmB, p, tmA, tmB, p, Fp32StagedEpilogue{});
   } else {
     gemm_quadrant<EPI>(tmA, tmB, p);
   }
@@ -768,11 +716,11 @@ static int get_tensor_map(const void* ptr, int64_t rows, int64_t cols, int64_t l
   return 0;
 }
 
-// fp32 [rows, cols] output, row pitch ld floats; box = [128 rows, 32 floats = 128 B], SWIZZLE_128B (TMA epilogue)
+// fp32 [rows, cols] output, row pitch ld floats; box = [UNIT_M rows, 32 floats = 128 B], SWIZZLE_128B (TMA epilogue)
 static int get_c_map(const void* ptr, int64_t rows, int64_t cols, int64_t ld, CUtensorMap* out) {
   static std::unordered_map<MapKey, CUtensorMap, MapKeyHash> cache;
   static std::mutex mu;
-  const MapKey key{ptr, rows, cols, ld, -32};
+  const MapKey key{ptr, rows, cols, ld, UNIT_M};
   std::lock_guard<std::mutex> lk(mu);
   auto it = cache.find(key);
   if (it != cache.end()) { *out = it->second; return 0; }
@@ -780,7 +728,7 @@ static int get_c_map(const void* ptr, int64_t rows, int64_t cols, int64_t ld, CU
   PHK_REQUIRE(fn, PHK_E_UNSUPPORTED, "cuTensorMapEncodeTiled not available from the driver");
   const cuuint64_t gdim[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
   const cuuint64_t gstride[1] = {(cuuint64_t)ld * 4};
-  const cuuint32_t box[2] = {32, (cuuint32_t)GM};
+  const cuuint32_t box[2] = {32, (cuuint32_t)UNIT_M};
   const cuuint32_t estr[2] = {1, 1};
   CUtensorMap m;
   const CUresult r = fn(&m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(ptr), gdim, gstride, box, estr,
@@ -806,15 +754,17 @@ static int maybe_tma_epilogue(EpiParams& p, int epilogue) {
 
 template <int EPI>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, const EpiParams& p, cudaStream_t st) {
+  constexpr int threads = EPI == 0 ? GG_THREADS : GTHREADS;
+  constexpr int smem = EPI == 0 ? UNIT_SMEM_TOTAL : SMEM_TOTAL;
   static unsigned long long configured_mask = 0;
   const bool configured = device_configured(&configured_mask);
   if (!configured) {
-    PHK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<EPI, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TOTAL));
+    PHK_CUDA(cudaFuncSetAttribute(gemm_bf16_kernel<EPI, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     mark_configured(&configured_mask);
   }
   const int tiles = p.m_tiles * p.n_tiles;
   const int grid = tiles < kNumSMs ? tiles : kNumSMs;
-  PHK_CUDA(launch_pdl(gemm_bf16_kernel<EPI, false>, dim3(grid), dim3(GTHREADS), (size_t)(SMEM_TOTAL), st, ta, tb, p, ta, tb, p));
+  PHK_CUDA(launch_pdl(gemm_bf16_kernel<EPI, false>, dim3(grid), dim3(threads), (size_t)smem, st, ta, tb, p, ta, tb, p));
   PHK_LAUNCH_CHECK();
   return 0;
 }
@@ -867,11 +817,12 @@ extern "C" int phk_gemm_bf16(const void* A, int64_t lda, const void* W, int64_t 
               PHK_E_ARG, "phk_gemm_bf16: GEGLU epilogue needs N % 128 == 0, an even ldc and no bias/residual");
   PHK_REQUIRE(M < (1LL << 31) - GM, PHK_E_UNSUPPORTED, "phk_gemm_bf16: M too large");
   if (M == 0) return 0;
+  const int um = epilogue == 0 ? UNIT_M : GM;  // rows of a work unit: the fp32 epilogue runs on 64-row units
   CUtensorMap ta, tb;
-  PHK_TRY(get_tensor_map(A, M, K, lda, GM, &ta));
+  PHK_TRY(get_tensor_map(A, M, K, lda, um, &ta));
   cudaStream_t st = to_stream(s);
   PHK_TRY(get_tensor_map(W, N, K, ldw, GN, &tb));
-  EpiParams p{C, ldc, M, N, K, bias, residual, seg_len, seg_stride, seg_off, (int)((M + GM - 1) / GM), (N + GN - 1) / GN};
+  EpiParams p{C, ldc, M, N, K, bias, residual, seg_len, seg_stride, seg_off, (int)((M + um - 1) / um), (N + GN - 1) / GN};
   PHK_REQUIRE((int64_t)p.m_tiles * p.n_tiles < (1LL << 31), PHK_E_UNSUPPORTED, "phk_gemm_bf16: too many tiles");
   PHK_TRY(maybe_tma_epilogue(p, epilogue));
   if (epilogue == 2) return launch_gemm_geglu(ta, tb, p, st);

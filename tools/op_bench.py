@@ -51,8 +51,11 @@ xn_h, raw_h = torch.empty(R, D, dtype=bf, device=dev), torch.empty(R, D, dtype=b
 timeit("layernorm -> bf16 (+raw)", lambda: L.check(lib.phk_layernorm(L.ptr(x), L.ptr(g), L.ptr(b), L.ptr(xn_h), L.ptr(raw_h), R, D, 1, 0, 0, 0, sp())),
        R * D * 8, "TB/s")
 
-for (M, N, K, epi, name) in [(4608, 512, 512, 0, "gemm q/out-proj (+res)"), (4608, 1024, 512, 0, "gemm kv-proj"),
+# out-proj and FF2 (+ the fp32 residual, in place) also at 2304 rows: the first MaskGit layer of a CFG pair and the
+# training step's products
+for (M, N, K, epi, name) in [(4608, 512, 512, 0, "gemm out-proj (+res)"), (4608, 1024, 512, 0, "gemm kv-proj"),
                              (4608, 2816, 512, 2, "gemm FF1 + GEGLU"), (4608, 512, 1408, 0, "gemm FF2 (+res)"),
+                             (2304, 512, 512, 0, "gemm out-proj (+res)"), (2304, 512, 1408, 0, "gemm FF2 (+res)"),
                              (4096, 512, 6144, 0, "gemm patch-embed"), (2304, 65536, 512, 0, "gemm logits head (unfused)")]:
     a = torch.randn(M, K, device=dev).to(bf)
     w = torch.randn(N, K, device=dev).to(bf)
