@@ -658,6 +658,7 @@ int phk_debug_step_graph(int32_t on);
  *   ids_in  (b,n) int64   network input: ids with the mask id at the masked positions (MaskGit) or with the sampled
  *                         predictions at the masked positions (critic)
  *   targets (b,n) int64 + token_mask (b,n) uint8   MaskGit: loss = mean over masked rows of CE(logits, target)
+ *                                                  (an all-false mask gives loss 0 and zero gradients, not NaN)
  *   labels  (b,n) float 0/1                        critic : loss = mean over all rows of BCE_with_logits(score, label)
  *   context (b,L,dim_context) fp32 raw text embeddings or NULL; text_mask (b,L) uint8; video_mask (b,n) uint8 or NULL
  *   grads   a table of the SAME layout as `m` whose float pointers address ZERO-FILLED gradient buffers of the

@@ -315,6 +315,10 @@ inline unsigned ew_grid_fwd(int64_t total) {
   const int64_t b = (total + 255) / 256;
   return (unsigned)(b < 1 ? 1 : (b > kNumSMs * 16 ? kNumSMs * 16 : b));
 }
+inline unsigned ew_grid(int64_t total) {
+  const int64_t b = (total + 255) / 256;
+  return (unsigned)(b < 1 ? 1 : (b > kNumSMs * 16 ? kNumSMs * 16 : b));
+}
 
 // out[c] += sum_r x[r, c]   (bias gradients); grid (ceil(C/256), row chunks), atomics across chunks
 __global__ void __launch_bounds__(256) colsum_kernel(const float* __restrict__ x, int64_t rows, int cols, int64_t ld,
@@ -589,6 +593,23 @@ __global__ void geglu_bwd_kernel(const float* __restrict__ h, const float* __res
     dh[r * 2 * inner + j] = d * gate * cdf;
     dh[r * 2 * inner + inner + j] = d * val * (cdf + gate * pdf);
   }
+}
+
+// g [R, inner] = GEGLU(h [R, 2 inner]) followed by the FF dropout site d (d.p == 0: the site is off, phk_geglu)
+int geglu_dropout_fwd(const float* h, float* g, int64_t R, int inner, const DropSite& d, phk_stream_t s) {
+  if (d.p > 0.f) {
+    PHK_KERNEL_LAUNCH(geglu_dropout_kernel, dim3(ew_grid_fwd(R * inner)), dim3(256), (size_t)(0), to_stream(s), h, g, R, inner, d);
+    PHK_LAUNCH_CHECK();
+    return 0;
+  }
+  return phk_geglu(h, g, R, inner, s);
+}
+
+// dh [R, 2 inner] = d/dh of GEGLU + dropout site d, from dg [R, inner] (dh is written, not added)
+int geglu_backward(const float* h, const float* dg, float* dh, int64_t R, int inner, const DropSite& d, cudaStream_t st) {
+  PHK_KERNEL_LAUNCH(geglu_bwd_kernel, dim3(ew_grid(R * inner)), dim3(256), (size_t)(0), st, h, dg, dh, R, inner, d);
+  PHK_LAUNCH_CHECK();
+  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -1145,6 +1166,26 @@ __global__ void __launch_bounds__(128) peg_bwd_kernel(const float* __restrict__ 
   }
 }
 
+// PEG backward over R = B T H W positions (pad_t0 = 2 causal, 1 otherwise): db += colsum(dy), dw (dsconv.weight
+// [D, 27]) += .., dx = dy + conv^T(dy) (written).  D > 1024 is refused before anything is written.
+int peg_backward(const float* x, const float* w, const float* dy, float* dx, float* dw, float* db, int64_t R, int T,
+                 int H, int W, int D, int pad_t0, cudaStream_t st) {
+  PHK_REQUIRE(D <= 128 * PEG_DW_MAXJ, PHK_E_UNSUPPORTED, "train: PEG backward needs dim <= 1024");
+  PHK_TRY(colsum(dy, R, D, D, db, st));
+  if (t_det.p) {  // deterministic mode: one [D, 27] slot per chunk of positions, added in order
+    PHK_REQUIRE(peg_det_floats(D) <= t_det.floats, PHK_E_WORKSPACE, "train: deterministic reduction scratch too small");
+    PHK_KERNEL_LAUNCH(peg_bwd_dw_fixed_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, x, dy, R, T, H, W, D, pad_t0, t_det.p);
+    PHK_LAUNCH_CHECK();
+    PHK_TRY(add_slots(t_det.p, PEG_DW_CHUNKS, 27 * (int64_t)D, dw, st));
+  } else {
+    PHK_KERNEL_LAUNCH(peg_bwd_dw_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, x, dy, dw, R, T, H, W, D, pad_t0);
+    PHK_LAUNCH_CHECK();
+  }
+  PHK_KERNEL_LAUNCH(peg_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, x, w, dy, dx, T, H, W, D, pad_t0);
+  PHK_LAUNCH_CHECK();
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // Embedding backward (phenaki_pytorch.py:194-199): x = tok[id] + pos[p]; the gradient-shrink trick lets only the
 // alpha branch carry gradient.  dtok[id] += a * dx ; dpos[p] += a * dx
@@ -1231,6 +1272,21 @@ __global__ void embed_pos_fixed_kernel(const float* __restrict__ dx, float* __re
   }
 }
 
+// dtok[clamp(ids[r])] += alpha dx[r] ; dpos[r % n] += alpha dx[r] over R rows (ids clamped to [0, vocab_rows))
+int embed_backward(const int64_t* ids, const float* dx, float* dtok, float* dpos, int64_t R, int n, int D, float alpha,
+                   int vocab_rows, cudaStream_t st) {
+  if (t_det.p) {
+    PHK_KERNEL_LAUNCH(embed_tok_fixed_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, ids, dx, dtok, R, D, alpha, vocab_rows);
+    PHK_LAUNCH_CHECK();
+    PHK_KERNEL_LAUNCH(embed_pos_fixed_kernel, dim3(ew_grid((int64_t)n * D)), dim3(256), (size_t)(0), st, dx, dpos, R, n, D, alpha);
+    PHK_LAUNCH_CHECK();
+    return 0;
+  }
+  PHK_KERNEL_LAUNCH(embed_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, ids, dx, dtok, dpos, n, D, alpha, vocab_rows);
+  PHK_LAUNCH_CHECK();
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------------------------------
 // ContinuousPositionBias backward (attention.py:257-275): bias[h,i,j] = table[u(i,j), h], table = MLP(in[u]).
 // The MLP runs over the U distinct coordinate deltas; its backward is three dgrad/wgrad pairs on [U, .] matrices.
@@ -1296,11 +1352,6 @@ __global__ void cpb_dtable_fixed_kernel(const float* __restrict__ dbias, float* 
         }
     dtable[idx] = a;
   }
-}
-
-inline unsigned ew_grid(int64_t total) {
-  const int64_t b = (total + 255) / 256;
-  return (unsigned)(b < 1 ? 1 : (b > kNumSMs * 16 ? kNumSMs * 16 : b));
 }
 
 int64_t cpb_bwd_scratch_floats(const phk_cpb_t& c, int d0, int d1, int d2) {
@@ -1433,6 +1484,32 @@ __global__ void __launch_bounds__(1024) loss_reduce_kernel(const float* __restri
   for (int64_t r = threadIdx.x; r < rows; r += blockDim.x) a += row_loss[r];
   a = block_sum(a, red);
   if (threadIdx.x == 0) *loss = a;
+}
+
+// MaskGit head loss over R rows of V logits: *count = max(#masked rows, 1), then per row the CE loss / count and the
+// dlogits IN PLACE (zeros on unmasked rows)
+int ce_rows(float* logits, const int64_t* targets, const uint8_t* mask, float* count, float scale, float* row_loss,
+            int64_t R, int V, cudaStream_t st) {
+  PHK_KERNEL_LAUNCH(mask_count_kernel, dim3(1), dim3(256), (size_t)(0), st, mask, R, count);
+  PHK_LAUNCH_CHECK();
+  PHK_KERNEL_LAUNCH(ce_rows_kernel, dim3((unsigned)R), dim3(256), (size_t)(0), st, logits, targets, mask, (const float*)count, scale, row_loss, V);
+  PHK_LAUNCH_CHECK();
+  return 0;
+}
+
+// critic head over R rows: score = emb . w + b, per row the BCE-with-logits loss / R and dscore
+int bce_rows(const float* emb, const float* w, const float* b, const float* labels, float scale, float* row_loss,
+             float* dscore, int64_t R, int D, cudaStream_t st) {
+  PHK_KERNEL_LAUNCH(bce_rows_kernel, dim3((unsigned)((R + 7) / 8)), dim3(256), (size_t)(0), st, emb, w, b, labels, scale, row_loss, dscore, R, D);
+  PHK_LAUNCH_CHECK();
+  return 0;
+}
+
+// *loss = sum of the R row losses (one CTA: a fixed order)
+int loss_reduce(const float* row_loss, int64_t R, float* loss, cudaStream_t st) {
+  PHK_KERNEL_LAUNCH(loss_reduce_kernel, dim3(1), dim3(1024), (size_t)(0), st, row_loss, R, loss);
+  PHK_LAUNCH_CHECK();
+  return 0;
 }
 
 // demb[r, :] = dscore[r] * w
@@ -1713,12 +1790,7 @@ int layer_forward(const LayerCall& c, int l, const float* x0, LayerSave& Sv, flo
   // feed forward (attention.py:45-53)
   PHK_TRY(phk_layernorm(Sv.x3, Ly.ff.ln_g, Ly.ff.ln_b, Sv.xn3, nullptr, R, D, 0, 0, 0, 0, s));
   PHK_TRY(linear_fwd(prec, tc, Sv.xn3, Ly.ff.w1, Sv.h, R, 2 * inner, D, nullptr, nullptr, s));
-  if (d_ff.p > 0.f) {
-    PHK_KERNEL_LAUNCH(geglu_dropout_kernel, dim3(ew_grid_fwd(R * inner)), dim3(256), (size_t)(0), st, Sv.h, Sv.g, R, inner, d_ff);
-    PHK_LAUNCH_CHECK();
-  } else {
-    PHK_TRY(phk_geglu(Sv.h, Sv.g, R, inner, s));
-  }
+  PHK_TRY(geglu_dropout_fwd(Sv.h, Sv.g, R, inner, d_ff, s));
   return linear_fwd(prec, tc, Sv.g, Ly.ff.w2, *xout, R, D, inner, nullptr, Sv.x3, s);  // x4 = x3 + g W2^T
 }
 
@@ -1741,8 +1813,7 @@ int layer_backward(const LayerCall& c, int l, const LayerSave& Sv, float** dx, f
   // feed forward: x4 = x3 + geglu(LN(x3) W1^T) W2^T
   PHK_TRY(dgrad_p(prec, tc, d, Ly.ff.w2, G.dg, R, D, inner, 0, s));
   PHK_TRY(wgrad_p(prec, tc, d, Sv.g, (float*)Gy.ff.w2, R, D, inner, s));
-  PHK_KERNEL_LAUNCH(geglu_bwd_kernel, dim3(ew_grid(R * inner)), dim3(256), (size_t)(0), st, Sv.h, G.dg, G.dh, R, inner, d_ff);
-  PHK_LAUNCH_CHECK();
+  PHK_TRY(geglu_backward(Sv.h, G.dg, G.dh, R, inner, d_ff, st));
   PHK_TRY(wgrad_p(prec, tc, G.dh, Sv.xn3, (float*)Gy.ff.w1, R, 2 * inner, D, s));
   PHK_TRY(dgrad_p(prec, tc, G.dh, Ly.ff.w1, G.dtmp, R, 2 * inner, D, 0, s));
   PHK_TRY(ln_backward(Sv.x3, Ly.ff.ln_g, G.dtmp, d, 1, (float*)Gy.ff.ln_g, (float*)Gy.ff.ln_b, G.stats, R, D, st));
@@ -1782,19 +1853,8 @@ int layer_backward(const LayerCall& c, int l, const LayerSave& Sv, float** dx, f
   }
   if (!Ly.has_peg) return 0;  // x1 = x0
   // PEG: x1 = x0 + conv(x0) + b
-  PHK_TRY(colsum(d, R, D, D, (float*)Gy.peg.b, st));
-  PHK_REQUIRE(D <= 128 * PEG_DW_MAXJ, PHK_E_UNSUPPORTED, "train: PEG backward needs dim <= 1024");
-  if (t_det.p) {  // deterministic mode: one [D, 27] slot per chunk of positions, added in order
-    PHK_REQUIRE(peg_det_floats(D) <= t_det.floats, PHK_E_WORKSPACE, "train: deterministic reduction scratch too small");
-    PHK_KERNEL_LAUNCH(peg_bwd_dw_fixed_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, Sv.x0, (const float*)d, R, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal ? 2 : 1, t_det.p);
-    PHK_LAUNCH_CHECK();
-    PHK_TRY(add_slots(t_det.p, PEG_DW_CHUNKS, 27 * (int64_t)D, (float*)Gy.peg.w, st));
-  } else {
-    PHK_KERNEL_LAUNCH(peg_bwd_dw_kernel, dim3(27, PEG_DW_CHUNKS), dim3(128), (size_t)(0), st, Sv.x0, d, (float*)Gy.peg.w, R, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal ? 2 : 1);
-    PHK_LAUNCH_CHECK();
-  }
-  PHK_KERNEL_LAUNCH(peg_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, Sv.x0, Ly.peg.w, d, *dx_alt, c.pegT, c.pegH, c.pegW, D, Ly.peg.causal ? 2 : 1);
-  PHK_LAUNCH_CHECK();
+  PHK_TRY(peg_backward(Sv.x0, Ly.peg.w, d, *dx_alt, (float*)Gy.peg.w, (float*)Gy.peg.b, R, c.pegT, c.pegH, c.pegW, D,
+                       Ly.peg.causal ? 2 : 1, st));
   *dx = *dx_alt;
   *dx_alt = d;
   return 0;
@@ -1921,16 +1981,7 @@ int step_backward(Step& S, float* d_context, void** prog, int nprog) {
   }
   // ---------------------------------------------------------------- embeddings, position-bias MLP
   const float alpha = m->is_critic ? 1.0f : m->shrink_alpha;
-  if (t_det.p) {
-    PHK_KERNEL_LAUNCH(embed_tok_fixed_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, S.ids, (const float*)dx, (float*)grads->token_emb, R, D, alpha, m->num_tokens + 1);
-    PHK_LAUNCH_CHECK();
-    PHK_KERNEL_LAUNCH(embed_pos_fixed_kernel, dim3(ew_grid((int64_t)n * D)), dim3(256), (size_t)(0), st, (const float*)dx, (float*)grads->pos_emb, R, n, D, alpha);
-    PHK_LAUNCH_CHECK();
-  } else {
-    PHK_KERNEL_LAUNCH(embed_bwd_kernel, dim3((unsigned)R), dim3(128), (size_t)(0), st, S.ids, dx, (float*)grads->token_emb, (float*)grads->pos_emb, n, D,
-                                                 alpha, m->num_tokens + 1);
-    PHK_LAUNCH_CHECK();
-  }
+  PHK_TRY(embed_backward(S.ids, dx, (float*)grads->token_emb, (float*)grads->pos_emb, R, n, D, alpha, m->num_tokens + 1, st));
   if (m->has_bias) {
     float* csc = ar.f(cpb_bwd_scratch_floats(m->pos_bias, pt, ph, pw));
     PHK_REQUIRE(csc, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (position-bias backward)");
@@ -2139,8 +2190,7 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
   if (bce) {
     float* dscore = ar.f(R);
     PHK_REQUIRE(dscore, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small");
-    PHK_KERNEL_LAUNCH(bce_rows_kernel, dim3((unsigned)((R + 7) / 8)), dim3(256), (size_t)(0), st, S.emb, m->head_w, m->head_b, labels, loss_scale, row_loss, dscore, R, D);
-    PHK_LAUNCH_CHECK();
+    PHK_TRY(bce_rows(S.emb, m->head_w, m->head_b, labels, loss_scale, row_loss, dscore, R, D, st));
     PHK_TRY(wgrad(dscore, S.emb, (float*)grads->head_w, R, 1, D, st));  // [1, dim]: not worth a tensor-core launch
     PHK_TRY(colsum(dscore, R, 1, 1, (float*)grads->head_b, st));
     PHK_KERNEL_LAUNCH(outer_kernel, dim3(ew_grid(R * D)), dim3(256), (size_t)(0), st, dscore, m->head_w, S.dtmp, R, D);
@@ -2155,16 +2205,12 @@ extern "C" int phk_maskgit_train_step(const phk_maskgit_t* m, const phk_maskgit_
       PHK_REQUIRE(dl, PHK_E_WORKSPACE, "maskgit_train_step: workspace too small (dlogits)");
       PHK_CUDA(cudaMemcpyAsync(dl, logits, R * (int64_t)V * 4, cudaMemcpyDeviceToDevice, st));
     }
-    PHK_KERNEL_LAUNCH(mask_count_kernel, dim3(1), dim3(256), (size_t)(0), st, token_mask, R, cnt);
-    PHK_LAUNCH_CHECK();
-    PHK_KERNEL_LAUNCH(ce_rows_kernel, dim3((unsigned)R), dim3(256), (size_t)(0), st, dl, targets, token_mask, cnt, loss_scale, row_loss, V);
-    PHK_LAUNCH_CHECK();
+    PHK_TRY(ce_rows(dl, targets, token_mask, cnt, loss_scale, row_loss, R, V, st));
     PHK_TRY(wgrad_p(prec, S.tc, dl, S.emb, (float*)grads->head_w, R, V, D, s));
     PHK_TRY(colsum(dl, R, V, V, (float*)grads->head_b, st));
     PHK_TRY(dgrad_p(prec, S.tc, dl, m->head_w, S.dtmp, R, V, D, 0, s));
   }
-  PHK_KERNEL_LAUNCH(loss_reduce_kernel, dim3(1), dim3(1024), (size_t)(0), st, row_loss, R, loss_out);
-  PHK_LAUNCH_CHECK();
+  PHK_TRY(loss_reduce(row_loss, R, loss_out, st));
 
   // ---------------------------------------------------------------- backward through the transformer
   // (d_context: the context_norm backward each cross-attention layer runs for its gamma gradient also accumulates dx)

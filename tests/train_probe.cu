@@ -51,3 +51,68 @@ extern "C" int probe_attn_bwd_layout(int32_t b, int32_t H, int32_t n, int32_t m,
 extern "C" int probe_colsum(const float* x, int64_t rows, int32_t cols, int64_t ld, float* out, phk_stream_t s) {
   return phk::colsum(x, rows, cols, ld, out, phk::to_stream(s));
 }
+
+// ---- the rest of the backward: LayerNorm, GEGLU, PEG, embeddings, position-bias MLP, head losses ----
+
+// deterministic mode's reduction scratch (phk::t_det) for the calls that follow; p == NULL: the default path
+extern "C" int probe_set_det_scratch(float* p, int64_t floats) {
+  phk::t_det = phk::DetScratch{p, floats};
+  return 0;
+}
+
+// stats: float2 [rows] (mean, rstd), written
+extern "C" int probe_ln_backward(const float* x, const float* g, const float* dy, float* dx, int32_t accumulate,
+                                 float* dgamma, float* dbeta, float* stats, int64_t rows, int32_t dim, phk_stream_t s) {
+  return phk::ln_backward(x, g, dy, dx, accumulate, dgamma, dbeta, reinterpret_cast<float2*>(stats), rows, dim,
+                          phk::to_stream(s));
+}
+
+// the dropout site {p, scale, key (k0, k1), first counter base}; p == 0: off
+extern "C" int probe_geglu_dropout_fwd(const float* h, float* g, int64_t R, int32_t inner, float p, float scale,
+                                       uint32_t k0, uint32_t k1, uint64_t base, phk_stream_t s) {
+  return phk::geglu_dropout_fwd(h, g, R, inner, phk::DropSite{p, scale, k0, k1, base}, s);
+}
+
+extern "C" int probe_geglu_backward(const float* h, const float* dg, float* dh, int64_t R, int32_t inner, float p,
+                                    float scale, uint32_t k0, uint32_t k1, uint64_t base, phk_stream_t s) {
+  return phk::geglu_backward(h, dg, dh, R, inner, phk::DropSite{p, scale, k0, k1, base}, phk::to_stream(s));
+}
+
+extern "C" int probe_peg_backward(const float* x, const float* w, const float* dy, float* dx, float* dw, float* db,
+                                  int64_t R, int32_t T, int32_t H, int32_t W, int32_t D, int32_t pad_t0,
+                                  phk_stream_t s) {
+  return phk::peg_backward(x, w, dy, dx, dw, db, R, T, H, W, D, pad_t0, phk::to_stream(s));
+}
+
+extern "C" int probe_embed_backward(const int64_t* ids, const float* dx, float* dtok, float* dpos, int64_t R, int32_t n,
+                                    int32_t D, float alpha, int32_t vocab_rows, phk_stream_t s) {
+  return phk::embed_backward(ids, dx, dtok, dpos, R, n, D, alpha, vocab_rows, phk::to_stream(s));
+}
+
+extern "C" int probe_cpb_backward(const phk_cpb_t* c, const phk_cpb_t* G, const float* dbias, int32_t d0, int32_t d1,
+                                  int32_t d2, float* scratch, phk_stream_t s) {
+  return phk::cpb_backward(*c, *G, dbias, d0, d1, d2, scratch, phk::to_stream(s));
+}
+
+// out[0]: cpb_bwd_scratch_floats, out[1]: ln_det_floats(rows, dim), out[2]: peg_det_floats(dim)
+extern "C" int probe_scratch_floats(const phk_cpb_t* c, int32_t d0, int32_t d1, int32_t d2, int64_t rows, int32_t dim,
+                                    int64_t* out) {
+  out[0] = phk::cpb_bwd_scratch_floats(*c, d0, d1, d2);
+  out[1] = phk::ln_det_floats(rows, dim);
+  out[2] = phk::peg_det_floats(dim);
+  return 0;
+}
+
+extern "C" int probe_ce_rows(float* logits, const int64_t* targets, const uint8_t* mask, float* count, float scale,
+                             float* row_loss, int64_t R, int32_t V, phk_stream_t s) {
+  return phk::ce_rows(logits, targets, mask, count, scale, row_loss, R, V, phk::to_stream(s));
+}
+
+extern "C" int probe_bce_rows(const float* emb, const float* w, const float* b, const float* labels, float scale,
+                              float* row_loss, float* dscore, int64_t R, int32_t D, phk_stream_t s) {
+  return phk::bce_rows(emb, w, b, labels, scale, row_loss, dscore, R, D, phk::to_stream(s));
+}
+
+extern "C" int probe_loss_reduce(const float* row_loss, int64_t R, float* loss, phk_stream_t s) {
+  return phk::loss_reduce(row_loss, R, loss, phk::to_stream(s));
+}

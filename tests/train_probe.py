@@ -1,6 +1,8 @@
 """TEST INFRASTRUCTURE: the probe library of tests/train_probe.cu -- csrc/train.cu unchanged plus extern "C" wrappers
-around its internal product functions (sgemm_batched, linear_fwd / dgrad_p / wgrad_p, attention_backward, colsum), so
-that tests can drive each product on its own.  libphk.so does not export them.
+around its internal functions (the products sgemm_batched, linear_fwd / dgrad_p / wgrad_p, attention_backward, colsum;
+the rest of the backward ln_backward, geglu_dropout_fwd / geglu_backward, peg_backward, embed_backward, cpb_backward,
+ce_rows / bce_rows / loss_reduce; the deterministic-mode scratch t_det), so that tests can drive each one on its own.
+libphk.so does not export them.
 
 On the GPU the probe is compiled with the product's nvcc flags and linked with the other csrc objects that
 phenaki_pytorch_b200.build leaves behind; on the CPU executor the same wrappers are appended to the emulated train.cu."""
@@ -19,6 +21,7 @@ EMU_LIB = os.path.join(emu_runtime.EMU_DIR, "_build", "libphk_train_probe_emu.so
 INCLUDE_TRAIN = '#include "../phenaki_pytorch_b200/csrc/train.cu"'
 
 i64, i32, vp = C.c_int64, C.c_int32, C.c_void_p
+f32, u32, u64 = C.c_float, C.c_uint32, C.c_uint64
 PROTOTYPES = {
     "probe_sgemm_batched": [vp, i64, i64, vp, i64, i64, vp, i64, i64, i64, i64, i32, i32, i32, i64, i64, i64, i64, i64,
                             i64, i32, i32, vp],
@@ -27,6 +30,17 @@ PROTOTYPES = {
                                  i32, i32, i32, vp, i32, vp],
     "probe_attn_bwd_layout": [i32, i32, i32, i32, i32, i32, C.POINTER(i64)],
     "probe_colsum": [vp, i64, i32, i64, vp, vp],
+    "probe_set_det_scratch": [vp, i64],
+    "probe_ln_backward": [vp, vp, vp, vp, i32, vp, vp, vp, i64, i32, vp],
+    "probe_geglu_dropout_fwd": [vp, vp, i64, i32, f32, f32, u32, u32, u64, vp],
+    "probe_geglu_backward": [vp, vp, vp, i64, i32, f32, f32, u32, u32, u64, vp],
+    "probe_peg_backward": [vp, vp, vp, vp, vp, vp, i64, i32, i32, i32, i32, i32, vp],
+    "probe_embed_backward": [vp, vp, vp, vp, i64, i32, i32, f32, i32, vp],
+    "probe_cpb_backward": [C.POINTER(L.CpbT), C.POINTER(L.CpbT), vp, i32, i32, i32, vp, vp],
+    "probe_scratch_floats": [C.POINTER(L.CpbT), i32, i32, i32, i64, i32, C.POINTER(i64)],
+    "probe_ce_rows": [vp, vp, vp, vp, f32, vp, i64, i32, vp],
+    "probe_bce_rows": [vp, vp, vp, vp, f32, vp, vp, i64, i32, vp],
+    "probe_loss_reduce": [vp, i64, vp, vp],
 }
 
 
